@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the v2e hot path on B200 (see DESIGN.md "Measurement").
+"""bench.py -- headline benchmark of the v2e hot path on H100 (see DESIGN.md "Measurement").
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|reference_cuda]
-                    [--workload headline|s|c3|c5]
+                    [--workload headline|s|c3|c5] [--dump-outputs DIR]
 
 Headline workload (BASELINE.json: "Mevents/s + interpolated-frames/s ... 1280x720 at 10x slowdown"):
 one clip of 9 source frames (1280x720 uint8, smooth random texture translating 10 px per source
@@ -22,6 +22,8 @@ Secondary lines in the same JSON object (BASELINE.json configs, SURVEY.md 8d):
   config5 (--workload c5) ONE 1280x720 clip over the N ranks: SloMo sharded over frame pairs, all-to-all of row
                           bands, centre-surround pixel model sharded over pixel rows (halo exchange per Euler chunk)
 `--impl reference` times the UNMODIFIED reference (oracle/_ref: the vendored v2ecore package) on the host cores.
+`--dump-outputs DIR` writes what the headline's last timed step returned (rank 0) as DIR/*.npy, so that two builds
+can be compared output for output: the inputs (seeded clip, seeded device RNG) are the same for the same arguments.
 One JSON line on stdout (rank 0).
 """
 import argparse
@@ -56,14 +58,26 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"],
                     bf16_tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16 / BF16 -- not reached figures
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
-def ncu_traffic():
-    """DRAM bytes per launch from the committed ncu captures (profiles/r2_traffic.json, written by hand from
-    `ncu --set full` of the same kernels; bench.py never runs under a profiler)."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    return json.load(open(p)) if os.path.exists(p) else {}
+def dump_outputs(dirname, ev, offs, t):
+    """The arrays V2EPipeline.run returned in the last timed step: event rows [t, x, y, p] in canonical (t, y, x, p)
+    order (rows of one timestamp come in no fixed order), a fixed seeded sample of 3.5 M rows (56 MB) when there are
+    more; the total row count; per-frame row offsets; frame times."""
+    os.makedirs(dirname, exist_ok=True)
+    host = lambda a: a.cpu().numpy() if hasattr(a, "cpu") else np.asarray(a)
+    rows = host(ev).astype(np.float32)
+    rows = rows[np.lexsort((rows[:, 3], rows[:, 1], rows[:, 2], rows[:, 0]))]
+    n = len(rows)
+    cap = 3_500_000                         # the dump stays below 64 MB
+    if n > cap:
+        rows = rows[np.sort(np.random.default_rng(0).choice(n, cap, replace=False))]
+    np.save(os.path.join(dirname, "events.npy"), rows)
+    np.save(os.path.join(dirname, "event_count.npy"), np.array([n], np.float64))
+    np.save(os.path.join(dirname, "frame_offsets.npy"), host(offs).astype(np.float64))
+    np.save(os.path.join(dirname, "frame_times_s.npy"), np.asarray(t, np.float64))
 
 
 def source_clip(H, W, n_src, seed=0, px_per_frame=10, up=16, lo=40.0, hi=215.0):
@@ -148,7 +162,7 @@ def slomo_weights():
 
 
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md "clocks line")."""
+    """nvidia-smi sampling during the timed region: median SM clock, peak power, active throttle reasons."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -286,6 +300,7 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
     ap.add_argument("--no-cpu", action="store_true", help="development: skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the headline's last timed step's outputs as DIR/*.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -373,6 +388,7 @@ def main():
                 ev, offs, t, nf = pipe.run(src_dev, clip_seconds, t_offset=t0, return_device=True)
                 if world > 1:
                     gather_events(ev)
+            pipe.last_step = (ev, offs, t)
             return ev.shape[0]
         for _ in range(warmup):
             one()
@@ -480,6 +496,8 @@ def main():
     ms_dev, ev_dev, pipe = run_clips(src_host, src_dev, CLI_DEFAULTS, U, args.batch, n_interp, 48 * 1024 * 1024,
                                      args.steps, args.warmup, False, clip_s, 1234 + rank)
     clocks = sampler.stop() if rank == 0 else None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, *pipe.last_step)
     _a, _b = ctypes.c_longlong(0), ctypes.c_longlong(0)
     pipe.emulator._lib.v2e_emu_fused_stats(pipe.emulator._h, ctypes.byref(_a), ctypes.byref(_b))
     _c, _d = ctypes.c_int(0), ctypes.c_int(0)
@@ -495,7 +513,6 @@ def main():
     prof = {}
     replay = None
     if rank == 0 and not args.no_profile:
-        traffic = ncu_traffic()
         eng = pipe.slomo._engine
         em = pipe.emulator
         _lib.check(eng.lib.v2e_slomo_profile(eng._h, 1))
@@ -520,7 +537,6 @@ def main():
                                "frac": tf / pk["bf16_tflops_sustained"]})
         big = max(range(23), key=lambda i: ms23[i])
         achieved = conv_fl.value / (conv_ms.value * 1e-3) / 1e12
-        tr_conv = traffic.get("conv_all_layers_per_step")
         n_batches_p = -(-(NS - 1) // args.batch)
         # pixel model alone: the multi-frame path on a clean 1280x720 clip (the headline texture translating 1 px per
         # frame, CLI defaults, device RNG), K repetitions of one 80-frame chunk between one event pair. Measured on its
@@ -555,9 +571,9 @@ def main():
         bytes_frame = H * W * 53.0 + 16.0 * ev_per_frame                    # SURVEY 8(d): T = 1 form, per frame
         bytes_launch = H * W * (T * 1.0 + 52.0) + 16.0 * ev_per_frame * T   # SURVEY 8(d): one launch over T frames
         prof = {
-            "roofline": {"kernel": "conv_strip2 / conv_strip2up / conv_tc kernels (all UNet convolutions of one step, summed)",
+            "roofline": {"kernel": "conv_strip / conv_up2 / conv_tc kernels (all UNet convolutions of one step, summed)",
                          "bound": "tensor", "achieved": achieved, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
-                         "frac": achieved / pk["bf16_tflops_sustained"], "traffic": tr_conv,
+                         "frac": achieved / pk["bf16_tflops_sustained"],
                          "peak_source": pk["source"] + " (sustained 16-bit dense; burst %.1f)" % pk["bf16_tflops"],
                          "algorithmic_bytes": n_batches_p * (unet_activation_bytes(2, 4, Hd, Wd, args.batch) +
                                                              U * unet_activation_bytes(12, 5, Hd, Wd, args.batch)),
@@ -565,14 +581,12 @@ def main():
                          "launches_per_step": conv_n.value, "share_of_step": conv_ms.value / step_ms_prof,
                          "largest_layer": {"layer": names[big], "ms_per_launch": ms23[big] / n23[big],
                                            "tflops": fl23[big] / (ms23[big] * 1e-3) / 1e12,
-                                           "frac": fl23[big] / (ms23[big] * 1e-3) / 1e12 / pk["bf16_tflops_sustained"],
-                                           "traffic": traffic.get(names[big])},
+                                           "frac": fl23[big] / (ms23[big] * 1e-3) / 1e12 / pk["bf16_tflops_sustained"]},
                          "layers": layers},
             "roofline_emulator": {
                 "kernel": "emu_fused_update + count + plan + emit (multi-frame pixel model, one chunk of %d frames)" % T,
                 "bound": "hbm", "achieved": bytes_frame / (us_frame * 1e-6) / 1e9, "peak": pk["hbm_gbs"], "unit": "GB/s",
                 "frac": bytes_frame / (us_frame * 1e-6) / 1e9 / pk["hbm_gbs"],
-                "traffic": traffic.get("emu_fused_chunk"),
                 "bytes_per_frame": bytes_frame, "us_per_frame": us_frame, "frames_per_launch": T,
                 "us_per_chunk": uc.value, "us_update_kernel": uu.value,
                 "basis": "SURVEY 8(d) per-call figure (53 B/px + 16 B/event per frame: the frame-by-frame API's traffic) "
@@ -709,7 +723,7 @@ def slomo_event_delta(devname, wts):
         cnt.append((em.num_events_total, em.num_events_on, em.num_events_off))
         em.cleanup()
     (a, a_on, a_off), (b, b_on, b_off) = cnt
-    return {"what": "346x260 gradients.py clip, 2 pairs x10 = 20 frames: fp16 tcgen05 SloMo vs float32 torch reference "
+    return {"what": "346x260 gradients.py clip, 2 pairs x10 = 20 frames: fp16 wgmma SloMo vs float32 torch reference "
                     "frames, same pixel model (noise off)",
             "dn_abs_diff_hist": np.bincount(d.ravel(), minlength=4)[:8].tolist(), "dn_max": int(d.max()),
             "dn_mean": float(d.mean()),

@@ -1,9 +1,9 @@
 /*
- * v2e_b200 -- C ABI of the B200-native hot paths of SensorsINI/v2e.
+ * v2e_b200 -- C ABI of the H100-native (sm_90a) hot paths of SensorsINI/v2e.
  *
  * The reference is pure Python and has no FFI; its boundary for these paths is two
  * Python classes (SURVEY.md 8b). This header is the boundary a maintainer binds
- * (ctypes / cffi, see INTEGRATION.md) to put the sm_100a kernels behind
+ * (ctypes / cffi, see INTEGRATION.md) to put the sm_90a kernels behind
  *   v2ecore/emulator.py:35   class EventEmulator  (generate_events, :619)
  *   v2ecore/slomo.py:37      class SuperSloMo     (interpolate, :231)
  *
@@ -275,7 +275,7 @@ void *v2e_emu_state_ptr(V2eEmu *h, int which);
  * and the per-frame tensor code of v2ecore/slomo.py:330-444.                      */
 /* ------------------------------------------------------------------------- */
 
-/* conv2d(stride 1, "same" zero padding) + bias + LeakyReLU(slope) as a tcgen05 implicit GEMM
+/* conv2d(stride 1, "same" zero padding) + bias + LeakyReLU(slope) as a wgmma implicit GEMM
  * (model.py:72-76, 145-154, 213-225: every conv of the UNet is followed by leaky_relu(0.1)).
  * Activations: NHWC fp16, channel counts padded to a multiple of 16 (padding channels zero).
  *   x1_dev [N,H,W,C1], optional x2_dev [N,H,W,C2] (C2 = 0: none) -- the logical input is

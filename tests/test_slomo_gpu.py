@@ -1,4 +1,4 @@
-"""GPU parity tests of the SuperSloMo path: tcgen05 conv kernel, UNet, warps/blend, Pillow-exact
+"""GPU parity tests of the SuperSloMo path: wgmma conv kernels, UNet, warps/blend, Pillow-exact
 resizes and the SuperSloMo drop-in, against the float32 torch reference (oracle/slomo_ref.py) and
 the fixtures produced by the unmodified reference classes.
 
@@ -68,7 +68,7 @@ CONV_CASES = [
 
 @pytest.mark.parametrize("case", CONV_CASES)
 def test_conv_tc_matches_torch(case):
-    """tcgen05 implicit-GEMM conv + bias + LeakyReLU vs torch conv2d on the same fp16-rounded operands
+    """wgmma implicit-GEMM conv + bias + LeakyReLU vs torch conv2d on the same fp16-rounded operands
     (fp32 accumulate on both sides). Tolerance: fp16 output rounding, 2e-3 relative + 2e-3 absolute."""
     N, H, W, C1, C2, Cout, K, mode = case
     Lm, L = _lib()
@@ -129,8 +129,8 @@ def pack_w_strip(w, C1, C2, KC):
 
 @pytest.mark.parametrize("case", STRIP_CASES)
 def test_conv_strip_kernel_matches_torch(case):
-    """Strip kernels (resident weights, input-row ring, descriptor-shifted taps; row-stacked MMAs into a TMEM
-    accumulator ring) vs torch conv2d on the same fp16-rounded operands. Same tolerance as the per-tap kernel."""
+    """Strip kernel (resident weights, input-row ring, descriptor-shifted taps, two warpgroups taking turns over
+    pairs of output rows) vs torch conv2d on the same fp16-rounded operands. Same tolerance as the per-tap kernel."""
     N, H, W, C1, C2, Cout, K, mode = case
     Lm, L = _lib()
     g = torch.Generator().manual_seed(hash(case) & 0xFFFF)

@@ -1,4 +1,4 @@
-"""v2e_b200 -- B200-native (sm_100a) implementation of the two data-parallel hot paths of
+"""v2e_b200 -- H100-native (sm_90a) implementation of the two data-parallel hot paths of
 SensorsINI/v2e: the DVS pixel model (EventEmulator) and the SuperSloMo frame interpolator.
 
 Import is cheap and GPU-free; the CUDA library (v2e_b200/lib/libv2e_b200.so, C ABI in

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a shared library (nvcc, no torch headers involved).
+"""In-tree build of the sm_90a (H100) shared library (nvcc, no torch headers involved).
 
 The library is a plain C-ABI .so (include/v2e_b200.h); it links only the CUDA runtime and driver.
 nvcc cross-compiles without a GPU, so this also runs on the CPU-only build container.
@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libv2e_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "--expt-extended-lambda", "-Xcompiler", "-fPIC",
           "-I", os.path.join(os.path.dirname(HERE), "include")]
 

@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution + bias + LeakyReLU on the 5th-gen tensor cores (sm_100a).
+// Implicit-GEMM convolution + bias + LeakyReLU on the Hopper tensor cores (sm_90a, wgmma).
 //
 // Replaces the 23 conv2d+leaky_relu pairs of the reference's UNet (v2ecore/model.py:10-226, called
 // from v2ecore/slomo.py:343, 415-419), which the reference runs as stock cuDNN kernels.
@@ -6,20 +6,19 @@
 //   D[pixel, cout] = sum_{tap=(r,s)} sum_{c} X[n, y+r-ph, x+s-pw, c] * Wt[cout, tap, c]      (+bias, lrelu)
 //
 // Layout: activations NHWC fp16 (C padded to a multiple of 16), weights [Cout_pad][KH*KW*Ctot] fp16
-// (K index = tap*Ctot + c), accumulation fp32 in TMEM.
+// (K index = tap*Ctot + c), accumulation fp32 in registers.
 // One CTA computes a 128-pixel (8 rows x 16 columns) x BN-channel output tile:
-//   warp 0      : TMA producer. For every filter tap and every KC-channel slab it issues one 4-D tiled
+//   warp 8      : TMA producer. For every filter tap and every KC-channel slab it issues one 4-D tiled
 //                 load of the *shifted* 8x16 window (cp.async.bulk.tensor, 128B/64B/32B swizzle) --
 //                 out-of-bounds rows/columns are zero-filled by TMA, which is exactly the conv's zero
 //                 padding, so no im2col buffer and no halo logic -- plus one 2-D load of the BN x KC
 //                 weight slab. A concatenated input (up-blocks: cat(x, skip), model.py:150-153) is
 //                 read from two tensor maps, so the concat is never materialised.
-//   warp 1      : allocates TMEM, issues tcgen05.mma (M=128, N=BN, K=16, kind::f16) from the swizzled
-//                 shared-memory stages, commits to mbarriers.
-//   warps 2..5  : epilogue: tcgen05.ld the accumulator (lane == pixel), + bias, LeakyReLU(0.1),
-//                 convert and store NHWC (fp16) or the first channels as fp32 (network outputs).
-// Pipeline: kStages-deep mbarrier ring between producer and MMA issuer; two CTAs per SM overlap one
-// tile's epilogue with the other's main loop.
+//   warps 0..7  : two consumer warpgroups; warpgroup g issues wgmma (M=64, N=BN, K=16) for pixels
+//                 64g..64g+63 of the tile from the swizzled shared-memory stages, keeps one stage of MMAs
+//                 in flight, releases the stage before it, and finally applies bias + LeakyReLU(0.1) and
+//                 stores NHWC (fp16) or the first channels as fp32 (network outputs) from its registers.
+// Pipeline: a kStages-deep mbarrier ring between the producer and the two warpgroups.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -35,20 +34,20 @@
 
 namespace {
 
-constexpr int kTileH = 8, kTileW = 16, kBM = kTileH * kTileW;   // 128 pixels = UMMA M
-constexpr int kStages = 4;      // barrier slots; ConvParams::stages is the depth actually used (2-4)
-constexpr int kConvThreads = 192;
+constexpr int kTileH = 8, kTileW = 16, kBM = kTileH * kTileW;   // 128 pixels = two wgmma M = 64 halves
+constexpr int kStages = 4;
+constexpr int kConvThreads = 288;      // warps 0..3 and 4..7: consumer warpgroups, warp 8: TMA producer
+constexpr int kProducerWarp = 8;
+constexpr int kConsumerWarps = 8;      // every consumer warp arrives once on an empty barrier
 
 struct ConvParams {
     int N, H, W;
     int C1, C2;                 // padded channel counts of the two inputs (C2 = 0: single input)
     int KH, KW;
     int KC;                     // channels per K slab: 64 / 32 / 16  -> swizzle 128B / 64B / 32B
-    int BN;                     // output channels per CTA (UMMA N)
-    int stages;                 // depth of the producer / issuer ring (<= kStages)
-    int MT;                     // 8x16 pixel tiles per CTA (1 or 2, stacked vertically: M = 128 or 2 x 128)
+    int BN;                     // output channels per CTA (wgmma N)
+    int stages;                 // depth of the producer / consumer ring (<= kStages)
     int co_fast;                // grid order: 1 = output-channel blocks in gridDim.x
-    int cl;                     // 1: clusters of 2 CTAs along the tile axis, weight slabs multicast
     int tiles_x, tiles_y;
     int out_cstride;            // channel stride (elements) of the fp16 NHWC output
     int out_mode;               // 0: fp16 NHWC; 1: fp32 [N,H,W,8], first co_real channels
@@ -58,168 +57,141 @@ struct ConvParams {
     void *out;
 };
 
-__global__ void __launch_bounds__(kConvThreads)
+__device__ __forceinline__ uint8_t *align1024(uint8_t *p) { return (uint8_t *)(((uintptr_t)p + 1023) & ~(uintptr_t)1023); }
+
+__device__ __forceinline__ float lrelu(float x, float slope) { return x > 0.f ? x : x * slope; }
+
+// Row i (0 / 1) of this thread's share of a 64 x BN accumulator (layout: tc_common.cuh, wgmma): bias, LeakyReLU and
+// the store of output pixel `pix`. out_mode 0: fp16, channels co0 + column at stride cstride; 1: fp32 [.., 8], the
+// first 8 columns. The fp16 values are returned in h (for the pooled epilogue).
+template <int BN>
+__device__ __forceinline__ void epilogue_row(const float (&d)[BN / 2], int i, bool inb, size_t pix, int lane,
+                                             const float *bias, float slope, int out_mode, void *out, int cstride,
+                                             int co0, __half2 (&h)[BN / 8]) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+        const int c = 8 * j + 2 * (lane & 3);
+        const float x0 = lrelu(d[4 * j + 2 * i] + __ldg(bias + c), slope);
+        const float x1 = lrelu(d[4 * j + 2 * i + 1] + __ldg(bias + c + 1), slope);
+        h[j] = __floats2half2_rn(x0, x1);
+        if (inb) {
+            if (out_mode == 0) *(__half2 *)((__half *)out + pix * cstride + co0 + c) = h[j];
+            else if (j == 0) *(float2 *)((float *)out + pix * 8 + c) = make_float2(x0, x1);
+        }
+    }
+}
+
+template <int BN>
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBh, const ConvParams p) {
+               const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // carve: stages of [A 128 x KC fp16][B BN x KC fp16], 1024-byte aligned
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t *smem = align1024(smem_raw);
     const uint32_t a_bytes = kBM * p.KC * 2;
-    const uint32_t b_bytes_raw = p.BN * p.KC * 2;
+    const uint32_t b_bytes_raw = BN * p.KC * 2;
     const uint32_t b_bytes = (b_bytes_raw + 1023) & ~1023u;
-    const int MT = p.MT;                                   // vertically adjacent 8x16 tiles sharing the weight slab
-    const uint32_t stage_bytes = MT * a_bytes + b_bytes;
-    __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages], tmem_full_bar;
-    __shared__ uint32_t tmem_base_smem;
+    const uint32_t stage_bytes = a_bytes + b_bytes;
+    __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // output-channel block fastest (gridDim.x when p.co_fast): the CTAs that share an input window run together, so
     // the window comes from DRAM once and from L2 for its siblings
     const int tile = p.co_fast ? blockIdx.y : blockIdx.x;
     const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, n = tile / (p.tiles_x * p.tiles_y);
-    const int x0 = tx * kTileW, y0 = ty * kTileH * MT;
-    const int n0 = (p.co_fast ? blockIdx.x : blockIdx.y) * p.BN;
+    const int x0 = tx * kTileW, y0 = ty * kTileH;
+    const int n0 = (p.co_fast ? blockIdx.x : blockIdx.y) * BN;
     const int Ctot = p.C1 + p.C2;
     const int slabs = Ctot / p.KC;
     const int k_iters = p.KH * p.KW * slabs;
-    const uint32_t tmem_cols = MT * p.BN < 32 ? 32 : MT * p.BN;
 
-    // p.cl: clusters of two CTAs with the same output-channel block and neighbouring pixel tiles share every weight
-    // slab: each CTA loads half of it and multicasts it to both (tmBh: box of BN / 2 rows). A stage may be refilled
-    // only when BOTH issuers have released it, so the empty barriers count two arrivals, delivered by multicast commits.
-    const uint32_t crank = p.cl ? cluster_ctarank() : 0u;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], p.cl ? 2 : 1); }
-        mbar_init(&tmem_full_bar, 1);
+        for (int s = 0; s < kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
         fence_barrier_init();
     }
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         prefetch_tmap(&tmA);
         if (p.C2) prefetch_tmap(&tmA2);
         prefetch_tmap(&tmB);
-        if (p.cl) prefetch_tmap(&tmBh);
     }
-    if (warp == 1) {
-        tmem_alloc(&tmem_base_smem, tmem_cols);
-        tmem_relinquish();
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    if (p.cl) cluster_sync_all();            // the peer's barriers exist before anything is multicast into this CTA
-    tcgen05_fence_after();
-    const uint32_t tmem_acc = tmem_base_smem;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ===== TMA producer =====
         if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             const int ph = p.KH / 2, pw = p.KW / 2;
-            int it = 0;
             for (int tap = 0; tap < p.KH * p.KW; tap++) {
                 const int r = tap / p.KW, s = tap % p.KW;
-                for (int sl = 0; sl < slabs; sl++, it++) {
+                for (int sl = 0; sl < slabs; sl++) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t *sa = smem + stage * stage_bytes, *sb = sa + MT * a_bytes;
-                    mbar_expect_tx(&full_bar[stage], MT * a_bytes + b_bytes_raw);
+                    uint8_t *sa = smem + stage * stage_bytes, *sb = sa + a_bytes;
+                    mbar_expect_tx(&full_bar[stage], a_bytes + b_bytes_raw);
                     const int c = sl * p.KC;
-                    for (int mt = 0; mt < MT; mt++) {
-                        if (c < p.C1) tma_load_4d(sa + mt * a_bytes, &tmA, &full_bar[stage], c, x0 + s - pw, y0 + mt * kTileH + r - ph, n);
-                        else tma_load_4d(sa + mt * a_bytes, &tmA2, &full_bar[stage], c - p.C1, x0 + s - pw, y0 + mt * kTileH + r - ph, n);
-                    }
-                    if (p.cl) {
-                        const uint32_t hb = b_bytes_raw / 2;
-                        tma_load_2d_multicast(sb + crank * hb, &tmBh, &full_bar[stage], tap * Ctot + c, n0 + (int)crank * (p.BN / 2),
-                                              (uint16_t)3);
-                    } else {
-                        tma_load_2d(sb, &tmB, &full_bar[stage], tap * Ctot + c, n0);
-                    }
+                    if (c < p.C1) tma_load_4d(sa, &tmA, &full_bar[stage], c, x0 + s - pw, y0 + r - ph, n);
+                    else tma_load_4d(sa, &tmA2, &full_bar[stage], c - p.C1, x0 + s - pw, y0 + r - ph, n);
+                    tma_load_2d(sb, &tmB, &full_bar[stage], tap * Ctot + c, n0);
                     if (++stage == p.stages) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: converged warp, one elected lane issues (see umma_f16_pred) =====
-        const uint32_t leader = elect_one();
-        const uint32_t swz = p.KC == 64 ? 2u : (p.KC == 32 ? 4u : 6u);   // SmemDescriptor layout_type
-        const uint32_t sbo = 8u * p.KC * 2u;                             // bytes between 8-row groups
-        const uint32_t idesc = make_idesc_f16(kBM, p.BN);
-        const uint64_t dhi = make_smem_desc(0, swz, sbo);                // everything but the start address
-        const uint32_t sa0 = smem_u32(smem) >> 4, stage16 = stage_bytes >> 4, a16 = a_bytes >> 4;
+    } else {
+        // ===== consumer warpgroup g: pixels 64g .. 64g+63 of the tile =====
+        const int g = warp >> 2;
+        const uint64_t d0 = make_smem_desc(smem_u32(smem), swizzle_layout(p.KC), 8u * p.KC * 2u);
+        const uint32_t stage16 = stage_bytes >> 4, a16 = a_bytes >> 4, half16 = (64u * p.KC * 2u) >> 4;
         const int ksteps = p.KC / 16;
-        int stage = 0;
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+        int stage = 0, prev = -1;
         uint32_t phase = 0;
         for (int it = 0; it < k_iters; it++) {
             mbar_wait(&full_bar[stage], phase);
-            tcgen05_fence_after();
-            const uint32_t alo = sa0 + (uint32_t)stage * stage16 + (uint32_t)(dhi & 0xFFFF0000u);
-            const uint32_t blo = alo + (uint32_t)MT * a16;
-            for (int mt = 0; mt < MT; mt++)
-                for (int j = 0; j < ksteps; j++)
-                    umma_f16_pred(tmem_acc + (uint32_t)(mt * p.BN), desc_with_lo(dhi, alo + (uint32_t)mt * a16 + 2u * j),
-                                  desc_with_lo(dhi, blo + 2u * j), idesc, (uint32_t)((it | j) != 0), leader);
-            if (p.cl) umma_commit_mc_pred(&empty_bar[stage], (uint16_t)3, leader);      // ... in both CTAs of the cluster
-            else umma_commit_pred(&empty_bar[stage], leader);     // frees the smem slot once these MMAs retire
+            const uint32_t base = (uint32_t)stage * stage16;
+            wgmma_fence();
+            for (int j = 0; j < ksteps; j++)
+                wgmma_f16<BN>(acc, desc_add(d0, base + (uint32_t)g * half16 + 2u * j), desc_add(d0, base + a16 + 2u * j),
+                              (uint32_t)((it | j) != 0));
+            wgmma_commit();
+            wgmma_wait<1>();                 // the stage before this one has been read: hand it back
+            if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+            prev = stage;
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
         }
-        umma_commit_pred(&tmem_full_bar, leader);            // accumulator complete
-    } else {
-        // ===== epilogue: 4 warps, TMEM lane group = warp % 4 =====
-        const int q = warp & 3;
-        const int m = q * 32 + lane;                     // pixel row of the tile == TMEM lane
-        mbar_wait(&tmem_full_bar, 0);
-        tcgen05_fence_after();
-        for (int mt = 0; mt < MT; mt++) {
-            const int py = y0 + mt * kTileH + m / kTileW, px = x0 + m % kTileW;
-            const bool inb = py < p.H && px < p.W && n < p.N;      // n >= N: the padding tile of an odd cluster grid
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        __half2 hv[BN / 8];
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int m = 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+            const int py = y0 + m / kTileW, px = x0 + m % kTileW;
+            const bool inb = py < p.H && px < p.W;
             const size_t pix = ((size_t)n * p.H + py) * p.W + px;
-            for (int c0 = 0; c0 < p.BN; c0 += 16) {
-                uint32_t v[16];
-                tmem_ld_32x32b_x16(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * p.BN + c0), v);
-                tmem_ld_wait();
-                float f[16];
-#pragma unroll
-                for (int j = 0; j < 16; j++) {
-                    float x = __uint_as_float(v[j]) + __ldg(p.bias + n0 + c0 + j);
-                    f[j] = x > 0.f ? x : x * p.slope;
-                }
-                if (inb) {
-                    if (p.out_mode == 0) {
-                        __half2 h[8];
-#pragma unroll
-                        for (int j = 0; j < 8; j++) h[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-                        uint4 *dst = (uint4 *)((__half *)p.out + pix * p.out_cstride + n0 + c0);
-                        dst[0] = *(uint4 *)&h[0];
-                        dst[1] = *(uint4 *)&h[4];
-                    } else if (c0 == 0 && n0 == 0) {
-                        float4 *dst = (float4 *)((float *)p.out + pix * 8);
-                        dst[0] = make_float4(f[0], f[1], f[2], f[3]);
-                        dst[1] = make_float4(f[4], f[5], f[6], f[7]);
-                    }
-                }
-            }
+            epilogue_row<BN>(acc, i, inb, pix, lane, p.bias + n0, p.slope, p.out_mode, p.out, p.out_cstride, n0, hv);
         }
-        tcgen05_fence_before();
     }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_acc, tmem_cols);
-    }
-    if (p.cl) cluster_sync_all();            // nobody leaves while the peer may still arrive on its barriers
 }
 
 
 constexpr int kRowTile = 128;
 
 // ---------------------------------------------------------------------------------------------
-// Strip kernel: the full-resolution layers (N = 32 output channels, 7x7 / 3x3) that dominate the UNet.
-// A CTA walks down a 128-pixel-wide column strip. The layer's whole weight tensor stays resident in
-// shared memory; input rows live in a ring of NSLOT row buffers ([128+KW-1 pixels] x KC channels per
-// slab, TMA-swizzled). Moving one output row down costs ONE new input row from L2 (instead of KH rows
-// with a per-tile halo, or KH*KW windows with per-tap loads); every filter tap (r, s) is a descriptor
-// offset: ring slot of input row y+r-ph, start + s pixels. Two TMEM accumulators overlap the epilogue of
-// row y with the MMAs of row y+1.
+// Strip kernel: the full-resolution layers (Cout_pad <= 64, 7x7 / 5x5 / 3x3) that dominate the UNet.
+// A CTA walks down a 128-pixel-wide column strip. The layer's weights (or the slice of the output channels
+// this CTA class computes) stay resident in shared memory; input rows live in a ring of NSLOT row buffers
+// ([128+KW-1 pixels] x KC channels per slab, TMA-swizzled). Moving one output row down costs ONE new input
+// row from L2 (instead of KH rows with a per-tile halo, or KH*KW windows with per-tap loads); every filter
+// tap (r, s) is a descriptor offset: ring slot of input row y+r-ph, start + s pixels.
+//   warp 8     : TMA producer: the weights once per CTA, then one row (all slabs) per ring slot.
+//   warps 0..7 : two consumer warpgroups, taking turns over PAIRS of output rows of an item (warpgroup g:
+//                pairs g, g+2, ...). A row is 2 x (M=64) wgmma tiles over the 128 pixels, N = BN, accumulated
+//                in registers; then bias, LeakyReLU and the store. A ring slot is released by both
+//                warpgroups (every row of the item exactly once each) when neither needs it any more.
+// POOL: F.avg_pool2d(out, 2) written beside the output (model.py:71: the pool that opens a down block). A pair
+// is rows (2k, 2k+1) of the item (items start on even rows), so the 2x2 window is in one warpgroup: the upper
+// row's fp16 activations stay in registers, the horizontal neighbour is the lane 4 apart.
 // ---------------------------------------------------------------------------------------------
 struct StripParams {
     int N, H, W;
@@ -228,82 +200,89 @@ struct StripParams {
     int KC, BN;
     int tiles_x, seg_h, n_seg, n_items;
     int nslot;
-    int variant;                   // 0: per-tap MMAs (first strip kernel), 1: row-stacked (strip2)
-    int acc_slots, tmem_cols;      // strip2: accumulator ring (slots of BN columns), TMEM allocation
-    void *pool_out;                // strip2 POOL variants: F.avg_pool2d(out, 2) written beside the output
-    int pool_cstride;              //   [N, H/2, W/2, pool_cstride] fp16 (model.py:71: the pool that opens a down block)
-    long long *dbg;                // STRIP2_DEBUG builds: per-CTA issuer wait cycles
-    int n_split, cout_pad;         // strip2: output channels split over n_split CTA classes of BN = cout_pad / n_split
+    void *pool_out;                // POOL: [N, H/2, W/2, pool_cstride] fp16
+    int pool_cstride;
+    int n_split, cout_pad;         // output channels split over n_split CTA classes of BN = cout_pad / n_split
                                    // (layers whose whole weight tensor does not fit in shared memory)
     int slab_bytes;                // bytes of one row buffer of one slab (1024-aligned)
-    int w_bytes;                   // all weights: slabs*taps*BN*KC*2
-    int w_rows_per_load, w_loads;
+    int w_bytes;                   // resident weights
+    int w_rows_per_load, w_loads;  // fused up-sampling kernel: weight rows per TMA load, loads
     int out_cstride, out_mode, co_real;
     float slope;
     const float *bias;
     void *out;
 };
 constexpr int kMaxSlot = 12;
+constexpr int kStripThreads = 288;      // warps 0..3 and 4..7: consumer warpgroups, warp 8: TMA producer
 
-constexpr int kStripThreads = 224;      // warps: 0 producer, 1 issuer A, 2-5 epilogue, 6 issuer B
+// Ring bookkeeping of one consumer warpgroup over the input rows of one item: rows are waited for in order and
+// released in order, each exactly once (a slot's empty barrier counts the arrivals of all eight consumer warps).
+struct RowRing {
+    uint64_t *full, *empty;
+    uint32_t nslot, cnt;           // cnt: ring rows filled before this item (all items)
+    int waited, released;
+    __device__ __forceinline__ uint32_t slot(int i) const { return (cnt + (uint32_t)i) % nslot; }
+    __device__ __forceinline__ void wait_upto(int n) {
+        for (; waited < n; waited++) {
+            const uint32_t g = cnt + (uint32_t)waited;
+            mbar_wait(&full[g % nslot], (g / nslot) & 1u);
+        }
+    }
+    // every wgmma that read rows < n has completed (wgmma_wait) before this is called
+    __device__ __forceinline__ void release_upto(int n, int lane) {
+        wait_upto(n);              // observe every fill, so that a later wait on the slot cannot alias this phase
+        __syncwarp();
+        for (; released < n; released++)
+            if (lane == 0) mbar_arrive(&empty[slot(released)]);
+    }
+};
 
-template <int KW, int KC>
-__global__ void __launch_bounds__(kStripThreads)
+template <int KW, int KC, int BN, bool POOL>
+__global__ void __launch_bounds__(kStripThreads, 1)
 conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                   const __grid_constant__ CUtensorMap tmB, const StripParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    __shared__ __align__(8) uint64_t full_bar[kMaxSlot], empty_bar[kMaxSlot], w_bar, tmem_full_bar[4], tmem_empty_bar[4];
-    __shared__ uint32_t tmem_base_smem;
+    uint8_t *smem = align1024(smem_raw);
+    __shared__ __align__(8) uint64_t full_bar[kMaxSlot], empty_bar[kMaxSlot], w_bar;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int Ctot = p.C1 + p.C2;
-    const int slabs = Ctot / KC;
-    const int taps = p.KH * KW;
+    constexpr int KH = KW, ph = KH / 2, pw = KW / 2, taps = KH * KW;
     constexpr int PW = kRowTile + KW - 1;
-    const int ph = p.KH / 2, pw = KW / 2;
+    constexpr uint32_t tile_bytes = BN * KC * 2;            // one (slab, tap) weight tile
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int slabs = (p.C1 + p.C2) / KC;
     const uint32_t row_bytes = (uint32_t)p.slab_bytes * slabs;       // one ring slot (all slabs)
     uint8_t *ring = smem + ((p.w_bytes + 1023) & ~1023);
-    const uint32_t acc_cols = p.BN < 32 ? 32 : p.BN;
-    const uint32_t tmem_cols = acc_cols * 4;              // two issuers x double buffering
+    // CTA class: which slice of the output channels this CTA computes (weights resident per slice)
+    const int split = (int)blockIdx.x % p.n_split, co_off = split * BN;
+    const int item0 = (int)blockIdx.x / p.n_split, item_step = (int)gridDim.x / p.n_split;
 
     if (threadIdx.x == 0) {
-        // a ring slot is free again when BOTH issuers have retired their last MMA that reads it
-        for (int s = 0; s < p.nslot; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+        for (int s = 0; s < p.nslot; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
         mbar_init(&w_bar, 1);
-        for (int s = 0; s < 4; s++) { mbar_init(&tmem_full_bar[s], 1); mbar_init(&tmem_empty_bar[s], 4); }
         fence_barrier_init();
     }
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         prefetch_tmap(&tmA);
         if (p.C2) prefetch_tmap(&tmA2);
         prefetch_tmap(&tmB);
     }
-    if (warp == 1) {
-        tmem_alloc(&tmem_base_smem, tmem_cols);
-        tmem_relinquish();
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ===== TMA producer =====
         if (lane == 0) {
             mbar_expect_tx(&w_bar, (uint32_t)p.w_bytes);
-            for (int l = 0; l < p.w_loads; l++)
-                tma_load_2d(smem + (size_t)l * p.w_rows_per_load * KC * 2, &tmB, &w_bar, 0, l * p.w_rows_per_load);
+            for (int t = 0; t < slabs * taps; t++)              // tile (slab, tap) of this CTA's output channels
+                tma_load_2d(smem + (size_t)t * tile_bytes, &tmB, &w_bar, 0, t * p.cout_pad + co_off);
             uint32_t cnt = 0;                                   // input rows loaded so far (all items)
-            for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+            for (int item = item0; item < p.n_items; item += item_step) {
                 const int tx = item % p.tiles_x, rest = item / p.tiles_x;
                 const int seg = rest % p.n_seg, n = rest / p.n_seg;
                 const int ya = seg * p.seg_h, yb = min(p.H, ya + p.seg_h);
                 const int x0 = tx * kRowTile;
                 for (int i = ya - ph; i < yb + ph; i++, cnt++) {
                     const int slot = (int)(cnt % (uint32_t)p.nslot);
-                    const uint32_t phase = (cnt / (uint32_t)p.nslot) & 1u;
-                    mbar_wait(&empty_bar[slot], phase ^ 1);
+                    mbar_wait(&empty_bar[slot], ((cnt / (uint32_t)p.nslot) & 1u) ^ 1u);
                     mbar_expect_tx(&full_bar[slot], (uint32_t)(PW * KC * 2 * slabs));
                     uint8_t *dst = ring + (size_t)slot * row_bytes;
                     for (int sl = 0; sl < slabs; sl++) {
@@ -314,508 +293,138 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 }
             }
         }
-    } else if (warp == 1 || warp == 6) {
-        // ===== two MMA issuers (converged warps, one elected lane each): issuer A takes the even output
-        // rows of an item, issuer B the odd ones, each into its own pair of TMEM accumulators, so two
-        // instruction streams feed the tensor pipe. Taps / k-steps are fully unrolled. =====
-        const int who = warp == 6;
-        const uint32_t leader = elect_one();
-        constexpr uint32_t swz = KC == 64 ? 2u : (KC == 32 ? 4u : 6u);
-        constexpr uint32_t rowb = (uint32_t)KC * 2u;
-        constexpr uint32_t sbo = 8u * rowb;
-        constexpr int ksteps = KC / 16;
-        const uint32_t idesc = make_idesc_f16(kBM, p.BN);
-        const uint64_t dhi = make_smem_desc(0, swz, sbo);
-        const uint32_t lo_flags = (uint32_t)(dhi & 0xFFFF0000u);
-        const uint32_t w16 = (smem_u32(smem) >> 4) | lo_flags, ring16 = (smem_u32(ring) >> 4) | lo_flags;
-        const uint32_t row16 = row_bytes >> 4, slab16 = (uint32_t)p.slab_bytes >> 4;
-        const uint32_t tap16 = ((uint32_t)p.BN * rowb) >> 4;              // one tap's weight tile
-        mbar_wait(&w_bar, 0);
-        uint32_t cnt = 0;                                   // index of the first input row of this item
-        uint32_t acc = 0, acc_phase = 0;                    // this issuer's accumulator ring (2 deep)
-        for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-            const int rest = item / p.tiles_x;
-            const int seg = rest % p.n_seg;
-            const int ya = seg * p.seg_h, yb = min(p.H, ya + p.seg_h);
-            const int rows_in = (yb - ya) + 2 * ph;
-            int waited = 0;                                 // input rows of this item known to be in smem
-            int released = 0;                               // input rows of this item this issuer has released
-            for (int yr = who; yr < yb - ya; yr += 2) {     // output row (relative to the item)
-                const int need = yr + p.KH;                 // input rows 0 .. yr+KH-1 of the item
-                for (; waited < need; waited++) {
-                    const uint32_t g = cnt + (uint32_t)waited;
-                    mbar_wait(&full_bar[g % (uint32_t)p.nslot], (g / (uint32_t)p.nslot) & 1u);
-                }
-                const uint32_t ai = (uint32_t)who * 2u + acc;
-                mbar_wait(&tmem_empty_bar[ai], acc_phase ^ 1);
-                tcgen05_fence_after();
-                const uint32_t tmem_acc = tmem_base + ai * acc_cols;
-                uint32_t first = 0;                         // 0 for the very first MMA of the row (overwrite)
-                for (int r = 0; r < p.KH; r++) {
-                    const uint32_t g = cnt + (uint32_t)(yr + r);
-                    const uint32_t a_row = ring16 + (g % (uint32_t)p.nslot) * row16;
-                    for (int sl = 0; sl < slabs; sl++) {
-                        const uint32_t a_lo = a_row + (uint32_t)sl * slab16;
-                        const uint32_t b_lo = w16 + (uint32_t)((sl * taps + r * KW)) * tap16;
-#pragma unroll
-                        for (int s = 0; s < KW; s++) {
-#pragma unroll
-                            for (int j = 0; j < ksteps; j++) {
-                                umma_f16_pred(tmem_acc, desc_with_lo(dhi, a_lo + (uint32_t)(s * (rowb >> 4) + 2 * j)),
-                                              desc_with_lo(dhi, b_lo + (uint32_t)s * tap16 + (uint32_t)(2 * j)), idesc,
-                                              first, leader);
-                                first = 1;
-                            }
-                        }
-                    }
-                }
-                umma_commit_pred(&tmem_full_bar[ai], leader);
-                // this issuer's next row is yr+2 and reads input rows >= yr+2: release everything below
-                for (; released <= yr + 1 && released < rows_in; released++) {
-                    const uint32_t g = cnt + (uint32_t)released;
-                    umma_commit_pred(&empty_bar[g % (uint32_t)p.nslot], leader);
-                }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-            // end of the item: observe every fill (so that a later wait on the same slot cannot alias an
-            // earlier phase of the same parity), then release what is left: each issuer releases every
-            // input row of the item exactly once
-            for (; waited < rows_in; waited++) {
-                const uint32_t g = cnt + (uint32_t)waited;
-                mbar_wait(&full_bar[g % (uint32_t)p.nslot], (g / (uint32_t)p.nslot) & 1u);
-            }
-            for (; released < rows_in; released++) {
-                const uint32_t g = cnt + (uint32_t)released;
-                umma_commit_pred(&empty_bar[g % (uint32_t)p.nslot], leader);
-            }
-            cnt += (uint32_t)rows_in;
-        }
     } else {
-        // ===== epilogue (warps 2..5: TMEM lane group = warp % 4) =====
-        const int q = warp & 3;
-        const int m = q * 32 + lane;
-        uint32_t accs[2] = {0, 0}, phases[2] = {0, 0};      // accumulator ring position of issuer A / B
-        for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+        // ===== consumer warpgroup g =====
+        const int g = warp >> 2;
+        constexpr uint32_t sbo = 8u * KC * 2u, rowb16 = (KC * 2u) >> 4, half16 = (64u * KC * 2u) >> 4;
+        constexpr uint32_t tile16 = tile_bytes >> 4;
+        constexpr int ksteps = KC / 16;
+        const uint64_t dw = make_smem_desc(smem_u32(smem), swizzle_layout(KC), sbo);
+        const uint64_t dr = make_smem_desc(smem_u32(ring), swizzle_layout(KC), sbo);
+        const uint32_t row16 = row_bytes >> 4, slab16 = (uint32_t)p.slab_bytes >> 4;
+        mbar_wait(&w_bar, 0);
+        RowRing rr{full_bar, empty_bar, (uint32_t)p.nslot, 0u, 0, 0};
+        for (int item = item0; item < p.n_items; item += item_step) {
             const int tx = item % p.tiles_x, rest = item / p.tiles_x;
             const int seg = rest % p.n_seg, n = rest / p.n_seg;
             const int ya = seg * p.seg_h, yb = min(p.H, ya + p.seg_h);
-            const int px = tx * kRowTile + m;
-            const bool inb = px < p.W;
-            for (int y = ya; y < yb; y++) {
-                const int who = (y - ya) & 1;
-                const uint32_t ai = (uint32_t)who * 2u + accs[who];
-                mbar_wait(&tmem_full_bar[ai], phases[who]);
-                tcgen05_fence_after();
-                const uint32_t tmem_acc = tmem_base + ai * acc_cols;
-                const size_t pix = ((size_t)n * p.H + y) * p.W + px;
-                for (int c0 = 0; c0 < p.BN; c0 += 16) {
-                    uint32_t v[16];
-                    tmem_ld_32x32b_x16(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-                    tmem_ld_wait();
-                    float f[16];
-#pragma unroll
-                    for (int j = 0; j < 16; j++) {
-                        float x = __uint_as_float(v[j]) + __ldg(p.bias + c0 + j);
-                        f[j] = x > 0.f ? x : x * p.slope;
-                    }
-                    if (inb) {
-                        if (p.out_mode == 0) {
-                            __half2 h[8];
-#pragma unroll
-                            for (int j = 0; j < 8; j++) h[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-                            uint4 *dst = (uint4 *)((__half *)p.out + pix * p.out_cstride + c0);
-                            dst[0] = *(uint4 *)&h[0];
-                            dst[1] = *(uint4 *)&h[4];
-                        } else if (c0 == 0) {
-                            float4 *dst = (float4 *)((float *)p.out + pix * 8);
-                            dst[0] = make_float4(f[0], f[1], f[2], f[3]);
-                            dst[1] = make_float4(f[4], f[5], f[6], f[7]);
-                        }
-                    }
-                }
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tmem_empty_bar[ai]);
-                if (++accs[who] == 2) { accs[who] = 0; phases[who] ^= 1; }
-            }
-        }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Strip kernel, row-stacked form ("strip2"): the same column-strip walk, but the MMA is turned round so
-// that ONE fetch of an input row feeds every output row it contributes to.
-//
-// With N = Cout = 16..64 a per-tap MMA (M=128, N=Cout, K=16) spends 32 cycles fetching its 128-row A
-// operand for 8..32 cycles of tensor work: the first strip kernel was bound by the A fetch (ncu: operand
-// fetch 48 %, tensor pipe 35 %). But input row i at horizontal shift s is the A operand of KH different
-// (output row, filter row) pairs: out[i+ph-r] += W[r][s] . in[i][x+s]. So the weights of one filter COLUMN
-// s are stacked into one B operand [W[KH-1][s]; ...; W[0][s]] (N = KH*Cout rows, e.g. 224 for the 7x7
-// layers) and the accumulators of consecutive output rows sit side by side in a TMEM ring (R slots of
-// Cout columns): one MMA (M=128, N=KH*Cout, K=16) adds input row i into all KH live output rows at once.
-// A is fetched once per KH*Cout output channels instead of once per Cout; MMAs per row drop by KH (98 ->
-// 14 for conv2), so one issuer warp is enough.
-//
-//   warp 0     : TMA producer. Weights once per CTA, tile (slab, r, s) placed at [(slab*KW + s)*KH + (KH-1-r)]
-//                so that the r-stack of a column is contiguous; then one box per (input row, channel slab)
-//                into a small ring (each entry is consumed by one burst of MMAs and released).
-//   warp 1     : MMA issuer. Per input row: wait for the accumulator slot of the output row that starts
-//                here, then for every slab / shift / k-step one MMA per contiguous slot range (the ring
-//                wrap and N <= 256 split a stack into at most a few ranges). Accumulate flag always on:
-//                a slot is zeroed by the epilogue when it is drained. After the row's last MMA the output
-//                row that received its last contribution (filter row KH-1) is committed to the epilogue.
-//   warps 2..5 : epilogue: tcgen05.ld, bias, LeakyReLU, store; tcgen05.st zeros; release the slot.
-// ---------------------------------------------------------------------------------------------
-constexpr int kMaxAcc = 32;
-constexpr int kStrip2Threads = 320;      // warps: 0 producer, 1 issuer, 2..9 epilogue
-
-template <int KW, int KC, bool POOL>
-__global__ void __launch_bounds__(kStrip2Threads)
-conv_strip2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                   const __grid_constant__ CUtensorMap tmB, const StripParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    __shared__ __align__(8) uint64_t full_bar[kMaxSlot], empty_bar[kMaxSlot], w_bar, acc_full[kMaxAcc], acc_empty[kMaxAcc];
-    __shared__ uint32_t tmem_base_smem;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int Ctot = p.C1 + p.C2;
-    const int slabs = Ctot / KC;
-    const int KH = p.KH;
-    constexpr int PW = kRowTile + KW - 1;
-    const int ph = KH / 2, pw = KW / 2;
-    uint8_t *ring = smem + ((p.w_bytes + 1023) & ~1023);
-    const int R = p.acc_slots;
-    const uint32_t BN = (uint32_t)p.BN;
-    const uint32_t tile_bytes = BN * (uint32_t)KC * 2u;        // one (slab, r, s) weight tile
-    // CTA class: which slice of the output channels this CTA computes (weights resident per slice)
-    const int split = (int)blockIdx.x % p.n_split, co_off = split * (int)BN;
-    const int item0 = (int)blockIdx.x / p.n_split, item_step = (int)gridDim.x / p.n_split;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < p.nslot; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&w_bar, 1);
-        for (int s = 0; s < R; s++) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], BN >= 32 ? 8u : 4u); }
-        fence_barrier_init();
-    }
-    if (warp == 0 && lane == 0) {
-        prefetch_tmap(&tmA);
-        if (p.C2) prefetch_tmap(&tmA2);
-        prefetch_tmap(&tmB);
-    }
-    if (warp == 1) {
-        tmem_alloc(&tmem_base_smem, (uint32_t)p.tmem_cols);
-        tmem_relinquish();
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            mbar_expect_tx(&w_bar, (uint32_t)p.w_bytes);
-            for (int sl = 0; sl < slabs; sl++)
-                for (int r = 0; r < KH; r++)
-                    for (int s = 0; s < KW; s++)
-                        tma_load_2d(smem + (size_t)((sl * KW + s) * KH + (KH - 1 - r)) * tile_bytes, &tmB, &w_bar, 0,
-                                    ((sl * KH + r) * KW + s) * p.cout_pad + co_off);
-            uint32_t cnt = 0;                                   // ring entries filled so far (all items)
-            for (int item = item0; item < p.n_items; item += item_step) {
-                const int tx = item % p.tiles_x, rest = item / p.tiles_x;
-                const int seg = rest % p.n_seg, n = rest / p.n_seg;
-                const int ya = seg * p.seg_h, yb = min(p.H, ya + p.seg_h);
-                const int x0 = tx * kRowTile;
-                for (int i = ya - ph; i < yb + ph; i++) {
-                    for (int sl = 0; sl < slabs; sl++, cnt++) {
-                        const int e = (int)(cnt % (uint32_t)p.nslot);
-                        const uint32_t phase = (cnt / (uint32_t)p.nslot) & 1u;
-                        mbar_wait(&empty_bar[e], phase ^ 1);
-                        mbar_expect_tx(&full_bar[e], (uint32_t)(PW * KC * 2));
-                        uint8_t *dst = ring + (size_t)e * p.slab_bytes;
-                        const int c = sl * KC;
-                        if (c < p.C1) tma_load_4d(dst, &tmA, &full_bar[e], c, x0 - pw, i, n);
-                        else tma_load_4d(dst, &tmA2, &full_bar[e], c - p.C1, x0 - pw, i, n);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer (converged warp, one elected lane) =====
-        const uint32_t leader = elect_one();
-        constexpr uint32_t swz = KC == 64 ? 2u : (KC == 32 ? 4u : 6u);
-        constexpr uint32_t rowb = (uint32_t)KC * 2u;
-        constexpr uint32_t sbo = 8u * rowb;
-        constexpr int ksteps = KC / 16;
-        const uint64_t dhi = make_smem_desc(0, swz, sbo);
-        const uint32_t lo_flags = (uint32_t)(dhi & 0xFFFF0000u);
-        const uint32_t w16 = (smem_u32(smem) >> 4) | lo_flags, ring16 = (smem_u32(ring) >> 4) | lo_flags;
-        const uint32_t slab16 = (uint32_t)p.slab_bytes >> 4, tile16 = tile_bytes >> 4;
-        const int nb_max = 256 / (int)BN;
-        mbar_wait(&w_bar, 0);
-        uint32_t cnt = 0;                                   // ring entries consumed so far
-        uint32_t orow = 0;                                  // output rows started before this item
-#ifdef STRIP2_DEBUG
-        long long t_acc = 0, t_full = 0, t_all = clock64();
-#endif
-        for (int item = item0; item < p.n_items; item += item_step) {
-            const int rest = item / p.tiles_x;
-            const int seg = rest % p.n_seg;
-            const int ya = seg * p.seg_h, yb = min(p.H, ya + p.seg_h);
             const int rows_out = yb - ya, rows_in = rows_out + 2 * ph;
-            for (int ii = 0; ii < rows_in; ii++) {
-                // input row ii of the item feeds output rows yl..yh (relative), filter row r = ii - yr
-                const int yl = max(0, ii - 2 * ph), yh = min(rows_out - 1, ii);
-                if (ii < rows_out) {                        // output row ii starts here: its slot must be drained
-                    const uint32_t g = orow + (uint32_t)ii;
-#ifdef STRIP2_DEBUG
-                    long long t0 = clock64();
-#endif
-                    mbar_wait(&acc_empty[g % (uint32_t)R], (g / (uint32_t)R) & 1u);
-#ifdef STRIP2_DEBUG
-                    t_acc += clock64() - t0;
-#endif
-                    tcgen05_fence_after();
-                }
-                // contiguous slot ranges of the stack (ring wrap, N <= 256)
-                uint32_t rd[4], rb[4], ri[4];
-                int nr = 0;
-                for (int yr = yl; yr <= yh && nr < 4;) {
-                    const int slot = (int)((orow + (uint32_t)yr) % (uint32_t)R);
-                    int nb = yh - yr + 1;
-                    nb = min(nb, min(R - slot, nb_max));
-                    rd[nr] = tmem_base + (uint32_t)slot * BN;
-                    rb[nr] = (uint32_t)(yr - ii + KH - 1) * tile16;
-                    ri[nr] = make_idesc_f16(kBM, nb * (int)BN);
-                    nr++;
-                    yr += nb;
-                }
-                for (int sl = 0; sl < slabs; sl++, cnt++) {
-                    const uint32_t e = cnt % (uint32_t)p.nslot;
-#ifdef STRIP2_DEBUG
-                    long long t1 = clock64();
-#endif
-                    mbar_wait(&full_bar[e], (cnt / (uint32_t)p.nslot) & 1u);
-#ifdef STRIP2_DEBUG
-                    t_full += clock64() - t1;
-#endif
-                    tcgen05_fence_after();
-                    const uint32_t a_lo = ring16 + e * slab16;
-                    const uint32_t b_sl = w16 + (uint32_t)(sl * KW * KH) * tile16;
+            rr.waited = 0; rr.released = 0;
+            for (int q = g; 2 * q < rows_out; q += 2) {
+                rr.release_upto(2 * q, lane);                   // rows only the other warpgroup needed
+                const int nrows = min(2, rows_out - 2 * q);
+                __half2 prev[2][2][BN / 8];
+                for (int k = 0; k < nrows; k++) {
+                    const int yr = 2 * q + k;                   // output row (relative to the item)
+                    rr.wait_upto(yr + KH);
+                    float acc[2][BN / 2];
+                    uint32_t first = 0;
+                    wgmma_fence();
+                    for (int r = 0; r < KH; r++) {
+                        const uint32_t a_row = rr.slot(yr + r) * row16;
+                        for (int sl = 0; sl < slabs; sl++) {
+                            const uint32_t a_lo = a_row + (uint32_t)sl * slab16;
+                            const uint32_t b_lo = (uint32_t)(sl * taps + r * KW) * tile16;
 #pragma unroll
-                    for (int s = 0; s < KW; s++) {
+                            for (int s = 0; s < KW; s++) {
 #pragma unroll
-                        for (int j = 0; j < ksteps; j++) {
-                            const uint64_t adesc = desc_with_lo(dhi, a_lo + (uint32_t)(s * (rowb >> 4) + 2 * j));
-                            const uint32_t b_lo = b_sl + (uint32_t)(s * KH) * tile16 + (uint32_t)(2 * j);
-#pragma unroll
-                            for (int k = 0; k < 4; k++)
-                                if (k < nr)
-                                    umma_f16_pred(rd[k], adesc, desc_with_lo(dhi, b_lo + rb[k]), ri[k], 1u, leader);
+                                for (int j = 0; j < ksteps; j++) {
+                                    const uint64_t bd = desc_add(dw, b_lo + (uint32_t)s * tile16 + 2u * j);
+                                    wgmma_f16<BN>(acc[0], desc_add(dr, a_lo + (uint32_t)s * rowb16 + 2u * j), bd, first);
+                                    wgmma_f16<BN>(acc[1], desc_add(dr, a_lo + half16 + (uint32_t)s * rowb16 + 2u * j), bd, first);
+                                    first = 1;
+                                }
+                            }
                         }
                     }
-                    umma_commit_pred(&empty_bar[e], leader);            // entry free once these MMAs retire
-                }
-                if (ii >= 2 * ph) {                         // output row ii-2ph just got its last filter row
-                    const uint32_t g = orow + (uint32_t)(ii - 2 * ph);
-                    umma_commit_pred(&acc_full[g % (uint32_t)R], leader);
-                }
-            }
-            orow += (uint32_t)rows_out;
-        }
-#ifdef STRIP2_DEBUG
-        if (lane == 0 && p.dbg) {
-            p.dbg[blockIdx.x * 4 + 0] = t_acc; p.dbg[blockIdx.x * 4 + 1] = t_full;
-            p.dbg[blockIdx.x * 4 + 2] = clock64() - t_all; p.dbg[blockIdx.x * 4 + 3] = orow;
-        }
-#endif
-    } else {
-        // ===== epilogue (warps 2..9). A warp reads TMEM lanes (warp % 4)*32..+31 = 32 pixels of the row; the two
-        // warps that share a lane group split the BN columns (BN = 16: the second group idles). One warp per
-        // scheduler cannot hide the ld -> math -> store chain within a row period of the stacked MMAs, so the
-        // epilogue is spread over eight warps and kept short: bias in registers, one tcgen05.ld per row, the
-        // output pointer advanced instead of recomputed. =====
-        const int q = warp & 3;
-        const int grp = (warp - 2) >> 2;                      // 0: warps 2..5, 1: warps 6..9
-        const int m = q * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        const uint32_t ncol = BN >= 32 ? BN / 2 : BN;         // columns of this warp: 8 (never), 16 or 32
-        const uint32_t col0 = (uint32_t)grp * ncol;
-        if (grp == 0 || BN >= 32) {
-            // all slots start zeroed and released
-            for (int s = 0; s < R; s++)
-                for (uint32_t c0 = 0; c0 < ncol; c0 += 16)
-                    tmem_st_zero_32x32b_x16(tmem_base + lane_addr + (uint32_t)s * BN + col0 + c0);
-            tmem_st_wait();
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0)
-                for (int s = 0; s < R; s++) mbar_arrive(&acc_empty[s]);
-            float bias_r[32];
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs(acc[0]);
+                    wgmma_fence_regs(acc[1]);
+                    if (k == nrows - 1) rr.release_upto(min(rows_in, 2 * q + 4), lane);   // next pair starts at 2q+4
+                    const int y = ya + yr;
 #pragma unroll
-            for (int j = 0; j < 32; j++) bias_r[j] = (uint32_t)j < ncol ? __ldg(p.bias + co_off + col0 + j) : 0.f;
-            const float slope = p.slope;
-            uint32_t orow = 0;
-            for (int item = item0; item < p.n_items; item += item_step) {
-                const int tx = item % p.tiles_x, rest = item / p.tiles_x;
-                const int seg = rest % p.n_seg, n = rest / p.n_seg;
-                const int ya = seg * p.seg_h, yb = min(p.H, ya + p.seg_h);
-                const int px = tx * kRowTile + m;
-                const bool inb = px < p.W;
-                const size_t pix0 = ((size_t)n * p.H + ya) * p.W + px;
-                __half *o16 = (__half *)p.out + pix0 * p.out_cstride + co_off + col0;
-                float *o32 = (float *)p.out + pix0 * 8;
-                const size_t step16 = (size_t)p.W * p.out_cstride, step32 = (size_t)p.W * 8;
-                // POOL: 2x2 average of the stored (fp16) activations: previous row kept in registers, the
-                // horizontal neighbour is the adjacent lane; segments start on even rows (host side)
-                __half2 prev[POOL ? 16 : 1];
-                __half *pl = nullptr;
-                size_t pstep = 0;
-                if (POOL) {
-                    pl = (__half *)p.pool_out + (((size_t)n * (p.H / 2) + ya / 2) * (p.W / 2) + px / 2) * p.pool_cstride + co_off + col0;
-                    pstep = (size_t)(p.W / 2) * p.pool_cstride;
-                }
-                uint32_t g = orow, slot = g % (uint32_t)R, par = (g / (uint32_t)R) & 1u;
-                for (int y = ya; y < yb; y++) {
-                    mbar_wait(&acc_full[slot], par);
-                    tcgen05_fence_after();
-                    const uint32_t tmem_acc = tmem_base + lane_addr + slot * BN + col0;
-                    uint32_t v[32];
-                    tmem_ld_32x32b_x16(tmem_acc, v);
-                    if (ncol == 32) tmem_ld_32x32b_x16(tmem_acc + 16, v + 16);
-                    tmem_ld_wait();
-                    tmem_st_zero_32x32b_x16(tmem_acc);
-                    if (ncol == 32) tmem_st_zero_32x32b_x16(tmem_acc + 16);
-                    if (inb || POOL) {
-                        if (p.out_mode == 0) {
+                    for (int hf = 0; hf < 2; hf++) {
 #pragma unroll
-                            for (int c0 = 0; c0 < 32; c0 += 16) {
-                                if ((uint32_t)c0 < ncol) {
-                                    __half2 h[8];
+                        for (int i = 0; i < 2; i++) {
+                            const int m = 64 * hf + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+                            const int px = tx * kRowTile + m;
+                            const bool inb = px < p.W;
+                            const size_t pix = ((size_t)n * p.H + y) * p.W + px;
+                            __half2 hv[BN / 8];
+                            epilogue_row<BN>(acc[hf], i, inb, pix, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
+                                             p.out_cstride, co_off, hv);
+                            if (POOL) {
+                                if (k == 0) {
 #pragma unroll
-                                    for (int j = 0; j < 8; j++) {
-                                        const float x0 = __uint_as_float(v[c0 + 2 * j]) + bias_r[c0 + 2 * j];
-                                        const float x1 = __uint_as_float(v[c0 + 2 * j + 1]) + bias_r[c0 + 2 * j + 1];
-                                        h[j] = __floats2half2_rn(fmaxf(x0, x0 * slope), fmaxf(x1, x1 * slope));
-                                    }
-                                    if (inb) {
-                                        uint4 *dst = (uint4 *)(o16 + c0);
-                                        dst[0] = *(uint4 *)&h[0];
-                                        dst[1] = *(uint4 *)&h[4];
-                                    }
-                                    if (POOL) {
-                                        if (((y - ya) & 1) == 0) {
+                                    for (int j = 0; j < BN / 8; j++) prev[hf][i][j] = hv[j];
+                                } else {
+                                    // 2x2 average of the stored (fp16) activations; pixel m+1 is the lane 4 apart
+                                    __half2 *pl = (__half2 *)((__half *)p.pool_out +
+                                        (((size_t)n * (p.H / 2) + y / 2) * (p.W / 2) + px / 2) * p.pool_cstride + co_off);
 #pragma unroll
-                                            for (int j = 0; j < 8; j++) prev[c0 / 2 + j] = h[j];
-                                        } else {
-                                            __half2 hp[8];
-#pragma unroll
-                                            for (int j = 0; j < 8; j++) {
-                                                const float2 a = __half22float2(h[j]), b = __half22float2(prev[c0 / 2 + j]);
-                                                float s0 = a.x + b.x, s1 = a.y + b.y;       // exact: fp16 values in float32
-                                                s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
-                                                s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
-                                                hp[j] = __floats2half2_rn(s0 * 0.25f, s1 * 0.25f);
-                                            }
-                                            if (inb && (lane & 1) == 0) {
-                                                uint4 *dst = (uint4 *)(pl + c0);
-                                                dst[0] = *(uint4 *)&hp[0];
-                                                dst[1] = *(uint4 *)&hp[4];
-                                            }
-                                        }
+                                    for (int j = 0; j < BN / 8; j++) {
+                                        const float2 a = __half22float2(hv[j]), b = __half22float2(prev[hf][i][j]);
+                                        float s0 = a.x + b.x, s1 = a.y + b.y;       // exact: fp16 values in float32
+                                        s0 += __shfl_xor_sync(0xffffffffu, s0, 4);
+                                        s1 += __shfl_xor_sync(0xffffffffu, s1, 4);
+                                        if (inb && (lane & 4) == 0)
+                                            pl[(8 * j + 2 * (lane & 3)) / 2] = __floats2half2_rn(s0 * 0.25f, s1 * 0.25f);
                                     }
                                 }
                             }
-                        } else if (grp == 0 && inb) {
-                            float f[8];
-#pragma unroll
-                            for (int j = 0; j < 8; j++) {
-                                const float x = __uint_as_float(v[j]) + bias_r[j];
-                                f[j] = fmaxf(x, x * slope);
-                            }
-                            float4 *dst = (float4 *)o32;
-                            dst[0] = make_float4(f[0], f[1], f[2], f[3]);
-                            dst[1] = make_float4(f[4], f[5], f[6], f[7]);
                         }
                     }
-                    if (POOL && ((y - ya) & 1)) pl += pstep;
-                    o16 += step16;
-                    o32 += step32;
-                    tmem_st_wait();
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[slot]);
-                    if (++slot == (uint32_t)R) { slot = 0; par ^= 1u; }
                 }
-                orow += (uint32_t)(yb - ya);
             }
+            rr.release_upto(rows_in, lane);
+            rr.cnt += (uint32_t)rows_in;
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
     }
 }
 
 // ---------------------------------------------------------------------------------------------
-// strip2up: conv3x3(bilinear_up2(L)) + bias + LeakyReLU without materialising the up-sampled tensor
-// (model.py:140-147: up.forward = interpolate(x, scale_factor=2, mode='bilinear') -> conv1 -> leaky_relu).
+// Fused up-sampling convolution: conv3x3(bilinear_up2(L)) + bias + LeakyReLU without materialising the
+// up-sampled tensor (model.py:140-147: up.forward = interpolate(x, scale_factor=2, mode='bilinear') -> conv1 ->
+// leaky_relu).
 //
 // The x2 bilinear up-sampling (align_corners=False) is linear and shift-invariant with period 2, so it folds
 // into the convolution: out[2m+py][2j+px] = sum_{a,b in -1..1} Wf[py][px][a][b] . L[m+a][j+b] -- four
 // phase-specific 3x3 filters over the LOW-resolution tensor (Wf = W combined with the 0.25/0.75 coefficients,
-// built in float32 on the host, scratch/fold_upsample.py checks the identity). Same MACs as the convolution
-// over the up-sampled tensor, a quarter of the input bytes, no upsample kernel. In the strip2 scheme a
-// low-resolution input row k feeds SIX output rows (2k-2 .. 2k+3), so the stack is N = 6*Cout = 192 columns
-// per MMA (better A reuse than the 3-row stack of the plain 3x3), and the two horizontal phases are two
-// M tiles over the same A windows with their own weights and their own accumulator ring (epilogue warp group
-// g drains phase g and writes pixels 2j+g). Only the 2-pixel frame of the image differs (bilinear clamping
-// and the conv's zero padding are not shift-invariant there); a small direct kernel rewrites it afterwards.
+// built in float32 on the host). Same MACs as the convolution over the up-sampled tensor, a quarter of the
+// input bytes, no upsample kernel. The kernel walks a strip of 128 low-resolution columns like the strip kernel:
+// a consumer warpgroup takes a pair of output rows (2m, 2m+1), both read low rows m-1..m+1, and each row is
+// two horizontal phases x two 64-pixel halves of wgmma tiles (N = Cout_pad = 32); phase px is written to
+// pixels 2j+px. Only the 2-pixel frame of the image differs (bilinear clamping and the conv's zero padding
+// are not shift-invariant there); a small direct kernel rewrites it afterwards.
+// Folded weight tiles: [slab][px][b][q][Cout_pad][64], q = py + 2*(1-a).
 // ---------------------------------------------------------------------------------------------
 constexpr int kUpBlocks = 6;
 
-__global__ void __launch_bounds__(kStrip2Threads)
-conv_strip2up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const StripParams p) {
-    constexpr int KC = 64, KW = 3;
+__global__ void __launch_bounds__(kStripThreads, 1)
+conv_up2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const StripParams p) {
+    constexpr int KC = 64, KW = 3, BN = 32;
+    constexpr int PW = kRowTile + KW - 1;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    __shared__ __align__(8) uint64_t full_bar[kMaxSlot], empty_bar[kMaxSlot], w_bar, acc_full[kMaxAcc], acc_empty[kMaxAcc];
-    __shared__ uint32_t tmem_base_smem;
+    uint8_t *smem = align1024(smem_raw);
+    __shared__ __align__(8) uint64_t full_bar[kMaxSlot], empty_bar[kMaxSlot], w_bar;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int slabs = p.C1 / KC;
-    constexpr int PW = kRowTile + KW - 1;
     uint8_t *ring = smem + ((p.w_bytes + 1023) & ~1023);
-    const int R = p.acc_slots;
-    const uint32_t BN = (uint32_t)p.BN;
-    const uint32_t tile_bytes = BN * (uint32_t)KC * 2u;
+    const uint32_t row_bytes = (uint32_t)p.slab_bytes * slabs;
     const int hl = p.H / 2, wl = p.W / 2;                     // low-resolution input size
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.nslot; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+        for (int s = 0; s < p.nslot; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
         mbar_init(&w_bar, 1);
-        for (int s = 0; s < R; s++) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-    if (warp == 1) {
-        tmem_alloc(&tmem_base_smem, (uint32_t)p.tmem_cols);
-        tmem_relinquish();
-    }
-    tcgen05_fence_before();
+    if (warp == kProducerWarp && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
 
-    if (warp == 0) {
-        // ===== TMA producer: folded weights (already in stack order), then low-resolution rows =====
+    if (warp == kProducerWarp) {
+        // ===== TMA producer: folded weights (already in tile order), then low-resolution rows =====
         if (lane == 0) {
             mbar_expect_tx(&w_bar, (uint32_t)p.w_bytes);
             for (int l = 0; l < p.w_loads; l++)
@@ -826,158 +435,84 @@ conv_strip2up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                 const int seg = rest % p.n_seg, n = rest / p.n_seg;
                 const int ka = seg * p.seg_h, kb = min(hl, ka + p.seg_h);
                 const int j0 = tx * kRowTile;
-                for (int k = ka - 1; k <= kb; k++) {
-                    for (int sl = 0; sl < slabs; sl++, cnt++) {
-                        const int e = (int)(cnt % (uint32_t)p.nslot);
-                        const uint32_t phase = (cnt / (uint32_t)p.nslot) & 1u;
-                        mbar_wait(&empty_bar[e], phase ^ 1);
-                        mbar_expect_tx(&full_bar[e], (uint32_t)(PW * KC * 2));
-                        tma_load_4d(ring + (size_t)e * p.slab_bytes, &tmA, &full_bar[e], sl * KC, j0 - 1, k, n);
-                    }
+                for (int k = ka - 1; k <= kb; k++, cnt++) {
+                    const int slot = (int)(cnt % (uint32_t)p.nslot);
+                    mbar_wait(&empty_bar[slot], ((cnt / (uint32_t)p.nslot) & 1u) ^ 1u);
+                    mbar_expect_tx(&full_bar[slot], (uint32_t)(PW * KC * 2 * slabs));
+                    for (int sl = 0; sl < slabs; sl++)
+                        tma_load_4d(ring + (size_t)slot * row_bytes + (size_t)sl * p.slab_bytes, &tmA, &full_bar[slot],
+                                    sl * KC, j0 - 1, k, n);
                 }
             }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        const uint32_t leader = elect_one();
-        constexpr uint32_t rowb = (uint32_t)KC * 2u, sbo = 8u * rowb;
-        constexpr int ksteps = KC / 16;
-        const uint64_t dhi = make_smem_desc(0, 2u, sbo);                  // SWIZZLE_128B
-        const uint32_t lo_flags = (uint32_t)(dhi & 0xFFFF0000u);
-        const uint32_t w16 = (smem_u32(smem) >> 4) | lo_flags, ring16 = (smem_u32(ring) >> 4) | lo_flags;
-        const uint32_t slab16 = (uint32_t)p.slab_bytes >> 4, tile16 = tile_bytes >> 4;
-        const uint32_t phase_cols = (uint32_t)R * BN;                     // accumulator ring of phase 1 starts here
-        mbar_wait(&w_bar, 0);
-        uint32_t cnt = 0, orow = 0;
-        for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-            const int rest = item / p.tiles_x;
-            const int seg = rest % p.n_seg;
-            const int ka = seg * p.seg_h, kb = min(hl, ka + p.seg_h);
-            const int rows_out = 2 * (kb - ka), rows_in = (kb - ka) + 2;
-            for (int ii = 0; ii < rows_in; ii++) {
-                // low row k = ka-1+ii feeds output rows (relative) 2ii-4+q, q = 0..5
-                for (int t = 0; t < 2; t++) {                             // output rows that start here
-                    const int yr = 2 * ii + t;
-                    if (yr < rows_out) {
-                        const uint32_t g = orow + (uint32_t)yr;
-                        mbar_wait(&acc_empty[g % (uint32_t)R], (g / (uint32_t)R) & 1u);
-                    }
-                }
-                tcgen05_fence_after();
-                const int q_lo = max(0, 4 - 2 * ii), q_hi = min(kUpBlocks - 1, rows_out + 3 - 2 * ii);
-                uint32_t rd[3], rb[3], ri[3];
-                int nr = 0;
-                for (int q = q_lo; q <= q_hi && nr < 3;) {
-                    const int yr = 2 * ii - 4 + q;
-                    const int slot = (int)((orow + (uint32_t)yr) % (uint32_t)R);
-                    const int nb = min(q_hi - q + 1, R - slot);
-                    rd[nr] = (uint32_t)slot * BN;
-                    rb[nr] = (uint32_t)q * tile16;
-                    ri[nr] = make_idesc_f16(kBM, nb * (int)BN);
-                    nr++;
-                    q += nb;
-                }
-                for (int sl = 0; sl < slabs; sl++, cnt++) {
-                    const uint32_t e = cnt % (uint32_t)p.nslot;
-                    mbar_wait(&full_bar[e], (cnt / (uint32_t)p.nslot) & 1u);
-                    tcgen05_fence_after();
-                    const uint32_t a_lo = ring16 + e * slab16;
-#pragma unroll
-                    for (int px = 0; px < 2; px++) {
-                        const uint32_t d0 = tmem_base + (uint32_t)px * phase_cols;
-#pragma unroll
-                        for (int b = 0; b < KW; b++) {
-                            const uint32_t b_tile = w16 + (uint32_t)(((sl * 2 + px) * KW + b) * kUpBlocks) * tile16;
-#pragma unroll
-                            for (int j = 0; j < ksteps; j++) {
-                                const uint64_t adesc = desc_with_lo(dhi, a_lo + (uint32_t)(b * (rowb >> 4) + 2 * j));
-#pragma unroll
-                                for (int k = 0; k < 3; k++)
-                                    if (k < nr)
-                                        umma_f16_pred(d0 + rd[k], adesc, desc_with_lo(dhi, b_tile + rb[k] + (uint32_t)(2 * j)),
-                                                      ri[k], 1u, leader);
-                            }
-                        }
-                    }
-                    umma_commit_pred(&empty_bar[e], leader);
-                }
-                for (int t = 0; t < 2; t++) {                             // output rows that just completed
-                    const int yr = 2 * ii - 4 + t;
-                    if (yr >= 0 && yr < rows_out) {
-                        const uint32_t g = orow + (uint32_t)yr;
-                        umma_commit_pred(&acc_full[g % (uint32_t)R], leader);
-                    }
-                }
-            }
-            orow += (uint32_t)rows_out;
         }
     } else {
-        // ===== epilogue: warps 2..5 drain horizontal phase 0 (even output columns), warps 6..9 phase 1 =====
-        const int q4 = warp & 3, px = (warp - 2) >> 2;
-        const int m = q4 * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(q4 * 32) << 16;
-        const uint32_t col0 = (uint32_t)px * (uint32_t)R * BN;
-        for (int s = 0; s < R; s++)
-            for (uint32_t c0 = 0; c0 < BN; c0 += 16) tmem_st_zero_32x32b_x16(tmem_base + lane_addr + col0 + (uint32_t)s * BN + c0);
-        tmem_st_wait();
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0)
-            for (int s = 0; s < R; s++) mbar_arrive(&acc_empty[s]);
-        float bias_r[32];
-#pragma unroll
-        for (int j = 0; j < 32; j++) bias_r[j] = __ldg(p.bias + j);
-        const float slope = p.slope;
-        uint32_t orow = 0;
+        // ===== consumer warpgroup g: output row pairs g, g+2, ... of an item =====
+        const int g = warp >> 2;
+        constexpr uint32_t sbo = 8u * KC * 2u, rowb16 = (KC * 2u) >> 4, half16 = (64u * KC * 2u) >> 4;
+        constexpr uint32_t tile16 = (BN * KC * 2u) >> 4;
+        const uint64_t dw = make_smem_desc(smem_u32(smem), swizzle_layout(KC), sbo);
+        const uint64_t dr = make_smem_desc(smem_u32(ring), swizzle_layout(KC), sbo);
+        const uint32_t row16 = row_bytes >> 4, slab16 = (uint32_t)p.slab_bytes >> 4;
+        mbar_wait(&w_bar, 0);
+        RowRing rr{full_bar, empty_bar, (uint32_t)p.nslot, 0u, 0, 0};
         for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
             const int tx = item % p.tiles_x, rest = item / p.tiles_x;
             const int seg = rest % p.n_seg, n = rest / p.n_seg;
             const int ka = seg * p.seg_h, kb = min(hl, ka + p.seg_h);
-            const int jl = tx * kRowTile + m;                             // low-resolution column of this thread
-            const bool inb = jl < wl;
-            const size_t pix0 = ((size_t)n * p.H + 2 * ka) * p.W + (size_t)(2 * jl + px);
-            __half *o16 = (__half *)p.out + pix0 * p.out_cstride;
-            const size_t step16 = (size_t)p.W * p.out_cstride;
-            uint32_t g = orow, slot = g % (uint32_t)R, par = (g / (uint32_t)R) & 1u;
-            for (int yr = 0; yr < 2 * (kb - ka); yr++) {
-                mbar_wait(&acc_full[slot], par);
-                tcgen05_fence_after();
-                const uint32_t tmem_acc = tmem_base + lane_addr + col0 + slot * BN;
-                uint32_t v[32];
-                tmem_ld_32x32b_x16(tmem_acc, v);
-                tmem_ld_32x32b_x16(tmem_acc + 16, v + 16);
-                tmem_ld_wait();
-                tmem_st_zero_32x32b_x16(tmem_acc);
-                tmem_st_zero_32x32b_x16(tmem_acc + 16);
-                if (inb) {
+            const int pairs = kb - ka, rows_in = pairs + 2;    // low rows ka-1 .. kb
+            rr.waited = 0; rr.released = 0;
+            for (int q = g; q < pairs; q += 2) {
+                rr.release_upto(q, lane);
+                rr.wait_upto(q + 3);                            // low rows ka-1+q .. ka+1+q
+                for (int py = 0; py < 2; py++) {
+                    float acc[2][2][BN / 2];                    // [px][64-pixel half]
+                    uint32_t first = 0;
+                    wgmma_fence();
+                    for (int t = 0; t < 3; t++) {
+                        const int qb = py + 2 * (2 - t);
+                        const uint32_t a_row = rr.slot(q + t) * row16;
+                        for (int sl = 0; sl < slabs; sl++) {
+                            const uint32_t a_lo = a_row + (uint32_t)sl * slab16;
 #pragma unroll
-                    for (int c0 = 0; c0 < 32; c0 += 16) {
-                        __half2 h[8];
+                            for (int b = 0; b < KW; b++) {
 #pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            const float x0 = __uint_as_float(v[c0 + 2 * j]) + bias_r[c0 + 2 * j];
-                            const float x1 = __uint_as_float(v[c0 + 2 * j + 1]) + bias_r[c0 + 2 * j + 1];
-                            h[j] = __floats2half2_rn(fmaxf(x0, x0 * slope), fmaxf(x1, x1 * slope));
+                                for (int j = 0; j < KC / 16; j++) {
+                                    const uint64_t a0 = desc_add(dr, a_lo + (uint32_t)b * rowb16 + 2u * j);
+                                    const uint64_t a1 = desc_add(dr, a_lo + half16 + (uint32_t)b * rowb16 + 2u * j);
+#pragma unroll
+                                    for (int px = 0; px < 2; px++) {
+                                        const uint64_t bd = desc_add(dw, (uint32_t)((((sl * 2 + px) * KW + b) * kUpBlocks + qb)) * tile16 + 2u * j);
+                                        wgmma_f16<BN>(acc[px][0], a0, bd, first);
+                                        wgmma_f16<BN>(acc[px][1], a1, bd, first);
+                                    }
+                                    first = 1;
+                                }
+                            }
                         }
-                        uint4 *dst = (uint4 *)(o16 + c0);
-                        dst[0] = *(uint4 *)&h[0];
-                        dst[1] = *(uint4 *)&h[4];
                     }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+#pragma unroll
+                    for (int px = 0; px < 2; px++) { wgmma_fence_regs(acc[px][0]); wgmma_fence_regs(acc[px][1]); }
+                    if (py == 1) rr.release_upto(min(rows_in, q + 2), lane);        // next pair starts at q+2
+                    const int y = 2 * (ka + q) + py;
+#pragma unroll
+                    for (int px = 0; px < 2; px++)
+#pragma unroll
+                        for (int hf = 0; hf < 2; hf++)
+#pragma unroll
+                            for (int i = 0; i < 2; i++) {
+                                const int jl = tx * kRowTile + 64 * hf + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+                                const size_t pix = ((size_t)n * p.H + y) * p.W + (size_t)(2 * jl + px);
+                                __half2 hv[BN / 8];
+                                epilogue_row<BN>(acc[px][hf], i, jl < wl, pix, lane, p.bias, p.slope, 0, p.out,
+                                                 p.out_cstride, 0, hv);
+                            }
                 }
-                o16 += step16;
-                tmem_st_wait();
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[slot]);
-                if (++slot == (uint32_t)R) { slot = 0; par ^= 1u; }
             }
-            orow += (uint32_t)(2 * (kb - ka));
+            rr.release_upto(rows_in, lane);
+            rr.cnt += (uint32_t)rows_in;
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
     }
 }
 
@@ -1130,36 +665,14 @@ int v2e_make_wgt_tmap(CUtensorMap *tm, const void *ptr, int Cout_pad, int Ktot, 
     return V2E_OK;
 }
 
-static int conv_use_mt2(long ctas) {
-    static int on = -1;
-    if (on < 0) { const char *e = getenv("V2E_CONV_MT2"); on = e ? atoi(e) : 1; }
-    if (!on) return 0;
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return ctas >= 2L * sms;
-}
 int v2e_conv_pick_kc(int C1, int C2) {
     int g = C2 ? (C1 < C2 ? C1 : C2) : C1;
     return g % 64 == 0 ? 64 : (g % 32 == 0 ? 32 : 16);
 }
 int v2e_conv_pick_bn(int Cout_pad) { return Cout_pad >= 128 ? 128 : Cout_pad; }
-// N = 256 tiles for the 256 / 512-channel layers: an A window (the shifted 8x16 input patch, re-fetched through L2 for
-// every filter tap) then feeds twice the math, 94 instead of 125 bytes per clock and SM from L2 at full tensor rate.
-// Two ring stages of 48 KB keep two CTAs per SM (and 2 x 256 TMEM columns). Only when the grid still fills the
-// machine: at least one full wave of 2 CTAs per SM. V2E_CONV_BN256=0 disables it (A/B measurements).
-static int conv_use_bn256(int Cout_pad, long tiles) {
-    static int on = -1;
-    if (on < 0) { const char *e = getenv("V2E_CONV_BN256"); on = e ? atoi(e) : 1; }
-    if (!on || Cout_pad % 256) return 0;
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return tiles * (Cout_pad / 256) >= 2L * sms;
-}
 
 struct V2eConvLaunch {
-    CUtensorMap tmA, tmA2, tmB, tmBh;
+    CUtensorMap tmA, tmA2, tmB;
     ConvParams p;
     dim3 grid;
     size_t smem;
@@ -1168,30 +681,16 @@ struct V2eConvLaunch {
 int v2e_conv_prepare(V2eConvLaunch *L, const void *x1, int C1, const void *x2, int C2, const void *wgt,
                      const float *bias, int Cout_pad, int KH, int KW, int N, int H, int W, void *out,
                      int out_cstride, int out_mode, int co_real, float slope) {
-    if (C1 % 16 || C2 % 16 || Cout_pad % 16 || (Cout_pad > 128 && Cout_pad % 128))
+    if (C1 % 16 || C2 % 16 || !(Cout_pad == 16 || Cout_pad == 32 || Cout_pad == 64 || (Cout_pad > 0 && Cout_pad % 128 == 0)))
         return v2e_set_error(V2E_E_INVALID, "conv: channel counts must be padded to 16 (Cout to 16/32/64/128k)%s", "");
     memset(L, 0, sizeof(*L));
     ConvParams &p = L->p;
     p.N = N; p.H = H; p.W = W; p.C1 = C1; p.C2 = C2; p.KH = KH; p.KW = KW;
     p.KC = v2e_conv_pick_kc(C1, C2);
     p.BN = v2e_conv_pick_bn(Cout_pad);
-    p.stages = 3;
-    p.MT = 1;
+    p.stages = kStages;
     p.tiles_x = (W + kTileW - 1) / kTileW;
     p.tiles_y = (H + kTileH - 1) / kTileH;
-    if (out_mode == 0 && conv_use_bn256(Cout_pad, (long)p.tiles_x * p.tiles_y * N)) { p.BN = 256; p.stages = 2; }
-    else if (out_mode == 0 && p.BN == 128 && p.KC == 64 &&
-             conv_use_mt2((long)p.tiles_x * ((p.tiles_y + 1) / 2) * N * (Cout_pad / 128))) {
-        // two vertically adjacent pixel tiles per CTA share every weight slab: the same 94 B/clk as the N = 256 tiles
-        p.MT = 2; p.stages = 2;
-        p.tiles_y = (p.tiles_y + 1) / 2;
-    }
-    {
-        // experiment (V2E_CONV_KC32=1): the 48 KB stages of the two variants above as four 24 KB stages of 32 channels
-        static int kc32 = -1;
-        if (kc32 < 0) { const char *e = getenv("V2E_CONV_KC32"); kc32 = e ? atoi(e) : 0; }
-        if (kc32 && p.stages == 2 && p.KC == 64) { p.KC = 32; p.stages = 4; }
-    }
     p.out_cstride = out_cstride; p.out_mode = out_mode; p.co_real = co_real; p.slope = slope;
     p.bias = bias; p.out = out;
     int rc;
@@ -1204,42 +703,29 @@ int v2e_conv_prepare(V2eConvLaunch *L, const void *x1, int C1, const void *x2, i
         if (co_fast < 0) { const char *e = getenv("V2E_CONV_CO_FAST"); co_fast = e ? atoi(e) : 1; }
         const unsigned tiles = (unsigned)(p.tiles_x * p.tiles_y * N), cob = (unsigned)(Cout_pad / p.BN);
         p.co_fast = (co_fast && cob > 1 && tiles <= 65535u) ? 1 : 0;
-        // clusters of two along the tile axis (weight-slab multicast): V2E_CONV_CLUSTER=1
-        static int cl = -1;
-        if (cl < 0) { const char *e = getenv("V2E_CONV_CLUSTER"); cl = e ? atoi(e) : 0; }
-        p.cl = (cl && p.BN >= 32 && (tiles + 1) / 2 * 2 <= 65534u && tiles >= 64) ? 1 : 0;
-        const unsigned tiles_l = p.cl ? (tiles + 1) / 2 * 2 : tiles;
-        L->grid = p.co_fast ? dim3(cob, tiles_l, 1) : dim3(tiles_l, cob, 1);
-        L->tmBh = L->tmB;
-        if (p.cl && (rc = v2e_make_wgt_tmap(&L->tmBh, wgt, Cout_pad, KH * KW * (C1 + C2), p.KC, p.BN / 2))) return rc;
+        L->grid = p.co_fast ? dim3(cob, tiles, 1) : dim3(tiles, cob, 1);
     }
-    size_t stage = (size_t)p.MT * kBM * p.KC * 2 + (((size_t)p.BN * p.KC * 2 + 1023) & ~(size_t)1023);
+    size_t stage = (size_t)kBM * p.KC * 2 + (((size_t)p.BN * p.KC * 2 + 1023) & ~(size_t)1023);
     L->smem = stage * p.stages + 1024;
     return V2E_OK;
 }
 
-int v2e_conv_launch(const V2eConvLaunch *L, cudaStream_t st) {
+template <int BN>
+static cudaError_t conv_launch_bn(const V2eConvLaunch *L, cudaStream_t st) {
     static PerDeviceOnce attr_once;
-    if (attr_once.first()) cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (attr_once.first()) cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    conv_tc_kernel<BN><<<L->grid, kConvThreads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p);
+    return cudaGetLastError();
+}
+
+int v2e_conv_launch(const V2eConvLaunch *L, cudaStream_t st) {
     cudaError_t e;
-    if (L->p.cl) {
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = L->grid;
-        cfg.blockDim = dim3(kConvThreads);
-        cfg.dynamicSmemBytes = L->smem;
-        cfg.stream = st;
-        cudaLaunchAttribute attr;
-        attr.id = cudaLaunchAttributeClusterDimension;
-        attr.val.clusterDim.x = L->p.co_fast ? 1 : 2;
-        attr.val.clusterDim.y = L->p.co_fast ? 2 : 1;
-        attr.val.clusterDim.z = 1;
-        cfg.attrs = &attr;
-        cfg.numAttrs = 1;
-        e = cudaLaunchKernelEx(&cfg, conv_tc_kernel, L->tmA, L->tmA2, L->tmB, L->tmBh, L->p);
-    } else {
-        conv_tc_kernel<<<L->grid, kConvThreads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->tmBh, L->p);
-        e = cudaGetLastError();
+    switch (L->p.BN) {
+        case 16: e = conv_launch_bn<16>(L, st); break;
+        case 32: e = conv_launch_bn<32>(L, st); break;
+        case 64: e = conv_launch_bn<64>(L, st); break;
+        case 128: e = conv_launch_bn<128>(L, st); break;
+        default: return v2e_set_error(V2E_E_UNSUPPORTED, "conv_tc_kernel: unsupported tile width%s", "");
     }
     if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "conv_tc_kernel launch: %s", cudaGetErrorString(e));
     return V2E_OK;
@@ -1282,32 +768,27 @@ static int make_rowseg_tmap(CUtensorMap *tm, const void *ptr, int N, int H, int 
     return V2E_OK;
 }
 
-// strip2 configuration of a layer: ring entries (one slab of one input row each), accumulator slots, TMEM
-// columns, CTAs per SM. Returns 0 when the layer does not fit (weights resident + >= 3 ring entries,
-// R >= KH+1 slots of BN columns).
-static int strip2_config(int C1, int C2, int Cout_pad, int KH, int KW, int kc, int *nslot, int *acc_slots,
-                         int *tmem_cols, int *ctas_per_sm, int *n_split) {
+// Shared memory of one CTA (227 KB on sm_90, 228 KB per SM): the whole budget, or half of it for two CTAs per SM.
+constexpr size_t kSmemFull = 222 * 1024, kSmemHalf = 110 * 1024;
+
+// Strip configuration of a layer: ring slots (one input row, all slabs, each), CTAs per SM, output-channel split.
+// Returns 0 when the layer does not fit (resident weights of a slice of >= 16 output channels + KH+1 ring rows:
+// the rows a pair of output rows reads). Two CTAs per SM when the weights and KH+3 rows (both warpgroups busy)
+// fit in half of the shared memory.
+static int strip_config(int C1, int C2, int Cout_pad, int KH, int KW, int kc, int *nslot, int *ctas_per_sm, int *n_split) {
     if (Cout_pad > 64) return 0;
     const int slabs = (C1 + C2) / kc;
-    const size_t slab = ((size_t)(kRowTile + KW - 1) * kc * 2 + 1023) & ~(size_t)1023;
-    const size_t half = 110 * 1024, full = 222 * 1024;
+    const size_t row = (((size_t)(kRowTile + KW - 1) * kc * 2 + 1023) & ~(size_t)1023) * slabs;
     for (int split = 1; split <= 2; split++) {
         const int bn = Cout_pad / split;
         if (bn < 16 || bn % 16) break;
         const size_t wb = ((size_t)slabs * KH * KW * bn * kc * 2 + 1023) & ~(size_t)1023;
-        int two = 0;
-        if (wb + 2048 + 4 * slab <= half && (KH + 1) * bn <= 256) two = 1;
-        const size_t budget = two ? half : full;
-        if (wb + 2048 + 3 * slab > budget) continue;
-        int ns = (int)((budget - wb - 2048) / slab);
+        const int two = wb + 2048 + (size_t)(KH + 3) * row <= kSmemHalf;
+        const size_t budget = two ? kSmemHalf : kSmemFull;
+        if (wb + 2048 + (size_t)(KH + 1) * row > budget) continue;
+        int ns = (int)((budget - wb - 2048) / row);
         if (ns > kMaxSlot) ns = kMaxSlot;
-        const int tmem_budget = two ? 256 : 512;
-        int R = tmem_budget / bn;
-        if (R > kMaxAcc) R = kMaxAcc;
-        if (R < KH + 1) continue;
-        int cols = 32;
-        while (cols < R * bn) cols <<= 1;
-        *nslot = ns; *acc_slots = R; *tmem_cols = cols; *ctas_per_sm = two ? 2 : 1; *n_split = split;
+        *nslot = ns; *ctas_per_sm = two ? 2 : 1; *n_split = split;
         return 1;
     }
     return 0;
@@ -1323,61 +804,29 @@ static int strip_min_w() {
     return v;
 }
 
-static int strip_variant_forced() {
-    static int v = -2;
-    if (v == -2) {
-        const char *e = getenv("V2E_STRIP_VARIANT");       // A/B measurements: 0 = per-tap MMAs, 1 = row-stacked
-        v = e ? atoi(e) : -1;
-    }
-    return v;
-}
-
-// Slab width and ring depth for the strip kernels; returns KC (0: layer does not qualify), *nslot_out.
+// Slab width for the strip kernel; returns KC (0: layer does not qualify), *nslot_out.
 int v2e_strip_pick(int C1, int C2, int Cout_pad, int KH, int KW, int W, int *nslot_out) {
     // wide layers only: narrow rows waste part of the last 128-pixel strip (320 = 2.5 strips) and the per-tap
     // kernel's 8x16 tiles take over. V2E_STRIP_MIN_W overrides the threshold for A/B measurements.
-    if (Cout_pad > 128 || W < strip_min_w() || (KW != 3 && KW != 5 && KW != 7)) return 0;
+    if (Cout_pad > 64 || KH != KW || W < strip_min_w() || (KW != 3 && KW != 5 && KW != 7)) return 0;
     const int g = C2 ? (C1 < C2 ? C1 : C2) : C1;
     const int kc = g % 64 == 0 ? 64 : (g % 32 == 0 ? 32 : 16);
-    const int slabs = (C1 + C2) / kc;
-    {
-        int ns, R, cols, cps, nsp;
-        if (strip_variant_forced() != 0 && strip2_config(C1, C2, Cout_pad, KH, KW, kc, &ns, &R, &cols, &cps, &nsp)) {
-            if (nslot_out) *nslot_out = ns;
-            return kc;
-        }
-        if (strip_variant_forced() == 1) return 0;
-    }
-    // the first strip kernel (per-tap MMAs) only pays on rows of at least four strips
-    if (W < 4 * kRowTile) return 0;
-    const size_t wb = ((size_t)slabs * KH * KW * Cout_pad * kc * 2 + 1023) & ~(size_t)1023;
-    const size_t slab = ((size_t)(kRowTile + KW - 1) * kc * 2 + 1023) & ~(size_t)1023;
-    // two CTAs per SM (two MMA issue streams, epilogues overlap) when weights + a (KH+2)-row ring fit in
-    // half of the shared memory; otherwise one CTA with as deep a ring as fits
-    const size_t half = 110 * 1024, full = 222 * 1024;
-    int nslot = 0;
-    if (Cout_pad <= 64 && wb + 2048 + (size_t)(KH + 1) * slab * slabs <= half) {   // TMEM: 2 CTAs x 4 accumulators
-        nslot = (int)((half - wb - 2048) / (slab * slabs));
-    } else {
-        if (wb + 2048 >= full) return 0;
-        nslot = (int)((full - wb - 2048) / (slab * slabs));
-    }
-    if (nslot > kMaxSlot) nslot = kMaxSlot;
-    if (nslot < KH + 1) return 0;
-    if (nslot_out) *nslot_out = nslot;
+    int ns, cps, nsp;
+    if (!strip_config(C1, C2, Cout_pad, KH, KW, kc, &ns, &cps, &nsp)) return 0;
+    if (nslot_out) *nslot_out = ns;
     return kc;
 }
 
 size_t v2e_strip_launch_size(void) { return sizeof(V2eStripLaunch); }
 
-// 1 when the layer's strip2 configuration has a pooled epilogue (conv_strip2_kernel<KW, KC, true>): one CTA per SM
+// 1 when the layer's strip configuration has a pooled epilogue (conv_strip_kernel<KW, KC, BN, true>): one CTA per SM
 // (the pooled variant keeps a row of activations in registers), even image size
 int v2e_strip_pool_supported(int C1, int C2, int Cout_pad, int KH, int KW, int H, int W) {
-    if (strip_variant_forced() == 0 || (H & 1) || (W & 1) || Cout_pad < 32) return 0;
+    if ((H & 1) || (W & 1) || Cout_pad < 32) return 0;
     const int KC = v2e_strip_pick(C1, C2, Cout_pad, KH, KW, W, nullptr);
     if (!((KW == 7 && KC == 32) || (KW == 5 && KC == 64))) return 0;
-    int ns, R, cols, cps, nsp;
-    if (!strip2_config(C1, C2, Cout_pad, KH, KW, KC, &ns, &R, &cols, &cps, &nsp)) return 0;
+    int ns, cps, nsp;
+    if (!strip_config(C1, C2, Cout_pad, KH, KW, KC, &ns, &cps, &nsp)) return 0;
     return cps == 1 && Cout_pad / nsp >= 32;
 }
 
@@ -1387,10 +836,12 @@ int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2,
                       int pool_cstride) {
     memset(L, 0, sizeof(*L));
     StripParams &p = L->p;
-    int nslot = 0;
-    const int KC = v2e_strip_pick(C1, C2, Cout_pad, KH, KW, W, &nslot);
-    if (!KC) return v2e_set_error(V2E_E_INVALID, "layer does not qualify for the strip kernel%s", "");
-    p.N = N; p.H = H; p.W = W; p.C1 = C1; p.C2 = C2; p.KH = KH; p.KW = KW; p.KC = KC; p.BN = Cout_pad;
+    const int KC = v2e_strip_pick(C1, C2, Cout_pad, KH, KW, W, nullptr);
+    int nslot = 0, ctas_per_sm = 0, n_split = 0;
+    if (!KC || !strip_config(C1, C2, Cout_pad, KH, KW, KC, &nslot, &ctas_per_sm, &n_split))
+        return v2e_set_error(V2E_E_INVALID, "layer does not qualify for the strip kernel%s", "");
+    p.N = N; p.H = H; p.W = W; p.C1 = C1; p.C2 = C2; p.KH = KH; p.KW = KW; p.KC = KC;
+    p.n_split = n_split; p.cout_pad = Cout_pad; p.BN = Cout_pad / n_split;
     p.tiles_x = (W + kRowTile - 1) / kRowTile;
     // segment height: enough items to balance the SMs (>= ~6 per SM), at least 4*KH rows per item
     int seg_h = H;
@@ -1398,7 +849,7 @@ int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2,
     while (seg_h > 4 * KH && (long)strips * ((H + seg_h - 1) / seg_h) < 6L * n_sms) seg_h = (seg_h + 1) / 2;
     if (pool_out) {
         if (out_mode != 0 || !v2e_strip_pool_supported(C1, C2, Cout_pad, KH, KW, H, W))
-            return v2e_set_error(V2E_E_UNSUPPORTED, "strip2: this layer has no pooled epilogue%s", "");
+            return v2e_set_error(V2E_E_UNSUPPORTED, "strip: this layer has no pooled epilogue%s", "");
         seg_h = (seg_h + 1) & ~1;                      // 2x2 windows never straddle two items
     }
     p.pool_out = pool_out;
@@ -1407,27 +858,9 @@ int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2,
     p.n_seg = (H + seg_h - 1) / seg_h;
     p.n_items = strips * p.n_seg;
     p.nslot = nslot;
-    int ctas_per_sm = 0;
-    {
-        int ns, R, cols, cps, nsp;
-        p.n_split = 1; p.cout_pad = Cout_pad;
-        // strip2's epilogue evaluates the LeakyReLU as max(x, slope*x): 0 <= slope <= 1
-        if (strip_variant_forced() != 0 && slope >= 0.f && slope <= 1.f &&
-            strip2_config(C1, C2, Cout_pad, KH, KW, KC, &ns, &R, &cols, &cps, &nsp)) {
-            p.variant = 1; p.nslot = ns; p.acc_slots = R; p.tmem_cols = cols; ctas_per_sm = cps;
-            p.n_split = nsp; p.BN = Cout_pad / nsp;
-        }
-    }
-    if (pool_out && p.variant != 1) return v2e_set_error(V2E_E_UNSUPPORTED, "strip2: pooled epilogue needs the row-stacked kernel%s", "");
     const int slabs = (C1 + C2) / KC, taps = KH * KW;
     p.slab_bytes = (int)(((size_t)(kRowTile + KW - 1) * KC * 2 + 1023) & ~(size_t)1023);
-    p.w_bytes = slabs * taps * p.BN * KC * 2;          // resident per CTA (strip2: its slice of the output channels)
-    int rows_total = slabs * taps * Cout_pad;
-    int rpl = 256;                                           // rows per weight load: largest divisor <= 256, multiple of 8
-    while ((rows_total % rpl) || (rpl % 8)) rpl--;
-    if (p.variant == 1) rpl = p.BN;                          // strip2 places every (slab, r, s) tile itself
-    p.w_rows_per_load = rpl;
-    p.w_loads = rows_total / rpl;
+    p.w_bytes = slabs * taps * p.BN * KC * 2;          // resident per CTA: its slice of the output channels
     p.out_cstride = out_cstride; p.out_mode = out_mode; p.co_real = co_real; p.slope = slope;
     p.bias = bias; p.out = out;
     int rc;
@@ -1435,87 +868,62 @@ int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2,
     if (C2) { if ((rc = make_rowseg_tmap(&L->tmA2, x2, N, H, W, C2, KC, KW))) return rc; }
     else L->tmA2 = L->tmA;
     {
+        // weights [slabs][taps][Cout_pad][KC]: one box per (slab, tap) tile of this CTA class's BN output channels
         EncodeTiledFn fn = encode_fn();
+        const int rows_total = slabs * taps * Cout_pad;
         cuuint64_t dims[2] = {(cuuint64_t)KC, (cuuint64_t)rows_total};
         cuuint64_t strides[1] = {(cuuint64_t)KC * 2};
-        cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)rpl};
+        cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)p.BN};
         cuuint32_t es[2] = {1, 1};
         CUresult r = fn(&L->tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)wgt_row, dims, strides, box, es,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return v2e_set_error(V2E_E_CUDA, "cuTensorMapEncodeTiled failed for strip weights%s", "");
     }
-    if (p.variant == 1) L->smem = (size_t)((p.w_bytes + 1023) & ~1023) + (size_t)p.nslot * p.slab_bytes + 1024;
-    else L->smem = (size_t)((p.w_bytes + 1023) & ~1023) + (size_t)nslot * p.slab_bytes * slabs + 1024;
-    const int ctas = p.variant == 1 ? ctas_per_sm * n_sms : ((L->smem + 1024 <= 113 * 1024) ? 2 * n_sms : n_sms);
-    L->grid = p.n_items < ctas ? p.n_items : ctas;
-    if (p.variant == 1 && p.n_split > 1) {                   // every CTA class walks all items
-        int per = ctas / p.n_split;
-        if (per > p.n_items) per = p.n_items;
-        if (per < 1) per = 1;
-        L->grid = per * p.n_split;
-    }
+    L->smem = (size_t)((p.w_bytes + 1023) & ~1023) + (size_t)p.nslot * p.slab_bytes * slabs + 1024;
+    // every CTA class walks all items
+    int per = ctas_per_sm * n_sms / p.n_split;
+    if (per > p.n_items) per = p.n_items;
+    if (per < 1) per = 1;
+    L->grid = per * p.n_split;
     return V2E_OK;
 }
 
-#ifdef STRIP2_DEBUG
-static long long *g_dbg = nullptr;
-extern "C" void v2e_strip2_debug_dump(void) {
-    if (!g_dbg) return;
-    std::vector<long long> h(4 * 1024);
-    cudaMemcpy(h.data(), g_dbg, h.size() * 8, cudaMemcpyDeviceToHost);
-    double a = 0, f = 0, t = 0; int n = 0;
-    for (int i = 0; i < 1024; i++) if (h[i * 4 + 2]) { a += h[i * 4]; f += h[i * 4 + 1]; t += h[i * 4 + 2]; n++; }
-    if (n) printf("strip2 issuer: %d CTAs, avg cycles total %.0f, wait acc_empty %.0f (%.1f%%), wait full %.0f (%.1f%%), rows/CTA %.0f\n",
-                  n, t / n, a / n, 100 * a / t, f / n, 100 * f / t, (double)h[3]);
-    cudaMemset(g_dbg, 0, h.size() * 8);
+template <int KW, int KC, int BN, bool POOL>
+static cudaError_t strip_launch_t(const V2eStripLaunch *L, cudaStream_t st) {
+    static PerDeviceOnce attr_once;
+    if (attr_once.first())
+        cudaFuncSetAttribute(conv_strip_kernel<KW, KC, BN, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    conv_strip_kernel<KW, KC, BN, POOL><<<L->grid, kStripThreads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p);
+    return cudaGetLastError();
 }
-#endif
-int v2e_strip_launch(const V2eStripLaunch *L0, cudaStream_t st) {
-    V2eStripLaunch Lc = *L0;
-    V2eStripLaunch *L = &Lc;
-#ifdef STRIP2_DEBUG
-    if (!g_dbg) { cudaMalloc((void **)&g_dbg, 4 * 1024 * 8); cudaMemset(g_dbg, 0, 4 * 1024 * 8); }
-    L->p.dbg = g_dbg;
-#endif
-#define STRIP_CASE(KW_, KC_)                                                                                  \
-    if (L->p.KW == KW_ && L->p.KC == KC_) {                                                                    \
-        static PerDeviceOnce attr_once;                                                                         \
-        if (attr_once.first()) {                                                                                \
-            cudaFuncSetAttribute(conv_strip_kernel<KW_, KC_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024); \
-            cudaFuncSetAttribute(conv_strip2_kernel<KW_, KC_, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024); \
-        }                                                                                                       \
-        if (L->p.variant == 1 && L->p.pool_out)                                                                 \
-            return v2e_set_error(V2E_E_UNSUPPORTED, "strip2: no pooled variant for this filter width / slab%s", ""); \
-        if (L->p.variant == 1)                                                                                  \
-            conv_strip2_kernel<KW_, KC_, false><<<L->grid, kStrip2Threads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p); \
-        else                                                                                                    \
-            conv_strip_kernel<KW_, KC_><<<L->grid, kStripThreads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p);  \
-        launched = true;                                                                                        \
+
+template <int KW, int KC>
+static int strip_launch_kc(const V2eStripLaunch *L, cudaStream_t st, cudaError_t *e) {
+    const StripParams &p = L->p;
+    if (p.KW != KW || p.KC != KC) return 0;
+    if (p.pool_out) {
+        // the two layers that are followed by the pool of a down block at full / half resolution (conv2, down1.conv2)
+        if constexpr ((KW == 7 && KC == 32) || (KW == 5 && KC == 64)) {
+            if (p.BN == 32) { *e = strip_launch_t<KW, KC, 32, true>(L, st); return 1; }
+            if (p.BN == 64) { *e = strip_launch_t<KW, KC, 64, true>(L, st); return 1; }
+        }
+        return 0;
     }
-    bool launched = false;
-    // the two layers that are followed by the pool of a down block at full / half resolution (conv2, down1.conv2)
-#define STRIP_POOL_CASE(KW_, KC_)                                                                              \
-    if (L->p.variant == 1 && L->p.pool_out && L->p.KW == KW_ && L->p.KC == KC_) {                              \
-        static PerDeviceOnce attrp_once;                                                                        \
-        if (attrp_once.first())                                                                                 \
-            cudaFuncSetAttribute(conv_strip2_kernel<KW_, KC_, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024); \
-        conv_strip2_kernel<KW_, KC_, true><<<L->grid, kStrip2Threads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p); \
-        launched = true;                                                                                        \
-    }
-    STRIP_POOL_CASE(7, 32) STRIP_POOL_CASE(5, 64)
-#undef STRIP_POOL_CASE
-    if (launched) {
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "conv_strip2_kernel launch: %s", cudaGetErrorString(e));
-        return V2E_OK;
-    }
-    STRIP_CASE(3, 16) STRIP_CASE(3, 32) STRIP_CASE(3, 64)
-    STRIP_CASE(5, 16) STRIP_CASE(5, 32) STRIP_CASE(5, 64)
-    STRIP_CASE(7, 16) STRIP_CASE(7, 32) STRIP_CASE(7, 64)
-#undef STRIP_CASE
-    if (!launched) return v2e_set_error(V2E_E_UNSUPPORTED, "strip kernel: unsupported filter width / slab%s", "");
-    cudaError_t e = cudaGetLastError();
+    if (p.BN == 16) { *e = strip_launch_t<KW, KC, 16, false>(L, st); return 1; }
+    if (p.BN == 32) { *e = strip_launch_t<KW, KC, 32, false>(L, st); return 1; }
+    if (p.BN == 64) { *e = strip_launch_t<KW, KC, 64, false>(L, st); return 1; }
+    return 0;
+}
+
+int v2e_strip_launch(const V2eStripLaunch *L, cudaStream_t st) {
+    cudaError_t e = cudaSuccess;
+    const int launched = strip_launch_kc<3, 16>(L, st, &e) || strip_launch_kc<3, 32>(L, st, &e) ||
+                         strip_launch_kc<3, 64>(L, st, &e) || strip_launch_kc<5, 16>(L, st, &e) ||
+                         strip_launch_kc<5, 32>(L, st, &e) || strip_launch_kc<5, 64>(L, st, &e) ||
+                         strip_launch_kc<7, 16>(L, st, &e) || strip_launch_kc<7, 32>(L, st, &e) ||
+                         strip_launch_kc<7, 64>(L, st, &e);
+    if (!launched) return v2e_set_error(V2E_E_UNSUPPORTED, "strip kernel: unsupported filter width / slab / pooled epilogue%s", "");
     if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "conv_strip_kernel launch: %s", cudaGetErrorString(e));
     return V2E_OK;
 }
@@ -1525,7 +933,7 @@ extern "C" int v2e_conv2d_lrelu_sm100_strip(const void *x1_dev, int C1, const vo
                                             int KW, int N, int H, int W, void *out_dev, int out_cstride,
                                             int out_mode, int co_real, float slope, void *stream) {
     V2eStripLaunch L;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int rc = v2e_strip_prepare(&L, x1_dev, C1, x2_dev, C2, wgt_row_dev, bias_dev, Cout_pad, KH, KW, N, H, W,
@@ -1535,7 +943,7 @@ extern "C" int v2e_conv2d_lrelu_sm100_strip(const void *x1_dev, int C1, const vo
 }
 
 
-// ---- fused up-sample + 3x3 convolution (strip2up) host side ---------------------------------------------
+// ---- fused up-sample + 3x3 convolution host side ------------------------------------------------------
 struct V2eUpLaunch {
     CUtensorMap tmA, tmB;
     StripParams p;
@@ -1546,15 +954,15 @@ struct V2eUpLaunch {
     int C;
 };
 
-// 64-channel slabs, Cout_pad = 32, folded weights resident: slabs * 36 tiles of 32 x 64 fp16
+// 64-channel slabs, Cout_pad = 32, folded weights resident: slabs * 36 tiles of 32 x 64 fp16, + 3 ring rows
 int v2e_conv_up2_supported(int C, int Cout_pad, int W_out) {
     if (C != 64 || Cout_pad != 32 || W_out % 2 || W_out < 2 * strip_min_w()) return 0;   // the frame kernel is written for C = 64
     const size_t wb = (size_t)(C / 64) * 2 * 3 * kUpBlocks * Cout_pad * 64 * 2;
     const size_t slab = ((size_t)(kRowTile + 2) * 64 * 2 + 1023) & ~(size_t)1023;
-    return wb + 2048 + 3 * slab <= 222 * 1024;
+    return wb + 2048 + 3 * slab * (C / 64) <= kSmemFull;
 }
 
-// Folds the x2 bilinear up-sampling into the 3x3 filter (see conv_strip2up_kernel). w: float32 [cout][cin][3][3]
+// Folds the x2 bilinear up-sampling into the 3x3 filter (see conv_up2_kernel). w: float32 [cout][cin][3][3]
 // (the reference's state_dict layout); out: fp16 [C_pad/64][2 px][3 b][6 q][Cout_pad][64], zero padded.
 extern "C" int v2e_conv_up2_fold_weights(const float *w, int cout, int cin, int Cout_pad, int C_pad, void *out_host) {
     if (!w || !out_host || C_pad % 64 || cin > C_pad || cout > Cout_pad) return v2e_set_error(V2E_E_INVALID, "bad argument%s", "");
@@ -1604,14 +1012,14 @@ int v2e_conv_up2_prepare(V2eUpLaunch *L, const void *x_low, int C, const void *w
     p.seg_h = seg_h;
     p.n_seg = (hl + seg_h - 1) / seg_h;
     p.n_items = strips * p.n_seg;
-    p.variant = 2; p.acc_slots = 8; p.tmem_cols = 512; p.n_split = 1; p.cout_pad = Cout_pad;
+    p.n_split = 1; p.cout_pad = Cout_pad;
     const int slabs = C / KC;
     p.slab_bytes = (int)(((size_t)(kRowTile + 2) * KC * 2 + 1023) & ~(size_t)1023);
     p.w_bytes = slabs * 2 * 3 * kUpBlocks * Cout_pad * KC * 2;
     const int rows_total = slabs * 2 * 3 * kUpBlocks * Cout_pad;
     p.w_rows_per_load = kUpBlocks * Cout_pad;                  // 192 rows: one (slab, px, b) stack per load
     p.w_loads = rows_total / p.w_rows_per_load;
-    int ns = (int)((222 * 1024 - (size_t)p.w_bytes - 2048) / p.slab_bytes);
+    int ns = (int)((kSmemFull - (size_t)p.w_bytes - 2048) / ((size_t)p.slab_bytes * slabs));
     if (ns > kMaxSlot) ns = kMaxSlot;
     if (ns < 3) return v2e_set_error(V2E_E_INVALID, "fused up-sampling convolution: weights leave no room for the input ring%s", "");
     p.nslot = ns;
@@ -1630,7 +1038,7 @@ int v2e_conv_up2_prepare(V2eUpLaunch *L, const void *x_low, int C, const void *w
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) return v2e_set_error(V2E_E_CUDA, "cuTensorMapEncodeTiled failed for folded weights%s", "");
     }
-    L->smem = (size_t)((p.w_bytes + 1023) & ~1023) + (size_t)p.nslot * p.slab_bytes + 1024;
+    L->smem = (size_t)((p.w_bytes + 1023) & ~1023) + (size_t)p.nslot * p.slab_bytes * slabs + 1024;
     L->grid = p.n_items < n_sms ? p.n_items : n_sms;
     L->low = (const __half *)x_low;
     L->w_plain = (const __half *)wgt_plain;
@@ -1640,8 +1048,8 @@ int v2e_conv_up2_prepare(V2eUpLaunch *L, const void *x_low, int C, const void *w
 
 int v2e_conv_up2_launch(const V2eUpLaunch *L, cudaStream_t st) {
     static PerDeviceOnce attr_once;
-    if (attr_once.first()) cudaFuncSetAttribute(conv_strip2up_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    conv_strip2up_kernel<<<L->grid, kStrip2Threads, L->smem, st>>>(L->tmA, L->tmB, L->p);
+    if (attr_once.first()) cudaFuncSetAttribute(conv_up2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    conv_up2_kernel<<<L->grid, kStripThreads, L->smem, st>>>(L->tmA, L->tmB, L->p);
     // the 2-pixel frame, where clamping / zero padding break the shift invariance the folding relies on
     const StripParams &p = L->p;
     static int skip_frame = -1;                                   // measurement only: time the main kernel alone
@@ -1663,7 +1071,7 @@ int v2e_conv_up2_launch(const V2eUpLaunch *L, cudaStream_t st) {
     else
         conv_up2_border_kernel<128, 4><<<L->grid * 4, 128, bsm, st>>>(L->low, L->w_plain, p.bias, (__half *)p.out, p.N, p.H, p.W, p.out_cstride, p.slope);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "conv_strip2up_kernel launch: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "conv_up2_kernel launch: %s", cudaGetErrorString(e));
     return V2E_OK;
 }
 
@@ -1671,7 +1079,7 @@ extern "C" int v2e_conv2d_up2_lrelu_sm100(const void *x_low_dev, int C, const vo
                                           const float *bias_dev, int Cout_pad, int N, int H_out, int W_out, void *out_dev,
                                           int out_cstride, float slope, void *stream) {
     V2eUpLaunch L;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int rc = v2e_conv_up2_prepare(&L, x_low_dev, C, wgt_fold_dev, wgt_plain_dev, bias_dev, Cout_pad, N, H_out, W_out, out_dev,

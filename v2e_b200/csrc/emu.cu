@@ -1,4 +1,4 @@
-// DVS pixel model for sm_100a -- hand-written CUDA behind the C ABI in include/v2e_b200.h.
+// DVS pixel model for sm_90a (H100) -- hand-written CUDA behind the C ABI in include/v2e_b200.h.
 //
 // Replaces (reference = SensorsINI/v2e, /root/reference):
 //   v2ecore/emulator.py:619-1022  EventEmulator.generate_events
@@ -2095,7 +2095,7 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
     {
         // one wave of the update kernel: 3 resident blocks per SM (2 stages x 28 KB of shared memory each),
         // every block the same number of 128-pixel units
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         d.n_blocks = 3 * sms;
@@ -2187,7 +2187,7 @@ extern "C" int v2e_emu_set_pr_noise(V2eEmu *h, const float *pr_randn_dev, const 
     return V2E_OK;
 }
 
-// one block per list segment while they are all co-resident (148 SMs x 8 blocks), grid-stride beyond
+// one block per list segment while they are all co-resident (132 SMs x 8 blocks on H100), grid-stride beyond
 static inline int list_grid(const EmuDev &d) { return d.n_blocks < 1184 ? d.n_blocks : 1184; }
 static inline int grid_for(const EmuDev &d) { return (d.n_pad / kVec + kThreads - 1) / kThreads; }
 
@@ -2277,7 +2277,7 @@ static size_t frame_elem(int dt) { return dt == V2E_U8 ? 1 : (dt == V2E_F32 ? 4 
 // One cooperative launch for Euler steps [s0, s1) (emu_csdvs_iter_kernel). Returns false when the device / occupancy
 // does not allow a cooperative grid (the per-step kernels are used then).
 static bool cs_launch_iter(V2eEmu *h, double alpha_p, float alpha_h, int s0, int s1, int sharded, int slot, cudaStream_t st) {
-    static int coop = -1, blocks_per_sm = 0, sms = 148;
+    static int coop = -1, blocks_per_sm = 0, sms = 132;
     if (coop < 0) {
         int dev = 0;
         cudaGetDevice(&dev);
@@ -2463,7 +2463,7 @@ static int fused_cfg() {
 template <typename S, bool FAST, int WARPS, int MINB>
 static void launch_fused_update_cfg(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, size_t sm,
                                     cudaStream_t st) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int blocks = sms * MINB;
@@ -3039,19 +3039,19 @@ extern "C" double *v2e_emu_cs_recv_dev(V2eEmu *h) { return h ? h->cs_recv : null
 extern "C" uint64_t *v2e_emu_cs_max_dev(V2eEmu *h) { return h ? (uint64_t *)h->d.cs_max : nullptr; }
 extern "C" int v2e_emu_cs_pack(V2eEmu *h, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
-    emu_csdvs_pack_kernel<<<148, 256, 0, (cudaStream_t)stream>>>(h->d, h->cs_send, h->cs_K);
+    emu_csdvs_pack_kernel<<<132, 256, 0, (cudaStream_t)stream>>>(h->d, h->cs_send, h->cs_K);
     CU(cudaGetLastError());
     return V2E_OK;
 }
 extern "C" int v2e_emu_cs_unpack(V2eEmu *h, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
-    emu_csdvs_unpack_kernel<<<148, 256, 0, (cudaStream_t)stream>>>(h->d, h->cs_recv, h->cs_recv + (size_t)h->cs_K * h->d.W, h->cs_K);
+    emu_csdvs_unpack_kernel<<<132, 256, 0, (cudaStream_t)stream>>>(h->d, h->cs_recv, h->cs_recv + (size_t)h->cs_K * h->d.W, h->cs_K);
     CU(cudaGetLastError());
     return V2E_OK;
 }
 extern "C" int v2e_emu_cs_unpack_from(V2eEmu *h, const double *rows_above_dev, const double *rows_below_dev, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
-    emu_csdvs_unpack_kernel<<<148, 256, 0, (cudaStream_t)stream>>>(h->d, rows_above_dev, rows_below_dev, h->cs_K);
+    emu_csdvs_unpack_kernel<<<132, 256, 0, (cudaStream_t)stream>>>(h->d, rows_above_dev, rows_below_dev, h->cs_K);
     CU(cudaGetLastError());
     return V2E_OK;
 }

@@ -1,4 +1,4 @@
-// Stage-1 input preparation for sm_100a (SURVEY.md 8f rank 2): v2e.py:687-737 --
+// Stage-1 input preparation for sm_90a (H100) (SURVEY.md 8f rank 2): v2e.py:687-737 --
 //     frame[c_t:c_b, c_l:c_r] -> cv2.resize(dsize, interpolation=cv2.INTER_AREA) -> cv2.cvtColor(BGR2GRAY)
 // for 8-bit frames, bit-exact with OpenCV 4.x (restated in oracle/prep_oracle.py, pinned against cv2's own output):
 //   * integer scale factors (resize.cpp, resizeAreaFast_Invoker): integer box sum * float32(1/area), rounded half to

@@ -1,4 +1,4 @@
-// DVS frame rendering for sm_100a (SURVEY.md 8f rank 4): the histogram part of the reference's
+// DVS frame rendering for sm_90a (H100) (SURVEY.md 8f rank 4): the histogram part of the reference's
 // EventRenderer.render_events_to_frames (v2ecore/renderer.py:161-430 -> accumulate_event_frame :392-430 ->
 // hist2d_numba_seq, v2ecore/v2e_utils.py:474-486): per output frame, ON count minus OFF count per pixel of the events
 // of the frame's slice, clipped to +-full_scale_count, returned as (frame + fs) / (2 fs) in float64 (and, for the

@@ -1,4 +1,4 @@
-// SuperSloMo frame interpolation for sm_100a: everything of v2ecore/slomo.py:330-444 and
+// SuperSloMo frame interpolation for sm_90a (H100): everything of v2ecore/slomo.py:330-444 and
 // v2ecore/model.py:158-300 that runs per frame pair, behind the C ABI in include/v2e_b200.h.
 //
 //   set_pairs : uint8 frames (net resolution) -> normalised fp32 images (slomo.py:148-162: x/255 - 0.428)
@@ -6,7 +6,7 @@
 //   interp(t) : flow coefficients, two back-warps, 12-channel input (slomo.py:405-419)
 //               -> interpolation UNet(12,5) -> residual flows, visibility, two back-warps, blend
 //               (slomo.py:421-433) -> (x+0.428)*255 -> uint8 truncation (slomo.py:437, torchvision ToPILImage)
-// UNet convolutions: conv_tc.cu (tcgen05 implicit GEMM, fp16 operands, fp32 accumulate). avg_pool2d
+// UNet convolutions: conv_tc.cu (wgmma implicit GEMM, fp16 operands, fp32 accumulate). avg_pool2d
 // (model.py:72) and bilinear x2 (model.py:137-140) are NHWC fp16 streaming kernels here; the channel
 // concat of the up-blocks (model.py:150-153) is never materialised (the conv reads two tensors).
 // Also here: Pillow-exact 8-bit resampling (dataloader.py:142 LANCZOS, slomo.py:438 BILINEAR).
@@ -339,7 +339,7 @@ struct UNet {
     __half *w[23];
     __half *w_row[23];           // [slabs][taps][Cout_pad][KC] for layers that run on the strip kernel
     int row_kc[23];              // slab width of the strip kernel; 0: per-tap kernel
-    __half *w_fold[23];          // up-block conv1 with the x2 bilinear up-sampling folded in (strip2up), or null
+    __half *w_fold[23];          // up-block conv1 with the x2 bilinear up-sampling folded in (conv_up2_kernel), or null
     float *b[23];
     int cout_pad[23], c1p[23], c2p[23];
 };
@@ -480,7 +480,7 @@ extern "C" int v2e_slomo_create(int H, int W, int max_batch, const V2eUNetWeight
     CU(cudaMemset(h->nonfinite, 0, sizeof(int)));
     h->launch_mem.resize(v2e_conv_launch_size());
     h->row_mem.resize(v2e_strip_launch_size());
-    { int dev = 0; cudaGetDevice(&dev); h->n_sms = 148; cudaDeviceGetAttribute(&h->n_sms, cudaDevAttrMultiProcessorCount, dev); }
+    { int dev = 0; cudaGetDevice(&dev); h->n_sms = 132; cudaDeviceGetAttribute(&h->n_sms, cudaDevAttrMultiProcessorCount, dev); }
     h->force_tap_kernel = 0;
     h->no_fused_up = getenv("V2E_NO_FUSED_UP") ? 1 : 0;        // A/B measurements
     h->no_fused_pool = getenv("V2E_NO_FUSED_POOL") ? 1 : 0;

@@ -1,6 +1,6 @@
-// Inline-PTX wrappers for the Blackwell async machinery used by conv_tc.cu:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), descriptors.
-// Bit layouts follow cute/arch/mma_sm100_desc.hpp (SmemDescriptor, InstrDescriptor).
+// Inline-PTX wrappers for the Hopper async machinery used by conv_tc.cu:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors).
+// The descriptor layout is the sm_90 matrix descriptor of the PTX ISA (wgmma "Matrix Descriptor Format").
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -46,112 +46,77 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *tm, ui
         ::"r"(smem_u32(dst)), "l"((uint64_t)tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 
-// ---- thread-block clusters: TMA multicast and cross-CTA barrier arrival ----------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// the box lands at the same CTA-relative offset in every CTA of `mask`, and completes `bar` (same offset) in each
-__device__ __forceinline__ void tma_load_2d_multicast(void *dst, const CUtensorMap *tm, uint64_t *bar, int c0, int c1, uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(dst)), "l"((uint64_t)tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
-}
-
-// ---- tcgen05 -------------------------------------------------------------------------------------
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// whole warp; ncols power of two >= 32; result (TMEM base address) is written to *dst_smem
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], one thread issues for the CTA
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"((uint32_t)accumulate) : "memory");
-}
-// Predicated forms for a converged warp: every lane executes the (warp-uniform) surrounding code so that
-// descriptors live in uniform registers; only the lane with `leader != 0` issues. This keeps the issue
-// loop at a few instructions per MMA (a single-lane `if` makes the compiler wrap every UTCHMMA in an
-// ELECT / BRA.U.ANY loop and compute descriptors in the vector datapath).
+// 1 in exactly one lane of a converged warp
 __device__ __forceinline__ uint32_t elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred;
 }
-__device__ __forceinline__ void umma_f16_pred(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate, uint32_t leader) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "setp.ne.b32 q, %5, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(leader) : "memory");
-}
-__device__ __forceinline__ void umma_commit_pred(uint64_t *bar, uint32_t leader) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %1, 0;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-        ::"r"(smem_u32(bar)), "r"(leader) : "memory");
-}
-// arrives on `bar` (same CTA-relative offset) in every CTA of `mask` once this thread's MMAs have retired
-__device__ __forceinline__ void umma_commit_mc_pred(uint64_t *bar, uint16_t mask, uint32_t leader) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-        ::"r"(smem_u32(bar)), "h"(mask), "r"(leader) : "memory");
-}
-__device__ __forceinline__ uint64_t desc_with_lo(uint64_t hi_part, uint32_t lo) {
-    return (hi_part & 0xFFFFFFFF00000000ull) | (uint64_t)lo;
-}
-// arrives on the mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns: thread i of the warp gets lane (base_lane + i)
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t v[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// 32 lanes x 16 consecutive 32-bit columns set to zero (thread i of the warp writes lane base_lane + i)
-__device__ __forceinline__ void tmem_st_zero_32x32b_x16(uint32_t taddr) {
-    const uint32_t z = 0u;
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-        ::"r"(taddr), "r"(z) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// K-major operand tile in shared memory, rows of (swizzle-span) bytes, 8-row groups `sbo_bytes` apart.
-// layout_type: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B (cute::UMMA::LayoutType)
+// ---- wgmma ---------------------------------------------------------------------------------------
+// A warpgroup (4 consecutive warps, the first a multiple of 4) issues D[64 x N] (+)= A[64 x 16] * B[N x 16]^T with
+// both operands K-major in shared memory and D in registers: thread t of the warpgroup holds rows
+// 16*(t/32) + (t%32)/4 + 8*i and columns 8*j + 2*(t%4) + k in d[4*j + 2*i + k] (i, k in {0, 1}).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d) : "memory");
+}
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d) : "memory");
+}
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d) : "memory");
+}
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (N == 16) wgmma_m64n16k16(d, adesc, bdesc, scale_d);
+    else if constexpr (N == 32) wgmma_m64n32k16(d, adesc, bdesc, scale_d);
+    else if constexpr (N == 64) wgmma_m64n64k16(d, adesc, bdesc, scale_d);
+    else wgmma_m64n128k16(d, adesc, bdesc, scale_d);
+}
+
+// K-major operand tile in shared memory as TMA writes it with the matching swizzle: rows of `row_bytes`
+// (= the swizzle span: 128 / 64 / 32 B for 64 / 32 / 16 fp16 channels), 8-row groups 8*row_bytes apart.
+// The swizzle is a function of the shared-memory address, so a start address moved by whole rows (a filter
+// tap's pixel shift) or by 32 bytes (the next 16 channels) addresses the same data.
+// layout_type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
+__device__ __forceinline__ uint32_t swizzle_layout(int kc) { return kc == 64 ? 1u : (kc == 32 ? 2u : 3u); }
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t layout_type, uint32_t sbo_bytes) {
     uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);            // start_address  [0,14)
-    d |= (uint64_t)1 << 16;                                  // leading_byte_offset = 1 (unused, swizzled K-major)
+    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);            // start_address [0,14)
+    d |= (uint64_t)1 << 16;                                  // leading_byte_offset (unused, swizzled K-major)
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;       // stride_byte_offset [32,46)
-    d |= (uint64_t)1 << 46;                                  // version = 1 (Blackwell)
-    d |= (uint64_t)layout_type << 61;                        // layout_type [61,64)
+    d |= (uint64_t)layout_type << 62;                        // layout_type [62,64)
     return d;
 }
-// kind::f16, A/B fp16 K-major, fp32 accumulate
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(int M, int N) {
-    return (1u << 4)                       // c_format = F32
-         | (0u << 7) | (0u << 10)          // a_format = b_format = F16
-         | ((uint32_t)(N >> 3) << 17)      // n_dim
-         | ((uint32_t)(M >> 4) << 24);     // m_dim
-}
+// the descriptor with its start address (bits 0..13, 16-byte units) advanced by `add16`
+__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t add16) { return d + (uint64_t)add16; }

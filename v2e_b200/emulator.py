@@ -1,4 +1,4 @@
-"""EventEmulator -- drop-in for v2ecore/emulator.py:35 backed by the sm_100a kernels.
+"""EventEmulator -- drop-in for v2ecore/emulator.py:35 backed by the sm_90a (H100) kernels.
 
 Same constructor keywords, `generate_events(new_frame, t_frame)` contract, counters and state
 attribute names as the reference (emulator.py:86-117, 619-1022; SURVEY.md 8b). Host code here is

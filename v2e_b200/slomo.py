@@ -1,4 +1,4 @@
-"""SuperSloMo -- drop-in for v2ecore/slomo.py:37 backed by the sm_100a kernels.
+"""SuperSloMo -- drop-in for v2ecore/slomo.py:37 backed by the sm_90a (H100) kernels.
 
 Same constructor and `interpolate(source_frame_path, output_folder, frame_size)` contract as the
 reference (slomo.py:44-54, 231-495): reads `*.npy` luma frames from a folder, writes `<index>.png`
