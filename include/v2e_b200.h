@@ -361,6 +361,27 @@ int v2e_slomo_profile_read_layers(V2eSlomo *h, float *ms23, int *launches23, dou
 /* device pointers of the last flow / interpolation network outputs, fp32 [B][H][W][8] */
 const float *v2e_slomo_flow_ptr(V2eSlomo *h);
 const float *v2e_slomo_intrp_ptr(V2eSlomo *h);
+/* Test hooks: read-only views of the engine's internals, for checking every layer in its production
+ * configuration. Neither adds a launch or a synchronisation to set_pairs / interp.
+ * v2e_slomo_buffer_ptr: device pointer of an activation buffer (NHWC fp16, sized for max_batch; img: fp32
+ * [B+1][H][W]). index selects the level l (0..4, 1/2^(l+1) resolution) of pool / da / s and the up block k
+ * (0..4, 1/2^(4-k) resolution) of up / ua / ub; it is ignored otherwise. The flow and interpolation networks share
+ * the buffers, and up[k] is left stale when up block k ran the fused up-sampling convolution. NULL: unknown name. */
+typedef enum V2eSlomoBuffer {
+    V2E_SLOMO_BUF_IN16 = 0, V2E_SLOMO_BUF_X0 = 1, V2E_SLOMO_BUF_S1 = 2, V2E_SLOMO_BUF_POOL = 3, V2E_SLOMO_BUF_DA = 4,
+    V2E_SLOMO_BUF_S = 5, V2E_SLOMO_BUF_UP = 6, V2E_SLOMO_BUF_UA = 7, V2E_SLOMO_BUF_UB = 8, V2E_SLOMO_BUF_IMG = 9
+} V2eSlomoBuffer;
+void *v2e_slomo_buffer_ptr(V2eSlomo *h, int which, int index);
+/* Which kernel computed layer 0..22 (forward order of V2eUNetWeights) of net 0 (flow) / 1 (interpolation) in its
+ * last forward pass, as launched (options and V2E_NO_FUSED_* overrides applied). < 0: bad argument. */
+typedef enum V2eSlomoKernel {
+    V2E_SLOMO_KERNEL_NONE = 0,        /* not run yet */
+    V2E_SLOMO_KERNEL_TAP = 1,         /* per-tap implicit GEMM (v2e_conv2d_lrelu_sm100) */
+    V2E_SLOMO_KERNEL_STRIP = 2,       /* strip kernel (v2e_conv2d_lrelu_sm100_strip) */
+    V2E_SLOMO_KERNEL_STRIP_POOL = 3,  /* strip kernel writing the following 2x2 average pool from its epilogue */
+    V2E_SLOMO_KERNEL_UP2 = 4          /* fused x2 bilinear up-sampling convolution (v2e_conv2d_up2_lrelu_sm100) */
+} V2eSlomoKernel;
+int v2e_slomo_layer_kernel(V2eSlomo *h, int net, int layer);
 
 /* Pillow-exact 8-bit resampling of 'L' images (Pillow Resample.c; dataloader.py:142 uses LANCZOS,
  * slomo.py:438 BILINEAR). filter: 0 = BILINEAR, 1 = LANCZOS. Images are [n][h][w] uint8. */

@@ -58,6 +58,59 @@ class TapeRNG:
         return self.pos == len(self.tape)
 
 
+# ---- float64 references of the SuperSloMo convolutions and their error bars -----------------------------------
+# The convolution kernels multiply fp16 operands exactly and accumulate in fp32; fp16 outputs are then rounded once.
+# Against conv2d evaluated in float64 on the SAME fp16 operands the error of an output is therefore at most
+#   fp16 output rounding   <= ulp16(ref) / 2
+#   fp32 accumulation      <= (number of fp32 additions) * 2^-24 * (running |partial sum|) <= K * 2^-24 * S in the
+#                             worst case, S = conv2d(|x|, |w|) + |b|. The tensor cores add K = 16 products per step with
+#                             wider internal precision and the running sums cancel (|sum| << S), so in practice the
+#                             error is ~2^-20 S; 2^-16 * S keeps a large margin and is still far below the cost of
+#                             dropping one product out of K <= 9216 (~S / K >= 2^-13.2 * S).
+# LeakyReLU is 1-Lipschitz, so the same bar holds after the activation. The fp32 network heads are not rounded to
+# fp16: their bar is the accumulation term alone.
+SLOPE = float(np.float32(0.1))     # the kernels' LeakyReLU slope: 0.1 rounded to float32
+ACC_BAR = 2.0 ** -16
+
+
+def ulp16(x):
+    """Spacing of fp16 numbers at |x| (float64 tensor); 2^-24 in fp16's subnormal range."""
+    _, e = torch.frexp(x.abs().clamp_min(2.0 ** -14))      # |x| = m * 2^e, m in [0.5, 1)
+    return torch.ldexp(torch.ones_like(x), (e - 11).to(torch.int32))
+
+
+def ulp32(x):
+    """Spacing of float32 numbers at |x| (float64 tensor)."""
+    _, e = torch.frexp(x.abs().clamp_min(2.0 ** -126))
+    return torch.ldexp(torch.ones_like(x), (e - 24).to(torch.int32))
+
+
+def conv_ref64(x, w, b, pad, slope=SLOPE, drop_channel=None, drop_tap=None):
+    """lrelu(conv2d(x, w, b)) in float64 and S = conv2d(|x|, |w|) + |b|. x: [N, C, H, W], w: [Co, C, K, K] (both already
+    rounded to the operand precision), b: [Co]. drop_channel / drop_tap remove one input channel / one filter tap (r, s)
+    from the reference only: the perturbations that must make a comparison fail."""
+    x64, w64, b64 = x.double(), w.double(), b.double()
+    wr = w64.clone()
+    if drop_channel is not None:
+        wr[:, drop_channel] = 0
+    if drop_tap is not None:
+        wr[:, :, drop_tap[0], drop_tap[1]] = 0
+    ref = torch.nn.functional.leaky_relu(torch.nn.functional.conv2d(x64, wr, b64, padding=pad), slope)
+    S = torch.nn.functional.conv2d(x64.abs(), w64.abs(), padding=pad) + b64.abs().view(1, -1, 1, 1)
+    return ref, S
+
+
+def conv_bound(ref, S, fp16_out=True, acc=ACC_BAR):
+    """Largest |got - ref| the arithmetic allows (see above): ulp16(ref) + acc * S, or acc * S for fp32 outputs."""
+    return (ulp16(ref) if fp16_out else 0.0) + acc * S
+
+
+def err_ratio(got, ref, bound):
+    """max |got - ref| / bound (nan / inf in got count as failures)."""
+    r = (got.double() - ref).abs() / bound
+    return float("inf") if not torch.isfinite(r).all() else r.max().item()
+
+
 def split_events(events, counts):
     off = np.concatenate([[0], np.cumsum(counts)])
     return [events[off[i]:off[i + 1]] for i in range(len(counts))]

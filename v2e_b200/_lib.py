@@ -108,6 +108,8 @@ _SIGS = {
                                            ctypes.POINTER(_i), ctypes.POINTER(ctypes.c_double), _vp]),
     "v2e_slomo_flow_ptr": (_vp, [_vp]),
     "v2e_slomo_intrp_ptr": (_vp, [_vp]),
+    "v2e_slomo_buffer_ptr": (_vp, [_vp, _i, _i]),
+    "v2e_slomo_layer_kernel": (_i, [_vp, _i, _i]),
     "v2e_resize_create": (_i, [_i, _i, _i, _i, _i, _i, ctypes.POINTER(_vp)]),
     "v2e_resize_destroy": (_i, [_vp]),
     "v2e_resize_run": (_i, [_vp, _vp, _vp, _i, _vp]),

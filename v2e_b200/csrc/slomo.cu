@@ -377,6 +377,7 @@ struct V2eSlomo {
     int curB;
     std::vector<char> launch_mem, row_mem, up_mem;
     int n_sms, force_tap_kernel, no_fused_up, no_fused_pool;
+    int8_t ran[2][23];            // [flow, interp][layer]: V2E_SLOMO_KERNEL_* of the last launch (test hook)
     // measurement hooks: CUDA events around every conv launch
     int profile;
     std::vector<cudaEvent_t> ev;
@@ -485,6 +486,7 @@ extern "C" int v2e_slomo_create(int H, int W, int max_batch, const V2eUNetWeight
     h->no_fused_up = getenv("V2E_NO_FUSED_UP") ? 1 : 0;        // A/B measurements
     h->no_fused_pool = getenv("V2E_NO_FUSED_POOL") ? 1 : 0;
     h->up_mem.resize(v2e_conv_up2_launch_size());
+    memset(h->ran, V2E_SLOMO_KERNEL_NONE, sizeof(h->ran));
     *out = h;
     return V2E_OK;
 }
@@ -511,6 +513,8 @@ static int conv(V2eSlomo *h, const UNet &u, int li, const __half *x1, const __ha
     const bool row = u.row_kc[li] != 0 && !h->force_tap_kernel;
     V2eConvLaunch *L = (V2eConvLaunch *)h->launch_mem.data();
     V2eStripLaunch *R = (V2eStripLaunch *)h->row_mem.data();
+    h->ran[&u == &h->interp][li] = row ? (pool_out ? V2E_SLOMO_KERNEL_STRIP_POOL : V2E_SLOMO_KERNEL_STRIP)
+                                       : V2E_SLOMO_KERNEL_TAP;
     if (row)
         rc = v2e_strip_prepare(R, x1, u.c1p[li], x2, x2 ? u.c2p[li] : 0, u.w_row[li], u.b[li], u.cout_pad[li], u.L[li].k,
                                u.L[li].k, B, H, W, out, u.cout_pad[li], out_mode, u.L[li].cout, kSlope, h->n_sms,
@@ -542,6 +546,7 @@ static int conv(V2eSlomo *h, const UNet &u, int li, const __half *x1, const __ha
 
 static int conv_up2(V2eSlomo *h, const UNet &u, int li, const __half *x_low, int B, int H, int W, void *out, cudaStream_t st) {
     V2eUpLaunch *L = (V2eUpLaunch *)h->up_mem.data();
+    h->ran[&u == &h->interp][li] = V2E_SLOMO_KERNEL_UP2;
     int rc = v2e_conv_up2_prepare(L, x_low, u.c1p[li], u.w_fold[li], u.w[li], u.b[li], u.cout_pad[li], B, H, W, out,
                                   u.cout_pad[li], kSlope, h->n_sms);
     if (rc) return rc;
@@ -718,6 +723,29 @@ extern "C" int v2e_slomo_profile_read_layers(V2eSlomo *h, float *ms23, int *laun
 
 extern "C" const float *v2e_slomo_flow_ptr(V2eSlomo *h) { return h ? h->flow_out : nullptr; }
 extern "C" const float *v2e_slomo_intrp_ptr(V2eSlomo *h) { return h ? h->intrp_out : nullptr; }
+
+extern "C" void *v2e_slomo_buffer_ptr(V2eSlomo *h, int which, int index) {
+    if (!h) return nullptr;
+    const bool level = index >= 0 && index < 5;
+    switch (which) {
+        case V2E_SLOMO_BUF_IN16: return h->in16;
+        case V2E_SLOMO_BUF_X0: return h->x0;
+        case V2E_SLOMO_BUF_S1: return h->s1;
+        case V2E_SLOMO_BUF_POOL: return level ? h->pool[index] : nullptr;
+        case V2E_SLOMO_BUF_DA: return level ? h->da[index] : nullptr;
+        case V2E_SLOMO_BUF_S: return level ? h->s[index] : nullptr;
+        case V2E_SLOMO_BUF_UP: return level ? h->up[index] : nullptr;
+        case V2E_SLOMO_BUF_UA: return level ? h->ua[index] : nullptr;
+        case V2E_SLOMO_BUF_UB: return level ? h->ub[index] : nullptr;
+        case V2E_SLOMO_BUF_IMG: return h->img;
+        default: return nullptr;
+    }
+}
+
+extern "C" int v2e_slomo_layer_kernel(V2eSlomo *h, int net, int layer) {
+    if (!h || net < 0 || net > 1 || layer < 0 || layer >= 23) return v2e_set_error(V2E_E_INVALID, "bad net / layer%s", "");
+    return h->ran[net][layer];
+}
 
 // ---- Pillow-exact uint8 resize -------------------------------------------------------------------
 struct V2eResizer {

@@ -151,6 +151,49 @@ class SloMoEngine:
     def intrp_out(self):
         return self._view(self.lib.v2e_slomo_intrp_ptr)
 
+    # engine internals for layer-by-layer tests: v2e_slomo_buffer_ptr / v2e_slomo_layer_kernel (include/v2e_b200.h)
+    _BUFS = {"in16": 0, "x0": 1, "s1": 2, "pool": 3, "da": 4, "s": 5, "up": 6, "ua": 7, "ub": 8, "img": 9}
+    KERNELS = {0: None, 1: "tap", 2: "strip", 3: "strip_pool", 4: "up2"}
+
+    def activations(self):
+        """Views (no copies) of the engine's buffers for the current batch: fp16 NHWC "in16", "x0", "s1", lists of
+        five "pool", "da", "s" (level l at 1/2^(l+1) resolution) and "up", "ua", "ub" (up block k at 1/2^(4-k)), and
+        the fp32 normalised frames "img" [B+1, H, W]. The flow and interpolation networks share these buffers: read the
+        flow network's after set_pairs and before interp. up[k] is stale when up block k ran fused (layer_kernels)."""
+        from .emulator import _DevView
+        b, H, W = self.cur_b, self.h, self.w
+        shapes = unet_layer_shapes(12, 5)
+
+        def view(name, index, shape, typestr="<f2"):
+            ptr = self.lib.v2e_slomo_buffer_ptr(self._h, self._BUFS[name], index)
+            if not ptr:
+                raise RuntimeError("v2e_slomo_buffer_ptr: no buffer %s[%d]" % (name, index))
+            return torch.as_tensor(_DevView(ptr, shape, typestr, self), device=self.device)
+
+        a = {"in16": view("in16", 0, (b, H, W, 16)), "x0": view("x0", 0, (b, H, W, 32)),
+             "s1": view("s1", 0, (b, H, W, 32)), "img": view("img", 0, (b + 1, H, W), "<f4")}
+        for name, first, lvl in (("pool", 2, lambda l: l + 1), ("da", 2, lambda l: l + 1), ("s", 3, lambda l: l + 1),
+                                 ("up", 12, lambda k: 4 - k), ("ua", 12, lambda k: 4 - k), ("ub", 13, lambda k: 4 - k)):
+            a[name] = []
+            for i in range(5):
+                co, ci, _ = shapes[first + 2 * i]
+                c = ci if name in ("pool", "up") else co
+                a[name].append(view(name, i, (b, H >> lvl(i), W >> lvl(i), c)))
+        return a
+
+    def layer_kernels(self):
+        """{"flow": [...], "interp": [...]}: per layer (forward order), the kernel that ran it in the last forward pass
+        of that network: "tap", "strip", "strip_pool" (pool of the next down block from the epilogue), "up2" (fused x2
+        up-sampling), or None (not run yet)."""
+        out = {}
+        for net, name in ((0, "flow"), (1, "interp")):
+            codes = [self.lib.v2e_slomo_layer_kernel(self._h, net, i) for i in range(len(LAYER_NAMES))]
+            for c in codes:
+                if c < 0:
+                    _lib.check(c)
+            out[name] = [self.KERNELS[c] for c in codes]
+        return out
+
 
 class SuperSloMo(object):
     def __init__(self, model: str, auto_upsample: bool, upsampling_factor: object, batch_size=1,
