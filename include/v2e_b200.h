@@ -270,6 +270,15 @@ int v2e_emu_state_is_f64(V2eEmu *h);
 /* device pointer of a state array (same `which`), for zero-copy views */
 void *v2e_emu_state_ptr(V2eEmu *h, int which);
 
+/* Test hook, rng_mode 1 (not used by the stepping functions): the Philox draws of Philox frame index `frame_index`
+ * for every pixel of the handle, from the same device functions the kernels use. Each non-null output is a device
+ * array of H*W float32 indexed by the handle's pixel index: leak_randn the leak-jitter normal, shot_u01 the full
+ * shot-noise uniform (the kernels only complete it for prefix candidates), pr_randn the photoreceptor-noise normal.
+ * Leak and shot counters use rng_pixel_offset + pixel, like the kernels. Frame k >= 1 of a clip (frame 0 only
+ * initialises) is drawn with frame_index k - 1. Asynchronous on `stream`. */
+int v2e_emu_draw_noise(V2eEmu *h, uint32_t frame_index, float *leak_randn, float *shot_u01, float *pr_randn,
+                       void *stream);
+
 /* ------------------------------------------------------------------------- */
 /* SuperSloMo network pieces: replace v2ecore/model.py (UNet :158-226, backWarp :229-300)
  * and the per-frame tensor code of v2ecore/slomo.py:330-444.                      */

@@ -2,6 +2,8 @@
 UNMODIFIED reference (device="cpu") in the build container.
 
     python oracle/make_golden.py            # needs /root/reference
+    python oracle/make_golden.py optional   # SCIDVS / photoreceptor-noise fixtures only
+    python oracle/make_golden.py hdr        # log-encoded input (hdr=True) fixtures only
 
 Each fixture holds: the input frames and times, the constructor kwargs, the
 "tape" of every random draw the reference made (thresholds, noise-rate field,
@@ -162,10 +164,25 @@ def main_optional(emu_mod):
                    pos_thres=0.05, neg_thres=0.05), fr4, np.arange(6) * 1e-4)
 
 
+def main_hdr(emu_mod):
+    """hdr=True (emulator.py:100, 663-672): the frames are already natural-log intensities, float32."""
+    H, W, T = 24, 40, 8
+    fr = np.log1p(texture_frames(H, W, T, seed=13, speed=2.0).astype(np.float32)).astype(np.float32)
+    ts = np.arange(T) * 1e-3
+    save_case("emu_hdr", emu_mod,
+              dict(hdr=True, cutoff_hz=300, leak_rate_hz=0.1, shot_noise_rate_hz=5.0, refractory_period_s=0.001,
+                   sigma_thres=0.03, pos_thres=0.1, neg_thres=0.1), fr, ts)
+    save_case("emu_hdr_nolp", emu_mod,
+              dict(hdr=True, cutoff_hz=0, leak_rate_hz=0.1, shot_noise_rate_hz=5.0, refractory_period_s=0.001,
+                   sigma_thres=0.03, pos_thres=0.1, neg_thres=0.1), fr, ts)
+
+
 def main():
     emu_mod, _, _, _ = ref_shim.load_reference()
     if len(sys.argv) > 1 and sys.argv[1] == "optional":
         return main_optional(emu_mod)
+    if len(sys.argv) > 1 and sys.argv[1] == "hdr":
+        return main_hdr(emu_mod)
     H, W, T = 24, 40, 10
     fr = texture_frames(H, W, T)
     ts = np.arange(T) * 1e-3

@@ -9,7 +9,7 @@ GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 EMU_GOLDENS = ["emu_class_default", "emu_cli_noisy", "emu_clean", "emu_scalar_thres_f64",
                "emu_refractory_multi", "emu_float_frames", "emu_static_leak_shot",
-               "emu_ragged_13x37", "emu_csdvs", "emu_csdvs_120x176"]
+               "emu_ragged_13x37", "emu_csdvs", "emu_csdvs_120x176", "emu_hdr", "emu_hdr_nolp"]
 # optional pixel models: SCIDVS (emulator.py:58-80, 719-725), photoreceptor noise (emulator.py:694-703)
 EMU_GOLDENS_OPT = ["emu_scidvs", "emu_scidvs_f32", "emu_prnoise", "emu_prnoise_scidvs_csdvs"]
 
@@ -56,6 +56,65 @@ class TapeRNG:
 
     def exhausted(self):
         return self.pos == len(self.tape)
+
+
+class DeviceDrawRNG:
+    """Draw source for OracleEmulator(rng=..., shuffle=False) that hands the oracle the device RNG's own per-frame draws,
+    so that rng_mode="device" can be compared with the oracle bit for bit.
+
+    draws_for_frame(k) -> {"leak_randn", "shot_u01", "pr_randn"} ([H, W] float32, numpy or torch) for frame k >= 1 of
+    the clip; `frame` must hold the number of the frame being generated (run_oracle_with_draws sets it). Frame 0's
+    initial draws (thresholds, SCIDVS tau, noise-rate field) come from torch's global generator, as in device mode.
+    After that: randn gives the photoreceptor normals (when that model is on), then the leak normals; rand the shot
+    uniforms; randperm(n) the identity (device rows of one (frame, iteration, polarity) group have no order)."""
+
+    def __init__(self, draws_for_frame, photoreceptor_noise=False):
+        self.draws_for_frame = draws_for_frame
+        self.photoreceptor_noise = photoreceptor_noise
+        self.frame = 0
+        self._loaded = None
+        self.calls = []            # (frame, kind) of every per-frame draw served
+
+    def _load(self, kind, shape):
+        assert self.frame >= 1
+        if self._loaded != self.frame:
+            d = self.draws_for_frame(self.frame)
+            host = {k: (v.cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)) for k, v in d.items()}
+            self._randn = ([host["pr_randn"]] if self.photoreceptor_noise else []) + [host["leak_randn"]]
+            self._rand = [host["shot_u01"]]
+            self._loaded = self.frame
+        q = self._randn if kind == "randn" else self._rand
+        assert q, "frame %d: more %s draws than the device makes" % (self.frame, kind)
+        a = q.pop(0)
+        assert a.shape == tuple(shape) and a.dtype == np.float32, (a.shape, a.dtype, shape)
+        self.calls.append((self.frame, kind))
+        return torch.from_numpy(np.array(a))
+
+    def normal(self, mean, std, shape):
+        assert self.frame == 0, "normal() after the first frame"
+        return torch.normal(mean, std, size=shape, dtype=torch.float32)
+
+    def randn(self, shape):
+        if self.frame == 0:
+            return torch.randn(shape, dtype=torch.float32)
+        return self._load("randn", shape)
+
+    def rand(self, shape):
+        assert self.frame >= 1, "rand() in the first frame"
+        return self._load("rand", shape)
+
+    def randperm(self, n):
+        return torch.arange(n)
+
+
+def run_oracle_with_draws(orc, rng, frames, times):
+    """Runs the oracle over a clip with a DeviceDrawRNG, frame k's draws being those of the clip's frame k.
+    Returns the per-frame rows (canonical order)."""
+    out = []
+    for k, (f, t) in enumerate(zip(frames, times)):
+        rng.frame = k
+        out.append(canonical(orc.generate_events(f, float(t))))
+    return out
 
 
 # ---- float64 references of the SuperSloMo convolutions and their error bars -----------------------------------

@@ -130,6 +130,7 @@ _SIGS = {
     "v2e_emu_get_state": (_i, [_vp, _i, _vp, ctypes.POINTER(_i)]),
     "v2e_emu_state_is_f64": (_i, [_vp]),
     "v2e_emu_state_ptr": (_vp, [_vp, _i]),
+    "v2e_emu_draw_noise": (_i, [_vp, ctypes.c_uint32, _vp, _vp, _vp, _vp]),
 }
 
 

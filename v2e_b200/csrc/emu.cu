@@ -245,6 +245,19 @@ __device__ __forceinline__ void noise_px4(uint64_t seed, uint32_t g0, uint32_t f
     if ((g0 & 3u) == 0) noise_quad(seed, g0 >> 2, frame_index, n, pref);
     else noise_px4_unaligned(seed, g0, frame_index, n, pref);
 }
+// Photoreceptor-noise normals (emulator.py:698) of pixels 4q .. 4q+3 from one Philox call; radius and angle from 24
+// bits each. q is the handle's LOCAL quad index, not one offset by px_off like the leak / shot streams: that is safe
+// because a handle with photoreceptor_noise is never a row band (pixel sharding refuses the model: v2e_emu_phase_update,
+// v2e_emu_cs_begin), so its local and whole-frame pixel indices coincide.
+__device__ __forceinline__ void pr_noise_quad(uint64_t seed, uint32_t quad, uint32_t frame_index, float rn[4]) {
+    const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+    const uint4 r = philox4x32<kPhiloxRounds>(make_uint4(quad, frame_index, 2u, 0x70726e7au), key);
+    const float a = sqrt_approx(-2.0f * __logf(u01_open(r.x))), b = sqrt_approx(-2.0f * __logf(u01_open(r.z)));
+    float sa, ca, sb, cb;
+    __sincosf(6.283185307179586f * u01_half(r.y), &sa, &ca);
+    __sincosf(6.283185307179586f * u01_half(r.w), &sb, &cb);
+    rn[0] = a * ca; rn[1] = a * sa; rn[2] = b * cb; rn[3] = b * sb;
+}
 
 // ---------------------------------------------------------------------------------------------
 // vector load helpers: 4 consecutive elements starting at i (i % 4 == 0)
@@ -701,15 +714,7 @@ __global__ void __launch_bounds__(kThreads) emu_front_kernel(EmuDev d, FramePara
     if (d.pr_noise) {
         ld4(d.noise_arr, i0, na);
         if (pr_randn) load_f32x4_any(pr_randn, i0, d.n, rn);
-        else {
-            const uint2 key = make_uint2((uint32_t)d.seed, (uint32_t)(d.seed >> 32));
-            uint4 r = philox4x32<kPhiloxRounds>(make_uint4((uint32_t)(i0 >> 2), p.frame_index, 2u, 0x70726e7au), key);
-            float a = sqrt_approx(-2.0f * __logf(u01_open(r.x))), b = sqrt_approx(-2.0f * __logf(u01_open(r.z)));
-            float sa, ca, sb, cb;
-            __sincosf(6.283185307179586f * u01_half(r.y), &sa, &ca);
-            __sincosf(6.283185307179586f * u01_half(r.w), &sb, &cb);
-            rn[0] = a * ca; rn[1] = a * sa; rn[2] = b * cb; rn[3] = b * sb;
-        }
+        else pr_noise_quad(d.seed, (uint32_t)(i0 >> 2), p.frame_index, rn);
     }
 #pragma unroll
     for (int k = 0; k < 4; k++) {
@@ -1848,6 +1853,25 @@ __global__ void emu_chain_step_kernel(EmuDev d, int slot) {
 
 __global__ void __launch_bounds__(kThreads) emu_plan_kernel(EmuDev d, FrameParams p, int slot) {
     plan_frame(d, p, slot);
+}
+
+// v2e_emu_draw_noise: the device-RNG draws of one frame index for EVERY pixel of the handle, through the same
+// functions the update / fused / front kernels call (noise_px4, shot_uniform, pr_noise_quad). Those kernels draw the
+// shot uniform's low bits only for prefix candidates; here every pixel gets its full uniform.
+__global__ void __launch_bounds__(kThreads) emu_draw_noise_kernel(EmuDev d, uint32_t frame_index, float *leak_randn,
+                                                                  float *shot_u01, float *pr_randn) {
+    const int i0 = (blockIdx.x * kThreads + threadIdx.x) * kVec;
+    if (i0 >= d.n) return;
+    const uint32_t g0 = (uint32_t)i0 + d.px_off;
+    float lr[4], rn[4];
+    uint32_t pref[4];
+    noise_px4(d.seed, g0, frame_index, lr, pref);
+    if (pr_randn) pr_noise_quad(d.seed, (uint32_t)(i0 >> 2), frame_index, rn);
+    for (int k = 0; k < 4 && i0 + k < d.n; k++) {
+        if (leak_randn) leak_randn[i0 + k] = lr[k];
+        if (shot_u01) shot_u01[i0 + k] = shot_uniform(d.seed, (g0 + k) >> 2, frame_index, (int)((g0 + k) & 3u), pref[k]);
+        if (pr_randn) pr_randn[i0 + k] = rn[k];
+    }
 }
 
 }  // namespace
@@ -3217,6 +3241,16 @@ extern "C" int v2e_emu_time_update(V2eEmu *h, const void *frame_dev, int dtype, 
     if (rc) return rc;
     if (ce != cudaSuccess) return fail(V2E_E_CUDA, "v2e_emu_time_update: %s", cudaGetErrorString(ce));
     *us_per_launch = ms * 1e3f / (float)K;
+    return V2E_OK;
+}
+
+extern "C" int v2e_emu_draw_noise(V2eEmu *h, uint32_t frame_index, float *leak_randn, float *shot_u01, float *pr_randn,
+                                  void *stream) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    if (!leak_randn && !shot_u01 && !pr_randn) return V2E_OK;
+    emu_draw_noise_kernel<<<grid_for(h->d), kThreads, 0, (cudaStream_t)stream>>>(h->d, frame_index, leak_randn, shot_u01,
+                                                                                 pr_randn);
+    CU(cudaGetLastError());
     return V2E_OK;
 }
 

@@ -1033,6 +1033,23 @@ class EventEmulator(object):
         # a copy: the library owns the memory and frees it at reset() / cleanup()
         return torch.as_tensor(view, device=self.device).clone()
 
+    def device_draws(self, frame_index):
+        """rng_mode='device': the Philox draws of `frame_index` for every pixel of this emulator's handle, as [H, W]
+        float32 CUDA tensors: 'leak_randn' (leak jitter normal), 'shot_u01' (shot-noise uniform) and 'pr_randn'
+        (photoreceptor-noise normal). Frame k >= 1 of a clip uses frame_index k - 1 (frame 0 only initialises),
+        whichever of generate_events / generate_events_batch ran it. For checking the kernels against a CPU model
+        fed with the same draws; nothing here takes part in generating events."""
+        if not self._h:
+            raise RuntimeError("device_draws needs the handle the first frame creates")
+        out = {k: torch.empty((self._H, self._W), dtype=torch.float32, device=self.device)
+               for k in ("leak_randn", "shot_u01", "pr_randn")}
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.v2e_emu_draw_noise(
+                self._h, int(frame_index) & 0xFFFFFFFF, *(ctypes.c_void_p(out[k].data_ptr())
+                                                        for k in ("leak_randn", "shot_u01", "pr_randn")),
+                self._stream()))
+        return out
+
     lp_log_frame = property(lambda self: self._state("lp_log_frame"))
     base_log_frame = property(lambda self: self._state("base_log_frame"))
     timestamp_mem = property(lambda self: self._state("timestamp_mem"))
