@@ -71,11 +71,13 @@ typedef struct V2eEmuCfg {
     int32_t scidvs;                 /* emulator.py:114, 719-725: nonlinear CR high-pass before the change amplifier */
     int32_t photoreceptor_noise;    /* emulator.py:95, 694-703: Gaussian photoreceptor noise instead of injected
                                        shot events (needs shot_noise_rate_hz > 0 and cutoff_hz > 0, :196-204) */
-    uint32_t rng_pixel_offset;      /* rng_mode 1: index, in the WHOLE frame, of this handle's pixel 0. 0 unless the
-                                       handle owns a row band of a pixel-sharded clip (y0 * width): the Philox counters
-                                       use whole-frame pixel indices, so the bands draw what one GPU would draw */
-    uint32_t full_frame_px;         /* pixels of the WHOLE frame when the handle owns a row band (0: width * height):
-                                       the reference's float32 conv2d sums in a size-dependent order (centre-surround) */
+    uint32_t rng_pixel_offset;      /* index, in the WHOLE frame, of this handle's pixel 0. 0 unless the handle owns a
+                                       row band of a pixel-sharded clip (y0 * width): the Philox counters (rng_mode 1)
+                                       and the centre-surround Laplacian's summation order use whole-frame pixel
+                                       indices, so the bands compute what one GPU would compute */
+    uint32_t full_frame_px;         /* pixels of the WHOLE frame when the handle owns a row band (0: width * height;
+                                       a band has the frame's width): the reference's float32 conv2d sums in an order
+                                       that depends on the frame's size and the pixel's index (centre-surround) */
     int32_t own_row0, own_rows;     /* rows [own_row0, own_row0 + own_rows) of the handle emit events; the rest are halo
                                        rows of a pixel-sharded centre-surround handle (own_rows = 0: all rows) */
     int32_t cs_halo_rows;           /* K > 0: pixel-sharded centre-surround model -- K halo rows either side of the own
@@ -229,6 +231,9 @@ uint64_t *v2e_emu_cs_max_dev(V2eEmu *h);
 int v2e_emu_cs_advance(V2eEmu *h, int s0, int s1, void *stream);
 int v2e_emu_cs_update(V2eEmu *h, const void *frame_dev, int frame_dtype, const float *leak_randn_dev,
                       const float *shot_rand_dev, void *stream);
+/* counters: surround Euler iterations (one per frame; one per chunk when pixel-sharded) that ran as one cooperative
+ * launch / as one kernel per step (the cooperative launch was refused, or V2E_CS_COOP=0 at the first use) */
+int v2e_emu_cs_paths(V2eEmu *h, long long *coop, long long *per_step);
 int v2e_emu_phase_filter(V2eEmu *h, double t_frame, double t_previous, uint64_t capacity, int do_plan,
                          void *stream);
 /* per-(iteration,polarity) row counts of the frame just counted: counts_host[2*max_n]

@@ -166,12 +166,49 @@ int oracle_emu_first_frame(const OracleEmuCfg *cfg, OracleEmuState *st,
     return 0;
 }
 
+/* ---- float32 Laplacian: emulator.py:1115 -------------------------------- */
+/* Deliberate errors for the sensitivity tests (tests/test_emulator_centre_surround.py), all off by default:
+ * legacy_order restores the rule this file used to state (kernel order iff H*W >= 20000, no tail), alpha_h_ulps
+ * moves the float32 alpha_h of the surround update up by that many ulps. */
+static struct { int legacy_order, alpha_h_ulps; } g_perturb;
+void oracle_set_cs_perturbation(int legacy_order, int alpha_h_ulps) {
+    g_perturb.legacy_order = legacy_order;
+    g_perturb.alpha_h_ulps = alpha_h_ulps;
+}
+
+/* torch.conv2d(ReplicationPad2d(1)(h), [[0,1,0],[1,-4,1],[0,1,0]]) on the CPU (torch 2.11, AVX-512 build) for a
+ * [1,1,H,W] float32 field. Only the summation order of the five non-zero taps varies, by frame size and pixel:
+ *  - padded input of more than 20480 elements, (H+2)*(W+2) > 20480: oneDNN (ATen's use_mkldnn size heuristic)
+ *    accumulates in kernel order (((u+l)+c)+r)+d at every pixel;
+ *  - otherwise ATen's native im2col + GEMM pairs the taps, (u+l)+(c+(r+d)), except in the last n mod 16 elements of
+ *    the flattened output (the GEMM's 16-float vector remainder), which take kernel order again.
+ * Measured by bisecting over frame sizes and pinned by tests/test_laplacian_order.py against
+ * tests/golden/laplacian_conv2d.npz (oracle/make_golden_laplacian.py). i is the WHOLE frame's flattened index. */
+int oracle_lap_kernel_order(long H, long W, long i) {
+    if (g_perturb.legacy_order) return H * W >= 20000;
+    if ((H + 2) * (W + 2) > 20480) return 1;
+    return i >= (H * W) / 16 * 16;
+}
+
+static float lap_f32(const float *hf, long H, long W, long y, long x) {
+    long ym = y > 0 ? y - 1 : 0, yp = y < H - 1 ? y + 1 : H - 1;
+    long xm = x > 0 ? x - 1 : 0, xp = x < W - 1 ? x + 1 : W - 1;
+    float uu = hf[ym * W + x], ll = hf[y * W + xm], cc = -4.0f * hf[y * W + x];
+    float rr = hf[y * W + xp], dd = hf[yp * W + x];
+    return oracle_lap_kernel_order(H, W, y * W + x) ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
+}
+
+/* the whole Laplacian of an H x W float32 field, for the test against torch */
+void oracle_laplacian_f32(const float *hf, long H, long W, float *out) {
+    for (long y = 0; y < H; y++)
+        for (long x = 0; x < W; x++) out[y * W + x] = lap_f32(hf, H, W, y, x);
+}
+
 /* ---- CSDVS surround: emulator.py:1061-1124 ----------------------------- */
 /* Euler steps of h += alpha_p*(p-h) + alpha_h*lap(float32(h)), replicate pad,
  * until max|change| <= 1e-5 or num_steps. p,h float64; the 3x3 stencil is a
- * float32 conv2d (emulator.py:1115), products promoted back to float64.
- * Returns steps taken. conv2d accumulation order for the 5 non-zero taps of
- * [[0,1,0],[1,-4,1],[0,1,0]] is row-major over the kernel. */
+ * float32 conv2d (emulator.py:1115, lap_f32), products promoted back to float64.
+ * Returns steps taken. */
 int oracle_emu_csdvs(const OracleEmuCfg *cfg, OracleEmuState *st, double delta_time,
                      double tau_p, double tau_h) {
     long W = cfg->width, H = cfg->height, n = W * H;
@@ -181,7 +218,8 @@ int oracle_emu_csdvs(const OracleEmuCfg *cfg, OracleEmuState *st, double delta_t
     double alpha_p = adt / tau_p, alpha_h = adt / tau_h;
     const double *p = (const double *)st->lp;
     double *h = st->surround;
-    const int seq_order = n >= 20000;
+    float alpha_h_f = (float)alpha_h;
+    for (int k = 0; k < g_perturb.alpha_h_ulps; k++) alpha_h_f = nextafterf(alpha_h_f, INFINITY);
     float *hf = (float *)malloc(sizeof(float) * n);
     double *chg = (double *)malloc(sizeof(double) * n);
     double max_change = 2e-5;
@@ -190,19 +228,10 @@ int oracle_emu_csdvs(const OracleEmuCfg *cfg, OracleEmuState *st, double delta_t
         for (long i = 0; i < n; i++) hf[i] = (float)h[i];
         max_change = 0;
         for (long y = 0; y < H; y++) {
-            long ym = y > 0 ? y - 1 : 0, yp = y < H - 1 ? y + 1 : H - 1;
             for (long x = 0; x < W; x++) {
-                long xm = x > 0 ? x - 1 : 0, xp = x < W - 1 ? x + 1 : W - 1;
-                /* float32 conv2d of the replicate-padded field with [[0,1,0],[1,-4,1],[0,1,0]]. The
-                 * accumulation order is the CPU backend's (oneDNN, AVX-512 build of torch 2.11): probed
-                 * by exhaustive search over summation trees, see DESIGN.md */
-                float uu = hf[ym * W + x], ll = hf[y * W + xm], cc = -4.0f * hf[y * W + x];
-                float rr = hf[y * W + xp], dd = hf[yp * W + x];
-                /* torch 2.11 CPU conv2d: tensors of >= 20000 output elements (both BASELINE sizes) take the
-                 * path that accumulates the taps in kernel order; smaller ones pair them up */
-                float acc = seq_order ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
+                float acc = lap_f32(hf, H, W, y, x);
                 /* alpha_h is a Python float meeting a float32 tensor: rounded to float32, float32 product */
-                float h_term = (float)alpha_h * acc;
+                float h_term = alpha_h_f * acc;
                 double c = alpha_p * (p[y * W + x] - h[y * W + x]) + (double)h_term;
                 chg[y * W + x] = c;
                 double a = fabs(c);

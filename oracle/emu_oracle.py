@@ -79,6 +79,12 @@ def lib():
                                       ctypes.c_void_p, ctypes.c_long, ctypes.c_void_p]
         L.oracle_linspace_f32.restype = ctypes.c_float
         L.oracle_linspace_f32.argtypes = [ctypes.c_double, ctypes.c_double, ctypes.c_int64, ctypes.c_int64]
+        L.oracle_lap_kernel_order.restype = ctypes.c_int
+        L.oracle_lap_kernel_order.argtypes = [ctypes.c_long, ctypes.c_long, ctypes.c_long]
+        L.oracle_laplacian_f32.restype = None
+        L.oracle_laplacian_f32.argtypes = [ctypes.c_void_p, ctypes.c_long, ctypes.c_long, ctypes.c_void_p]
+        L.oracle_set_cs_perturbation.restype = None
+        L.oracle_set_cs_perturbation.argtypes = [ctypes.c_int, ctypes.c_int]
         _LIB = L
     return _LIB
 

@@ -4,6 +4,7 @@ UNMODIFIED reference (device="cpu") in the build container.
     python oracle/make_golden.py            # needs /root/reference
     python oracle/make_golden.py optional   # SCIDVS / photoreceptor-noise fixtures only
     python oracle/make_golden.py hdr        # log-encoded input (hdr=True) fixtures only
+    python oracle/make_golden.py cs         # centre-surround fixtures only
 
 Each fixture holds: the input frames and times, the constructor kwargs, the
 "tape" of every random draw the reference made (thresholds, noise-rate field,
@@ -177,12 +178,35 @@ def main_hdr(emu_mod):
                    sigma_thres=0.03, pos_thres=0.1, neg_thres=0.1), fr, ts)
 
 
+def main_cs(emu_mod):
+    """Centre-surround fixtures (emulator.py:1061-1124). The surround's float32 Laplacian sums its taps in an order
+    that depends on the frame size and, below 20 480 padded pixels, on the flattened index (oracle/emu_oracle.c,
+    oracle_lap_kernel_order): one fixture on each side of that switch and one whose flattened tail is non-empty."""
+    # centre-surround model (scripts/csdvs.sh:7-16: lambda 10 px, tau_p 0.5 ms, dt 1e-4 s, cutoff 100 Hz)
+    fr4 = texture_frames(20, 36, 6, seed=7)
+    save_case("emu_csdvs", emu_mod,
+              dict(cs_lambda_pixels=10, cs_tau_p_ms=0.5, cutoff_hz=100, refractory_period_s=1e-3,
+                   leak_rate_hz=0.1, shot_noise_rate_hz=1.0, sigma_thres=0.03), fr4, np.arange(6) * 1e-4)
+    # > 20480 padded pixels: the size class of both BASELINE resolutions (different float32 conv2d summation order)
+    save_case("emu_csdvs_120x176", emu_mod,
+              dict(cs_lambda_pixels=4, cs_tau_p_ms=2.0, cutoff_hz=200, leak_rate_hz=0, shot_noise_rate_hz=0,
+                   sigma_thres=0.02), texture_frames(120, 176, 5, seed=9), np.arange(5) * 5e-4)
+    # 37x53 = 1961 px: below the switch, the last 1961 mod 16 = 9 pixels take the other summation order; high contrast
+    # (1 px blocks, fast motion) so that the surround differs between the two orders
+    save_case("emu_csdvs_37x53", emu_mod,
+              dict(cs_lambda_pixels=3, cs_tau_p_ms=0.5, cutoff_hz=300, leak_rate_hz=0.1, shot_noise_rate_hz=1.0,
+                   sigma_thres=0.03, pos_thres=0.3, neg_thres=0.3),
+              texture_frames(37, 53, 6, seed=11, speed=3.0, block=1), np.arange(6) * 2e-4)
+
+
 def main():
     emu_mod, _, _, _ = ref_shim.load_reference()
     if len(sys.argv) > 1 and sys.argv[1] == "optional":
         return main_optional(emu_mod)
     if len(sys.argv) > 1 and sys.argv[1] == "hdr":
         return main_hdr(emu_mod)
+    if len(sys.argv) > 1 and sys.argv[1] == "cs":
+        return main_cs(emu_mod)
     H, W, T = 24, 40, 10
     fr = texture_frames(H, W, T)
     ts = np.arange(T) * 1e-3
@@ -222,15 +246,7 @@ def main():
     save_case("emu_ragged_13x37", emu_mod,
               dict(cutoff_hz=0, leak_rate_hz=0, shot_noise_rate_hz=0, sigma_thres=0.03), fr3,
               np.arange(8) * 1e-3)
-    # centre-surround model (scripts/csdvs.sh:7-16: lambda 10 px, tau_p 0.5 ms, dt 1e-4 s, cutoff 100 Hz)
-    fr4 = texture_frames(20, 36, 6, seed=7)
-    save_case("emu_csdvs", emu_mod,
-              dict(cs_lambda_pixels=10, cs_tau_p_ms=0.5, cutoff_hz=100, refractory_period_s=1e-3,
-                   leak_rate_hz=0.1, shot_noise_rate_hz=1.0, sigma_thres=0.03), fr4, np.arange(6) * 1e-4)
-    # >= 20000 pixels: the size class of both BASELINE resolutions (different float32 conv2d summation order)
-    save_case("emu_csdvs_120x176", emu_mod,
-              dict(cs_lambda_pixels=4, cs_tau_p_ms=2.0, cutoff_hz=200, leak_rate_hz=0, shot_noise_rate_hz=0,
-                   sigma_thres=0.02), texture_frames(120, 176, 5, seed=9), np.arange(5) * 5e-4)
+    main_cs(emu_mod)
     # BASELINE config 1: scripts/moving_dot.py 64x64, class defaults, seed 42 -> 27 917 events
     import importlib
     md = importlib.import_module("scripts.moving_dot")

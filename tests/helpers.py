@@ -9,7 +9,7 @@ GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 EMU_GOLDENS = ["emu_class_default", "emu_cli_noisy", "emu_clean", "emu_scalar_thres_f64",
                "emu_refractory_multi", "emu_float_frames", "emu_static_leak_shot",
-               "emu_ragged_13x37", "emu_csdvs", "emu_csdvs_120x176", "emu_hdr", "emu_hdr_nolp"]
+               "emu_ragged_13x37", "emu_csdvs", "emu_csdvs_120x176", "emu_csdvs_37x53", "emu_hdr", "emu_hdr_nolp"]
 # optional pixel models: SCIDVS (emulator.py:58-80, 719-725), photoreceptor noise (emulator.py:694-703)
 EMU_GOLDENS_OPT = ["emu_scidvs", "emu_scidvs_f32", "emu_prnoise", "emu_prnoise_scidvs_csdvs"]
 

@@ -56,6 +56,7 @@ _SIGS = {
     "v2e_emu_max_vec_dev": (_vp, [_vp]),
     "v2e_emu_fused_emit": (_i, [_vp, _vp, _u64, _u64, _vp]),
     "v2e_emu_fused_stats": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_longlong)]),
+    "v2e_emu_cs_paths": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_longlong)]),
     "v2e_emu_fused_frames": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_longlong)]),
     "v2e_emu_fused_last_reject": (_i, [_vp, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     "v2e_emu_time_fused": (_i, [_vp, _vp, _i, _i, _vp, _d, _vp, _u64, _i, ctypes.POINTER(ctypes.c_float),

@@ -71,7 +71,8 @@ struct EmuDev {                         // passed by value to every kernel
     double *surround2;                  // pong buffer
     int32_t *cs_cur;                    // which buffer holds the current surround
     unsigned long long *cs_max;         // [cs_cap] max|change| of every Euler step of the current frame (double bits)
-    int32_t cs_cap, cs_seq_order;
+    int32_t cs_cap;
+    int32_t cs_seq_from;                // pixels idx >= cs_seq_from sum the Laplacian in kernel order, the rest pairwise
     int32_t cs_ring;                    // buffers in the surround ring (2 unless pixel-sharded: steps per chunk + 1)
     int32_t cs_y_lo, cs_y_hi;           // rows of this handle that count for max|change| (the rank's own rows)
     int32_t own_lo, own_hi;             // pixels [own_lo, own_hi) emit events (a sharded centre-surround handle also
@@ -563,7 +564,7 @@ emu_csdvs_step_kernel(EmuDev d, double alpha_p, float alpha_h, int step, int i, 
         const double hc = h[idx];
         const float uu = (float)h[ym * d.W + x], ll = (float)h[y * d.W + xm], cc = -4.0f * (float)hc;
         const float rr = (float)h[y * d.W + xp], dd = (float)h[yp * d.W + x];
-        const float acc = d.cs_seq_order ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
+        const float acc = idx >= d.cs_seq_from ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
         const float h_term = alpha_h * acc;
         const double chg = alpha_p * (pp[idx] - hc) + (double)h_term;
         hn[idx] = hc + chg;
@@ -616,7 +617,7 @@ emu_csdvs_iter_kernel(EmuDev d, double alpha_p, float alpha_h, int s0, int s1, i
             const double hc = h[idx];
             const float uu = (float)h[ym * d.W + x], ll = (float)h[y * d.W + xm], cc = -4.0f * (float)hc;
             const float rr = (float)h[y * d.W + xp], dd = (float)h[yp * d.W + x];
-            const float acc = d.cs_seq_order ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
+            const float acc = idx >= d.cs_seq_from ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
             const float h_term = alpha_h * acc;
             const double chg = alpha_p * (pp[idx] - hc) + (double)h_term;
             hn[idx] = hc + chg;
@@ -1933,6 +1934,7 @@ struct V2eEmu {
     double cs_alpha_p; float cs_alpha_h;
     FrameParams cs_p;
     int cs_pending;             // v2e_emu_cs_begin ran, v2e_emu_cs_update not yet
+    long long n_cs_coop, n_cs_step;   // Euler iterations (frames, or chunks when sharded) run cooperatively / per step
 };
 
 thread_local char g_err[512] = "";
@@ -2090,9 +2092,14 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
         ALLOC(d.cs_cur, sizeof(int32_t));
         d.cs_cap = 8192;
         ALLOC(d.cs_max, (size_t)d.cs_cap * sizeof(unsigned long long));
-        // float32 conv2d summation order of the reference's CPU backend: decided by the size of the WHOLE frame
+        // float32 conv2d summation order of the reference's CPU backend (oracle_lap_kernel_order in
+        // oracle/emu_oracle.c): kernel order everywhere when the WHOLE frame's padded size (H+2)*(W+2) exceeds 20480,
+        // else pairwise except in the last full_px mod 16 pixels of the whole flattened frame. A row band has the
+        // frame's width, so full_frame_px / W is the frame's height; px_off turns a local index into a global one.
         const long long full_px = cfg->full_frame_px ? (long long)cfg->full_frame_px : (long long)d.n;
-        d.cs_seq_order = full_px >= 20000;
+        const long long full_h = full_px / d.W;
+        const long long tail0 = (full_h + 2) * (d.W + 2) > 20480 ? 0 : full_px / 16 * 16 - (long long)d.px_off;
+        d.cs_seq_from = (int32_t)(tail0 > 0 ? tail0 : 0);
         if (cfg->cs_halo_rows > 0) {
             const int K = cfg->cs_halo_rows;
             if (K > d.cs_y_hi - d.cs_y_lo) { v2e_emu_destroy(h); return fail(V2E_E_INVALID, "cs_halo_rows larger than the band"); }
@@ -2387,11 +2394,14 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
         float alpha_h = 0;
         if ((rc = cs_plan(h, p, &num_steps, &alpha_p, &alpha_h))) return rc;
         CU(cudaMemsetAsync(d.cs_max, 0, (size_t)num_steps * sizeof(unsigned long long), st));
-        if (!cs_launch_iter(h, alpha_p, alpha_h, 0, num_steps, 0, slot, st)) {
+        if (cs_launch_iter(h, alpha_p, alpha_h, 0, num_steps, 0, slot, st)) {
+            h->n_cs_coop++;
+        } else {
             const int gs = (d.n + kThreads - 1) / kThreads;
             for (int k = 0; k < num_steps; k++)
                 emu_csdvs_step_kernel<<<gs, kThreads, 0, st>>>(d, alpha_p, alpha_h, k, k, 0);
             emu_csdvs_finish_kernel<<<1, 1, 0, st>>>(d, num_steps, slot);
+            h->n_cs_step++;
         }
     }
     {
@@ -2644,6 +2654,12 @@ extern "C" int v2e_emu_fused_stats(V2eEmu *h, long long *chunks, long long *reje
     if (!h) return fail(V2E_E_INVALID, "null handle");
     if (chunks) *chunks = h->n_fused_chunks;
     if (rejected) *rejected = h->n_fused_rejected;
+    return V2E_OK;
+}
+extern "C" int v2e_emu_cs_paths(V2eEmu *h, long long *coop, long long *per_step) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    if (coop) *coop = h->n_cs_coop;
+    if (per_step) *per_step = h->n_cs_step;
     return V2E_OK;
 }
 extern "C" int v2e_emu_fused_frames(V2eEmu *h, long long *frames_multi, long long *frames_single) {
@@ -3083,10 +3099,13 @@ extern "C" int v2e_emu_cs_chunk(V2eEmu *h, int s0, int s1, void *stream) {
     if (!h || !h->cs_pending) return fail(V2E_E_STATE, "v2e_emu_cs_begin must precede v2e_emu_cs_chunk");
     if (s0 < 0 || s1 <= s0 || s1 > h->cs_num_steps || s1 - s0 > h->cs_K) return fail(V2E_E_INVALID, "bad chunk of Euler steps");
     const EmuDev &d = h->d;
-    if (!cs_launch_iter(h, h->cs_alpha_p, h->cs_alpha_h, s0, s1, 1, 0, (cudaStream_t)stream)) {
+    if (cs_launch_iter(h, h->cs_alpha_p, h->cs_alpha_h, s0, s1, 1, 0, (cudaStream_t)stream)) {
+        h->n_cs_coop++;
+    } else {
         const int gs = (d.n + kThreads - 1) / kThreads;
         for (int s = s0; s < s1; s++)
             emu_csdvs_step_kernel<<<gs, kThreads, 0, (cudaStream_t)stream>>>(d, h->cs_alpha_p, h->cs_alpha_h, s, s - s0, 1);
+        h->n_cs_step++;
     }
     CU(cudaGetLastError());
     return V2E_OK;

@@ -1033,6 +1033,13 @@ class EventEmulator(object):
         # a copy: the library owns the memory and frees it at reset() / cleanup()
         return torch.as_tensor(view, device=self.device).clone()
 
+    def cs_paths(self):
+        """Centre-surround model: (cooperative, per_step) = how many Euler iterations (frames; chunks when
+        pixel-sharded) ran as one cooperative launch and how many as one kernel per step."""
+        coop, per_step = ctypes.c_longlong(0), ctypes.c_longlong(0)
+        _lib.check(self._lib.v2e_emu_cs_paths(self._h, ctypes.byref(coop), ctypes.byref(per_step)))
+        return coop.value, per_step.value
+
     def device_draws(self, frame_index):
         """rng_mode='device': the Philox draws of `frame_index` for every pixel of this emulator's handle, as [H, W]
         float32 CUDA tensors: 'leak_randn' (leak jitter normal), 'shot_u01' (shot-noise uniform) and 'pr_randn'
