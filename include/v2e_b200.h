@@ -208,9 +208,12 @@ int32_t *v2e_emu_max_n_dev(V2eEmu *h);
  *   v2e_emu_cs_begin      low-pass of the band, Euler-step plan (*num_steps, emulator.py:1076-1078)
  *   for chunks [s0, s1) of at most K steps:
  *       v2e_emu_cs_pack        own edge rows of the current surround -> v2e_emu_cs_send_dev()  [2][K][W] float64
- *       (caller: exchange with the neighbours; into v2e_emu_cs_recv_dev(): [0] = the rows above, [1] = below)
- *       v2e_emu_cs_unpack      received rows -> halo rows
- *       v2e_emu_cs_chunk       steps s0 .. s1-1 (each into its own ring buffer; maxima over the own rows)
+ *                              ([0] = the top K own rows, [1] = the bottom K)
+ *       (caller: exchange with the neighbours, e.g. one all-gather of every rank's send buffer)
+ *       v2e_emu_cs_unpack_from the neighbours' rows -> halo rows, read where the exchange left them:
+ *                              rows_above_dev = the upper neighbour's bottom K rows [K][W], rows_below_dev = the lower
+ *                              neighbour's top K rows; NULL at the image border
+ *       v2e_emu_cs_chunk      steps s0 .. s1-1 (each into its own ring buffer; maxima over the own rows)
  *       (caller: all-reduce MAX of the uint64 at v2e_emu_cs_max_dev()[s0 .. s1) -- non-negative doubles order
  *        like their bit patterns)
  *       v2e_emu_cs_advance     first step with max|change| <= 1e-5 ends the iteration (device side, no host sync)
@@ -219,13 +222,8 @@ int32_t *v2e_emu_max_n_dev(V2eEmu *h);
 int v2e_emu_cs_begin(V2eEmu *h, const void *frame_dev, int frame_dtype, double t_frame, double t_previous,
                      uint64_t capacity, uint64_t ev_base_start, int *num_steps, void *stream);
 int v2e_emu_cs_pack(V2eEmu *h, void *stream);
-int v2e_emu_cs_unpack(V2eEmu *h, void *stream);
-/* the same, reading the neighbours' rows where the exchange left them (e.g. inside an all-gathered buffer):
- * rows_above_dev = the upper neighbour's bottom K rows [K][W], rows_below_dev = the lower neighbour's top K rows;
- * NULL at the image border */
 int v2e_emu_cs_unpack_from(V2eEmu *h, const double *rows_above_dev, const double *rows_below_dev, void *stream);
 double *v2e_emu_cs_send_dev(V2eEmu *h);
-double *v2e_emu_cs_recv_dev(V2eEmu *h);
 int v2e_emu_cs_chunk(V2eEmu *h, int s0, int s1, void *stream);
 uint64_t *v2e_emu_cs_max_dev(V2eEmu *h);
 int v2e_emu_cs_advance(V2eEmu *h, int s0, int s1, void *stream);
@@ -250,29 +248,21 @@ int v2e_emu_phase_emit(V2eEmu *h, double t_frame, double t_previous, float *even
                        uint64_t capacity, void *stream);
 
 /* Measurement hooks: when enabled, v2e_emu_step brackets each of its kernels with CUDA events on
- * `stream`. v2e_emu_profile_read synchronises and returns, for the last step, the summed device
- * time (ms) and launch count of the {update, filter, emit} kernels. */
+ * `stream`. v2e_emu_profile_read4 synchronises and returns, for the last step, the summed device
+ * time (ms) and launch count of the {update, filter, emit} kernels, and a fourth entry: the event
+ * bracket around an empty kernel launched once per frame while profiling -- the floor of this
+ * measurement method (launch + event processing), so that a reader can tell a kernel's duration
+ * from the cost of observing it. */
 int v2e_emu_profile(V2eEmu *h, int enable);
-int v2e_emu_profile_read(V2eEmu *h, float *ms_sum3, int *launches3, void *stream);
-/* Same with a fourth entry: the event bracket around an empty kernel launched once per frame while
- * profiling -- the floor of this measurement method (launch + event processing), so that a reader can
- * tell a kernel's duration from the cost of observing it. */
 int v2e_emu_profile_read4(V2eEmu *h, float *ms_sum4, int *launches4, void *stream);
 
-/* Average duration (microseconds) of the update kernel over K back-to-back launches on `frame_dev` and the
- * handle's current state, between one pair of CUDA events; the launches store out of place, so each does the work
- * of the real launch and the state is left untouched. rng_mode 1, plain pixel model only. Synchronises. */
-int v2e_emu_time_update(V2eEmu *h, const void *frame_dev, int frame_dtype, double t_frame, double t_previous,
-                        int K, float *us_per_launch, void *stream);
-
-/* State access for parity probes (emulator.py:756-764 reads them by name). which:
+/* State access for parity probes (emulator.py:756-764 reads them by name): the device pointer of a state
+ * array, for zero-copy views, or NULL when this configuration has none. which:
  * 0 lp_log_frame, 1 base_log_frame, 2 pos_thres, 3 neg_thres, 4 noise_rate_array,
- * 5 timestamp_mem, 6 cs_surround_frame, 7 scidvs_highpass (state dtype), 8 photoreceptor_noise_arr (float32),
- * 9 scidvs_tau_arr (float32). dst_host must hold H*W elements of the state's
- * dtype (*elem_size returns 4 or 8). Synchronous. */
-int v2e_emu_get_state(V2eEmu *h, int which, void *dst_host, int *elem_size);
+ * 5 timestamp_mem, 6 cs_surround_frame (float64), 7 scidvs_highpass (state dtype), 8 photoreceptor_noise_arr
+ * (float32), 9 scidvs_tau_arr (float32). lp, base and the high-pass have the state dtype: float64 when
+ * v2e_emu_state_is_f64, else float32; the others are float32. */
 int v2e_emu_state_is_f64(V2eEmu *h);
-/* device pointer of a state array (same `which`), for zero-copy views */
 void *v2e_emu_state_ptr(V2eEmu *h, int which);
 
 /* Test hook, rng_mode 1 (not used by the stepping functions): the Philox draws of Philox frame index `frame_index`

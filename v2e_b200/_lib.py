@@ -74,10 +74,8 @@ _SIGS = {
     "v2e_emu_max_n_dev": (_vp, [_vp]),
     "v2e_emu_cs_begin": (_i, [_vp, _vp, _i, _d, _d, _u64, _u64, ctypes.POINTER(_i), _vp]),
     "v2e_emu_cs_pack": (_i, [_vp, _vp]),
-    "v2e_emu_cs_unpack": (_i, [_vp, _vp]),
     "v2e_emu_cs_unpack_from": (_i, [_vp, _vp, _vp, _vp]),
     "v2e_emu_cs_send_dev": (_vp, [_vp]),
-    "v2e_emu_cs_recv_dev": (_vp, [_vp]),
     "v2e_emu_cs_chunk": (_i, [_vp, _i, _i, _vp]),
     "v2e_emu_cs_max_dev": (_vp, [_vp]),
     "v2e_emu_cs_advance": (_i, [_vp, _i, _i, _vp]),
@@ -125,10 +123,7 @@ _SIGS = {
     "v2e_events_to_h5_rows": (_i, [_vp, _u64, _vp, _vp]),
     "v2e_events_to_aedat2": (_i, [_vp, _u64, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "v2e_emu_profile": (_i, [_vp, _i]),
-    "v2e_emu_profile_read": (_i, [_vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(_i), _vp]),
     "v2e_emu_profile_read4": (_i, [_vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(_i), _vp]),
-    "v2e_emu_time_update": (_i, [_vp, _vp, _i, _d, _d, _i, ctypes.POINTER(ctypes.c_float), _vp]),
-    "v2e_emu_get_state": (_i, [_vp, _i, _vp, ctypes.POINTER(_i)]),
     "v2e_emu_state_is_f64": (_i, [_vp]),
     "v2e_emu_state_ptr": (_vp, [_vp, _i]),
     "v2e_emu_draw_noise": (_i, [_vp, ctypes.c_uint32, _vp, _vp, _vp, _vp]),

@@ -64,8 +64,6 @@ struct EmuDev {                         // passed by value to every kernel
     double refr_d, shot_inten_m1;       // refractory_period_s ; (SHOT_NOISE_INTEN_FACTOR-1)
     uint64_t seed;
     void *lp, *base;
-    void *lp_out, *base_out;            // where the update kernel stores lp / base: the same arrays, except while
-                                        // v2e_emu_time_update replays one frame out of place
     float *pos_thres, *neg_thres, *noise_rate, *tmem;
     double *surround;                   // CSDVS h, ping buffer (cs_cur == 0)
     double *surround2;                  // pong buffer
@@ -1076,8 +1074,8 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
                 pk += m << (pols[k] ? 8 : 0);
                 nact += recs[k] != 0;
             }
-            if (!lp_done) st4((S *)d.lp_out, i0, lp);
-            if (f_leak) st4((S *)d.base_out, i0, base);
+            if (!lp_done) st4((S *)d.lp, i0, lp);
+            if (f_leak) st4((S *)d.base, i0, base);
             *(short4 *)(d.rec + i0) = make_short4(recs[0], recs[1], recs[2], recs[3]);
         }
         // per-(iteration,polarity) histogram. Iterations 0 and 1 (almost all events) are counted per thread,
@@ -1929,7 +1927,7 @@ struct V2eEmu {
     int fused_skip, fused_penalty;                 // back-off: chunks to run frame by frame before the next attempt
     // pixel-sharded centre-surround model: plan of the current frame (v2e_emu_cs_begin) and the exchange buffers
     int cs_K;                   // halo rows = Euler steps per chunk (0: not sharded)
-    double *cs_send, *cs_recv;  // [2][K][W]
+    double *cs_send;            // [2][K][W]
     int cs_num_steps;
     double cs_alpha_p; float cs_alpha_h;
     FrameParams cs_p;
@@ -2063,8 +2061,6 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
     } while (0)
     ALLOC(d.lp, np * h->state_elem);
     ALLOC(d.base, np * h->state_elem);
-    d.lp_out = d.lp;
-    d.base_out = d.base;
     ALLOC(d.rec, np * sizeof(int16_t));
 
     if (d.per_pixel_thres) { ALLOC(d.pos_thres, np * 4); ALLOC(d.neg_thres, np * 4); }
@@ -2109,7 +2105,6 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
             ALLOC(d.cs_bufs, (size_t)d.cs_ring * np * 8);
             ALLOC(d.cs_done, sizeof(int32_t));
             ALLOC(h->cs_send, (size_t)2 * K * d.W * 8);
-            ALLOC(h->cs_recv, (size_t)2 * K * d.W * 8);
         } else {
             ALLOC(d.surround, np * 8);
             ALLOC(d.surround2, np * 8);
@@ -2155,7 +2150,7 @@ extern "C" int v2e_emu_destroy(V2eEmu *h) {
     delete[] h->pr_vrms;
     delete[] h->ls.t_frames;
     delete[] h->sched;
-    void *cs_ptrs[] = {d.cs_bufs, d.cs_done, h->cs_send, h->cs_recv};
+    void *cs_ptrs[] = {d.cs_bufs, d.cs_done, h->cs_send};
     for (void *p : cs_ptrs) if (p) cudaFree(p);
     void *fused_ptrs[] = {h->lp_alt, h->base_alt, h->rec_list, h->rec_cnt, h->blk_cnt, h->ff_dev, h->fp_dev, h->max_vec};
     for (void *p : fused_ptrs) if (p) cudaFree(p);
@@ -2589,7 +2584,7 @@ static int enqueue_fused_emit(V2eEmu *h, int T, float *events, uint64_t capacity
                               const int32_t *max_vec, bool commit, cudaStream_t st, int a = 0, int chain = 0) {
     const EmuDev d = shifted_dev(h->d, a);
     {
-        ProfScope ps(h, 1, 1, st);       // slot 1: v2e_emu_profile_read sums count + plan under "filter"
+        ProfScope ps(h, 1, 1, st);       // slot 1: v2e_emu_profile_read4 sums count + plan under "filter"
         emu_fused_plan_kernel<<<1, kThreads, (size_t)T * sizeof(uint32_t), st>>>(d, h->fp_dev + a, T, ev_base_start, capacity,
                                                                                  max_vec, a, chain);
     }
@@ -3075,17 +3070,10 @@ extern "C" int v2e_emu_cs_begin(V2eEmu *h, const void *frame, int dtype, double 
     return V2E_OK;
 }
 extern "C" double *v2e_emu_cs_send_dev(V2eEmu *h) { return h ? h->cs_send : nullptr; }
-extern "C" double *v2e_emu_cs_recv_dev(V2eEmu *h) { return h ? h->cs_recv : nullptr; }
 extern "C" uint64_t *v2e_emu_cs_max_dev(V2eEmu *h) { return h ? (uint64_t *)h->d.cs_max : nullptr; }
 extern "C" int v2e_emu_cs_pack(V2eEmu *h, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
     emu_csdvs_pack_kernel<<<132, 256, 0, (cudaStream_t)stream>>>(h->d, h->cs_send, h->cs_K);
-    CU(cudaGetLastError());
-    return V2E_OK;
-}
-extern "C" int v2e_emu_cs_unpack(V2eEmu *h, void *stream) {
-    if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
-    emu_csdvs_unpack_kernel<<<132, 256, 0, (cudaStream_t)stream>>>(h->d, h->cs_recv, h->cs_recv + (size_t)h->cs_K * h->d.W, h->cs_K);
     CU(cudaGetLastError());
     return V2E_OK;
 }
@@ -3194,72 +3182,18 @@ extern "C" int v2e_emu_profile(V2eEmu *h, int enable) {
     return V2E_OK;
 }
 
-static int profile_read_n(V2eEmu *h, float *ms_sum, int *launches, int kinds, void *stream) {
+extern "C" int v2e_emu_profile_read4(V2eEmu *h, float *ms_sum, int *launches, void *stream) {
     if (!h || !h->ev || !ms_sum || !launches) return fail(V2E_E_INVALID, "profiling not enabled");
     CU(cudaStreamSynchronize((cudaStream_t)stream));
-    for (int k = 0; k < kinds; k++) { ms_sum[k] = 0.f; launches[k] = 0; }
+    for (int k = 0; k < 4; k++) { ms_sum[k] = 0.f; launches[k] = 0; }
     for (int s = 0; s < h->d.max_slots; s++)
-        for (int k = 0; k < kinds; k++)
+        for (int k = 0; k < 4; k++)
             if (h->prof_used[s * kProfKinds + k]) {
                 float ms = 0.f;
                 CU(cudaEventElapsedTime(&ms, h->ev[(s * kProfKinds + k) * 2], h->ev[(s * kProfKinds + k) * 2 + 1]));
                 ms_sum[k] += ms;
                 launches[k] += 1;
             }
-    return V2E_OK;
-}
-extern "C" int v2e_emu_profile_read(V2eEmu *h, float *ms_sum3, int *launches3, void *stream) {
-    return profile_read_n(h, ms_sum3, launches3, 3, stream);
-}
-extern "C" int v2e_emu_profile_read4(V2eEmu *h, float *ms_sum4, int *launches4, void *stream) {
-    return profile_read_n(h, ms_sum4, launches4, 4, stream);
-}
-
-// Average duration of the update kernel: K back-to-back launches on the given frame and the handle's CURRENT
-// state, between ONE pair of CUDA events (no per-launch bracket, whose own cost is several microseconds). The
-// launches store lp / base into scratch arrays, so every one of them does exactly the work of the real launch
-// (same loads, same stores, same event density) and the handle's state is untouched; the per-frame scratch
-// (records, active list, histograms of slot 0) is reset by the next v2e_emu_step as usual.
-extern "C" int v2e_emu_time_update(V2eEmu *h, const void *frame_dev, int dtype, double t_frame, double t_previous,
-                                   int K, float *us_per_launch, void *stream) {
-    if (!h || !frame_dev || !us_per_launch || K < 1) return fail(V2E_E_INVALID, "bad argument");
-    if (!h->first_done) return fail(V2E_E_STATE, "v2e_emu_first_frame must run first");
-    if (h->d.rng_mode != 1 || h->d.csdvs || h->d.scidvs || h->d.pr_noise)
-        return fail(V2E_E_UNSUPPORTED, "v2e_emu_time_update: device RNG, plain pixel model only");
-    cudaStream_t st = (cudaStream_t)stream;
-    EmuDev &d = h->d;
-    const size_t bytes = (size_t)d.units * kUnitPx * h->state_elem;
-    void *lp2 = nullptr, *base2 = nullptr;
-    CU(cudaMalloc(&lp2, bytes));
-    if (cudaMalloc(&base2, bytes) != cudaSuccess) { cudaFree(lp2); return fail(V2E_E_CUDA, "cudaMalloc failed"); }
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
-    int rc = reset_slots(h, 0, 1, st);
-    d.lp_out = lp2;
-    d.base_out = base2;
-    FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter, 0);
-    for (int i = 0; i < 2 && !rc; i++)          // warm-up
-        rc = d.state_f64 ? launch_update<double>(h, p, frame_dev, dtype, nullptr, nullptr, 0, 0, 0, st)
-                         : launch_update<float>(h, p, frame_dev, dtype, nullptr, nullptr, 0, 0, 0, st);
-    cudaEventRecord(e0, st);
-    for (int i = 0; i < K && !rc; i++)
-        rc = d.state_f64 ? launch_update<double>(h, p, frame_dev, dtype, nullptr, nullptr, 0, 0, 0, st)
-                         : launch_update<float>(h, p, frame_dev, dtype, nullptr, nullptr, 0, 0, 0, st);
-    cudaEventRecord(e1, st);
-    d.lp_out = d.lp;
-    d.base_out = d.base;
-    cudaError_t ce = cudaStreamSynchronize(st);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(lp2);
-    cudaFree(base2);
-    if (!rc) rc = reset_slots(h, 0, 1, st);
-    if (rc) return rc;
-    if (ce != cudaSuccess) return fail(V2E_E_CUDA, "v2e_emu_time_update: %s", cudaGetErrorString(ce));
-    *us_per_launch = ms * 1e3f / (float)K;
     return V2E_OK;
 }
 
@@ -3297,15 +3231,4 @@ extern "C" void *v2e_emu_state_ptr(V2eEmu *h, int which) {
         case 9: return h->d.tau_arr;
     }
     return nullptr;
-}
-
-extern "C" int v2e_emu_get_state(V2eEmu *h, int which, void *dst, int *elem_size) {
-    if (!h || !dst) return fail(V2E_E_INVALID, "null argument");
-    void *src = v2e_emu_state_ptr(h, which);
-    if (!src) return fail(V2E_E_STATE, "state array not allocated for this configuration");
-    int es = (which <= 1 || which == 7) ? (int)h->state_elem : (which == 6 ? 8 : 4);
-    CU(cudaDeviceSynchronize());
-    CU(cudaMemcpy(dst, src, (size_t)h->d.n * es, cudaMemcpyDeviceToHost));
-    if (elem_size) *elem_size = es;
-    return V2E_OK;
 }

@@ -267,7 +267,7 @@ class EventEmulator(object):
         self.max_frames_per_step = int(max_frames_per_step)
         self.exact_order = exact_order
         # shard = (rank, world, process_group): this instance owns a band of rows of every frame
-        # (v2e_b200.parallel.row_band); see _generate_sharded
+        # (v2e_b200.parallel.row_band); see _first_frame and _phase_frame
         self.shard = shard
         self.event_rows_hint = None   # initial event-buffer rows (default: max(2*H*W, 65536))
         self.seed = seed
@@ -424,26 +424,16 @@ class EventEmulator(object):
         self.output_height = H if self.output_height is None else self.output_height
         self._state_f64 = bool(self._lib.v2e_emu_state_is_f64(h))
 
-    def _init_fields(self, H, W):
-        """emulator.py:439-511 draw order: normal(pos), normal(neg), [normal(scidvs tau)], randn(noise_rate)."""
-        pos = neg = nr = None
-        if self.sigma_thres > 0:
-            pos = torch.clamp(self.rng.normal(self.pos_thres_nominal, self.sigma_thres, (H, W)), min=0.01)
-            neg = torch.clamp(self.rng.normal(self.neg_thres_nominal, self.sigma_thres, (H, W)), min=0.01)
-            pos, neg = pos.contiguous(), neg.contiguous()
-        if self.scidvs:     # emulator.py:480-483: SCIDVS_TAU_S * exp(normal(0, SCIDVS_TAU_COV))
-            tau = (0.01 * torch.exp(self.rng.normal(0, 0.5, (H, W)))).contiguous()
-            _lib.check(self._lib.v2e_emu_set_scidvs_tau(self._h, ctypes.c_void_p(tau.data_ptr())))
-        if self.leak_rate_hz > 0:
-            r = self.rng.randn((H, W))
-            nr = torch.exp(math.log(10) * self.noise_rate_cov_decades * r).contiguous()
-        p = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-        _lib.check(self._lib.v2e_emu_set_fields(self._h, p(pos), p(neg), p(nr)))
-
-    def _ensure_event_buffers(self, rows):
-        if self._ev_dev is None or self._ev_dev.shape[0] < rows:
-            rows = max(int(rows), 16)
-            self._ev_dev = torch.empty((rows, 4), dtype=torch.float32, device=self.device)
+    def _grow_event_buffer(self, rows, keep=0):
+        """Makes the device event buffer hold at least `rows` rows; a new buffer starts with the old one's first
+        `keep` rows."""
+        if self._ev_dev is not None and self._ev_dev.shape[0] >= rows:
+            return
+        old = self._ev_dev if keep else None
+        self._ev_dev = None
+        self._ev_dev = torch.empty((max(int(rows), 16), 4), dtype=torch.float32, device=self.device)
+        if keep:
+            self._ev_dev[:keep].copy_(old[:keep])
 
     def _rows_to_host(self, n_rows, base=0, copy=True):
         """Device rows -> host ndarray through a pinned staging buffer. copy=False returns a view of that
@@ -457,18 +447,49 @@ class EventEmulator(object):
         out = self._ev_pin[:n_rows].numpy()
         return out.copy() if copy else out
 
-    def _check_time(self, t_frame):
-        if t_frame < self.t_previous:
-            raise ValueError("this frame time={} must be later than previous frame time={}".format(
-                t_frame, self.t_previous))
+    def _frame_times(self, t_frames, T):
+        """t_frames as floats, checked: T of them, none earlier than the frame before (the first: t_previous)."""
+        t_frames = [float(t) for t in t_frames]
+        if len(t_frames) != T:
+            raise ValueError("t_frames length mismatch")
+        for a, b in zip([self.t_previous] + t_frames[:-1], t_frames):
+            if b < a:
+                raise ValueError("this frame time={} must be later than previous frame time={}".format(b, a))
+        return t_frames
 
-    def _first_frame(self, fr, code, t_frame):
-        H, W = fr.shape[-2], fr.shape[-1]
-        self._create(H, W)
+    def _first_frame(self, fr, code, t_frame, H):
+        """Creates the handle for rows [ye0, ye1) of frames of H rows (the whole frame; when sharded, this rank's
+        band plus the centre-surround halo rows), initialises the state from `fr` (those rows) and draws the
+        per-pixel fields in the reference's order (emulator.py:439-511): normal(pos), normal(neg),
+        [normal(scidvs tau)], randn(noise_rate). Every field is drawn for the whole frame, so that a band gets the
+        values a single-GPU run gets, and keeps rows [ye0, ye1)."""
+        from .parallel import band_with_halo, row_band
+        rank, world = (0, 1) if self.shard is None else self.shard[:2]
+        y0, y1 = row_band(H, rank, world)
+        if self.shard is not None and y1 == y0:
+            raise ValueError("more ranks than pixel rows")
+        K = self.cs_halo_rows(H)
+        ye0, ye1 = band_with_halo(H, rank, world, K)
+        W = fr.shape[-1]
+        # Philox counters and the conv2d summation order refer to the whole frame
+        self._create(ye1 - ye0, W, px_offset=ye0 * W, own=(y0 - ye0, y1 - y0) if K else None, cs_halo=K,
+                     full_px=H * W)
+        self._full_h, self._ye0, self._cs_K = H, ye0, K
+        rows = lambda t: t[ye0:ye1].contiguous()
+        L, p = self._lib, lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
         with torch.cuda.device(self.device):
-            _lib.check(self._lib.v2e_emu_first_frame(self._h, ctypes.c_void_p(fr.data_ptr()), code,
-                                                     float(t_frame), float(self.t_previous), self._stream()))
-            self._init_fields(H, W)
+            _lib.check(L.v2e_emu_first_frame(self._h, p(fr), code, float(t_frame), float(self.t_previous),
+                                             self._stream()))
+            pos = neg = nr = None
+            if self.sigma_thres > 0:
+                pos = rows(torch.clamp(self.rng.normal(self.pos_thres_nominal, self.sigma_thres, (H, W)), min=0.01))
+                neg = rows(torch.clamp(self.rng.normal(self.neg_thres_nominal, self.sigma_thres, (H, W)), min=0.01))
+            if self.scidvs:     # emulator.py:480-483: SCIDVS_TAU_S * exp(normal(0, SCIDVS_TAU_COV))
+                tau = rows(0.01 * torch.exp(self.rng.normal(0, 0.5, (H, W))))
+                _lib.check(L.v2e_emu_set_scidvs_tau(self._h, p(tau)))
+            if self.leak_rate_hz > 0:
+                nr = rows(torch.exp(math.log(10) * self.noise_rate_cov_decades * self.rng.randn((H, W))))
+            _lib.check(L.v2e_emu_set_fields(self._h, p(pos), p(neg), p(nr)))
         self._initialized = True
         # the reference returns before `self.t_previous = t_frame` (emulator.py:717 vs :1011)
 
@@ -477,20 +498,21 @@ class EventEmulator(object):
         """emulator.py:619: returns float32 [N,4] rows [t, x, y, +-1] or None."""
         t_frame = float(t_frame)
         self.frame_counter += 1
-        self._check_time(t_frame)
+        self._frame_times([t_frame], 1)
         fr, code = self._to_device_frames(new_frame)
         if fr.dim() != 2:
             raise ValueError("new_frame must be [height, width]")
         if self.shard is not None:
-            return self._generate_sharded(fr, code, t_frame)
+            ye0, ye1 = self.ext_band(fr.shape[0])
+            return self._generate_band(fr[ye0:ye1], code, t_frame, fr.shape[0])
         if not self._initialized:
-            self._first_frame(fr, code, t_frame)
+            self._first_frame(fr, code, t_frame, fr.shape[0])
             return None
         if fr.shape != (self._H, self._W):
             raise ValueError("frame size changed")
         per_frame_rng = (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or self.photoreceptor_noise)
         if self.rng_mode == "replay" and (per_frame_rng or self.exact_order):
-            ev = self._generate_replay(fr, code, t_frame)
+            ev = self._phase_frame(fr, code, t_frame)
         else:
             total, _ = self._run_step(fr.unsqueeze(0), code, [t_frame])
             ev = self._rows_to_host(total)
@@ -533,52 +555,88 @@ class EventEmulator(object):
         self.photoreceptor_noise_vrms = v
         return v
 
-    # replay path: one frame, host draws interleaved exactly like the reference ----------------
-    def _generate_replay(self, fr, code, t_frame):
-        H, W, n = self._H, self._W, self._H * self._W
+    # one frame through the single-frame phase functions, host draws interleaved like the reference's ---------
+    def _phase_frame(self, fr, code, t_frame, return_device=False):
+        """One frame -- this handle's rows of it -- through the single-frame phases: every frame of a sharded
+        emulator, and unsharded frames in replay mode. In replay mode the host draws the per-frame fields and replays
+        the per-iteration randperm calls in the reference's order (emulator.py:694-698, 868, 897). Sharded, the
+        frame-global maximum (emulator.py:773-775) is all-reduced (MAX) between the update and the refractory filter.
+        Returns the rows (y of the whole frame) in the canonical order -- unsharded with exact_order, the reference's
+        own order -- on the host, or on the device with return_device, where device-RNG rows keep the kernels' order.
+        None when there are none."""
+        import torch.distributed as dist
+        sharded, replay = self.shard is not None, self.rng_mode == "replay"
+        group = self.shard[2] if sharded else None
+        H, W, ye0 = self._full_h, self._W, self._ye0
         L, h = self._lib, self._h
-        leak_on = self.leak_rate_hz > 0
-        shot_on = self.shot_noise_rate_hz > 0 and not self.photoreceptor_noise      # emulator.py:893
+        shot_pending = replay and self.shot_noise_rate_hz > 0 and not self.photoreceptor_noise      # emulator.py:893
+        tp = float(self.t_previous)
+        p = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
+
+        def field(draw):
+            # drawn for the whole frame, so that a band gets the values a single-GPU run gets; this handle's rows
+            return draw((H, W))[ye0:ye0 + self._H].contiguous().to(self.device)
         with torch.cuda.device(self.device):
             st = self._stream()
-            lr_dev = None
-            tp = float(self.t_previous)
-            if self.photoreceptor_noise:    # emulator.py:694-698: amplitude, then the randn draw, before the leak's
+            if replay and self.photoreceptor_noise:
+                # emulator.py:694-698: amplitude, then the randn draw, before the leak's
                 vr = (ctypes.c_double * 1)(self._pr_vrms(t_frame - tp))
-                pr_dev = self.rng.randn((H, W)).contiguous().to(self.device, non_blocking=False)
-                _lib.check(L.v2e_emu_set_pr_noise(h, ctypes.c_void_p(pr_dev.data_ptr()), vr, 1))
-            if leak_on:
-                lr_dev = self.rng.randn((H, W)).contiguous().to(self.device, non_blocking=False)
-            self._ensure_event_buffers(self.event_rows_hint or max(4 * n, 1 << 16))
+                pr_dev = field(self.rng.randn)
+                _lib.check(L.v2e_emu_set_pr_noise(h, p(pr_dev), vr, 1))
+            lr_dev = field(self.rng.randn) if replay and self.leak_rate_hz > 0 else None
+            self._grow_event_buffer(self.event_rows_hint or max(4 * self._H * W, 1 << 16))
             cap = self._ev_dev.shape[0]
             fp = ctypes.c_void_p(fr.data_ptr())
-            _lib.check(L.v2e_emu_phase_count(h, fp, code, t_frame, tp,
-                                             None if lr_dev is None else ctypes.c_void_p(lr_dev.data_ptr()),
-                                             None, 1 if shot_on else 0, cap, 0, st))
-            max_n = ctypes.c_int32(0)
-            counts = np.zeros(2 * self.iter_cap, np.uint32)
-            _lib.check(L.v2e_emu_read_counts(h, ctypes.byref(max_n), counts.ctypes.data_as(ctypes.c_void_p),
-                                             counts.size, st))
-            m = max_n.value
-            counts = counts[:2 * m].astype(np.int64)
-            sig_total = int(counts.sum())
-            # replay the per-iteration shuffles now: the shot draw comes after them (emulator.py:868, 897)
-            perms = []
-            for it in range(m):
-                k = int(counts[2 * it] + counts[2 * it + 1])
-                perms.append(self.rng.randperm(k).numpy() if k > 0 else None)
-            if shot_on:
-                sr_dev = self.rng.rand((H, W)).contiguous().to(self.device, non_blocking=False)
-                _lib.check(L.v2e_emu_phase_shot(h, fp, code, t_frame, tp, ctypes.c_void_p(sr_dev.data_ptr()),
-                                                cap, st))
-            _lib.check(L.v2e_emu_phase_emit(h, t_frame, tp, ctypes.c_void_p(self._ev_dev.data_ptr()), cap, st))
+            if not sharded:
+                _lib.check(L.v2e_emu_phase_count(h, fp, code, t_frame, tp, p(lr_dev), None, 1 if shot_pending else 0,
+                                                 cap, 0, st))
+            else:
+                if self._cs_K:
+                    self._cs_iterate(fp, code, t_frame, tp, cap, p(lr_dev), st, W)
+                else:
+                    _lib.check(L.v2e_emu_phase_update(h, fp, code, t_frame, tp, p(lr_dev), None, cap, 0, st))
+                mx = torch.as_tensor(_DevView(L.v2e_emu_max_n_dev(h), (1,), "<i4", self), device=self.device)
+                dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=group)
+                _lib.check(L.v2e_emu_phase_filter(h, t_frame, tp, cap, 0 if shot_pending else 1, st))
+            counts = perms = None
+            if replay or not return_device:
+                # per-(iteration, polarity) counts on the host (one synchronisation): the replayed randperm draws and
+                # the canonical row order need them
+                max_n = ctypes.c_int32(0)
+                counts = np.zeros(2 * self.iter_cap, np.uint32)
+                _lib.check(L.v2e_emu_read_counts(h, ctypes.byref(max_n), counts.ctypes.data_as(ctypes.c_void_p),
+                                                 counts.size, st))
+                counts = counts[:2 * max_n.value].astype(np.int64)
+            if replay:
+                # one randperm(n_i) per iteration, n_i = the events of the WHOLE frame (emulator.py:868): summed over
+                # the ranks when sharded, so that the seeded generator stays in step with an unsharded run
+                tot = counts
+                if sharded and len(counts):
+                    tot = torch.from_numpy(counts.copy()).to(self.device)
+                    dist.all_reduce(tot, op=dist.ReduceOp.SUM, group=group)
+                    tot = tot.cpu().numpy()
+                perms = []
+                for it in range(len(counts) // 2):
+                    k = int(tot[2 * it] + tot[2 * it + 1])
+                    perms.append(self.rng.randperm(k).numpy() if k > 0 else None)
+            if shot_pending:
+                sr_dev = field(self.rng.rand)
+                _lib.check(L.v2e_emu_phase_shot(h, fp, code, t_frame, tp, p(sr_dev), cap, st))
+            _lib.check(L.v2e_emu_phase_emit(h, t_frame, tp, p(self._ev_dev), cap, st))
             fi = self._collect_one(fp, code, t_frame, tp, st)
             self.last_frame_info = fi
-            ev = self._rows_to_host(int(fi.n_events))
+            n_ev = int(fi.n_events)
+            ev = self._ev_dev[:n_ev].clone() if counts is None else self._rows_to_host(n_ev)
         self._account(fi)
-        if fi.n_events == 0:
+        if n_ev == 0:
             return None
-        return self._canonical_then_shuffle(ev, counts, perms, int(fi.n_shot_on), int(fi.n_shot_off))
+        if counts is not None:
+            # a band's rows cannot take the reference's order: that shuffles the whole frame's rows
+            ev = self._canonical_then_shuffle(ev, counts, perms if not sharded and self.exact_order else None,
+                                              int(fi.n_shot_on), int(fi.n_shot_off))
+        if ye0:
+            ev[:, 2] += ye0
+        return torch.from_numpy(ev).to(self.device) if return_device and counts is not None else ev
 
     def _collect_one(self, fp, code, t_frame, tp, st):
         """Control block of the single frame just emitted. On V2E_E_CAPACITY (the frame is counted, its state
@@ -588,7 +646,7 @@ class EventEmulator(object):
         done, rows = ctypes.c_int(0), ctypes.c_uint64(0)
         rc = L.v2e_emu_collect(h, info, 1, ctypes.byref(done), ctypes.byref(rows), st)
         if rc == _lib.V2E_E_CAPACITY:
-            self._ensure_event_buffers(int(info[0].n_events) + 1024)
+            self._grow_event_buffer(int(info[0].n_events) + 1024)
             ts = (ctypes.c_double * 1)(t_frame)
             _lib.check(L.v2e_emu_step(h, fp, code, 1, ts, tp, None, None,
                                       ctypes.c_void_p(self._ev_dev.data_ptr()), self._ev_dev.shape[0], 0,
@@ -599,11 +657,6 @@ class EventEmulator(object):
         return info[0]
 
     # pixel-sharded path (SURVEY.md 8e, BASELINE config 5): this rank owns rows [y0, y1) ---------------
-    def _band(self, H):
-        from .parallel import row_band
-        rank, world, _ = self.shard
-        return row_band(H, rank, world)
-
     def cs_halo_rows(self, H):
         """Halo rows K of the pixel-sharded centre-surround model = Euler steps between two halo exchanges
         (0 when this emulator is not a sharded centre-surround one). Bounded by the smallest band."""
@@ -616,14 +669,8 @@ class EventEmulator(object):
 
     def ext_band(self, H):
         """Rows [ye0, ye1) this rank's handle covers: its own band plus the halo rows of the neighbours."""
-        y0, y1 = self._band(H)
-        K = self.cs_halo_rows(H)
-        return max(0, y0 - K), min(H, y1 + K)
-
-    def _full_then_band(self, draw, H, W, y0, y1):
-        """Every rank draws the FULL field from the same seeded generator (so the streams stay aligned
-        with a single-GPU run) and keeps its rows."""
-        return draw((H, W))[y0:y1].contiguous()
+        from .parallel import band_with_halo
+        return band_with_halo(H, self.shard[0], self.shard[1], self.cs_halo_rows(H))
 
     def generate_events_band(self, band_frame, t_frame, full_height):
         """Pixel-sharded operation with the rows already cut: band_frame is [y1-y0, W], this rank's rows
@@ -633,123 +680,21 @@ class EventEmulator(object):
             raise RuntimeError("generate_events_band needs shard=(rank, world, group)")
         t_frame = float(t_frame)
         self.frame_counter += 1
-        self._check_time(t_frame)
+        self._frame_times([t_frame], 1)
         fr, code = self._to_device_frames(band_frame)
         y0, y1 = self.ext_band(int(full_height))       # the band (+ halo rows for the centre-surround model)
         if fr.dim() != 2 or fr.shape[0] != y1 - y0:
             raise ValueError("band_frame must hold rows [%d, %d) of the frame" % (y0, y1))
-        return self._generate_sharded(fr, code, t_frame, full_height=int(full_height))
+        return self._generate_band(fr, code, t_frame, int(full_height))
 
-    def _generate_sharded(self, fr_full, code, t_frame, full_height=None, return_device=False):
-        import torch.distributed as dist
-        rank, world, group = self.shard
-        if full_height is None:
-            H, W = fr_full.shape
-        else:
-            H, W = full_height, fr_full.shape[1]
-        y0, y1 = self._band(H)
-        # rows the handle covers: the band itself, plus K halo rows either side for the centre-surround model
-        K = self.cs_halo_rows(H)
-        ye0, ye1 = self.ext_band(H)
-        if full_height is None:
-            fr = fr_full[ye0:ye1].contiguous()
-        else:
-            if fr_full.shape[0] != ye1 - ye0:
-                raise ValueError("band_frame must hold rows [%d, %d) of the frame (band + halo)" % (ye0, ye1))
-            fr = fr_full.contiguous()
-        hb = y1 - y0
-        if hb == 0:
-            raise ValueError("more ranks than pixel rows")
-        he = ye1 - ye0
-        L = self._lib
+    def _generate_band(self, fr, code, t_frame, H, return_device=False):
+        """Rows ext_band(H) of one frame of H rows."""
         if not self._initialized:
-            # Philox counters and the conv2d summation order refer to the whole frame
-            self._create(he, W, px_offset=ye0 * W, own=(y0 - ye0, hb) if K else None, cs_halo=K, full_px=H * W)
-            self._cs_K = K
-            with torch.cuda.device(self.device):
-                _lib.check(L.v2e_emu_first_frame(self._h, ctypes.c_void_p(fr.data_ptr()), code, float(t_frame),
-                                                 float(self.t_previous), self._stream()))
-                pos = neg = nr = None
-                if self.sigma_thres > 0:
-                    pos = torch.clamp(self.rng.normal(self.pos_thres_nominal, self.sigma_thres, (H, W)), min=0.01)[ye0:ye1].contiguous()
-                    neg = torch.clamp(self.rng.normal(self.neg_thres_nominal, self.sigma_thres, (H, W)), min=0.01)[ye0:ye1].contiguous()
-                if self.leak_rate_hz > 0:
-                    nr = torch.exp(math.log(10) * self.noise_rate_cov_decades * self.rng.randn((H, W)))[ye0:ye1].contiguous()
-                p = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-                _lib.check(L.v2e_emu_set_fields(self._h, p(pos), p(neg), p(nr)))
-            self._initialized = True
-            self._full_h = H
+            self._first_frame(fr, code, t_frame, H)
             return None
-        n = he * W
-        h = self._h
-        leak_on, shot_on = self.leak_rate_hz > 0, self.shot_noise_rate_hz > 0
-        replay = self.rng_mode == "replay"
-        with torch.cuda.device(self.device):
-            st = self._stream()
-            lr_dev = None
-            if leak_on and replay:
-                lr_dev = self._full_then_band(self.rng.randn, H, W, ye0, ye1).to(self.device)
-            self._ensure_event_buffers(self.event_rows_hint or max(4 * n, 1 << 16))
-            cap = self._ev_dev.shape[0]
-            tp = float(self.t_previous)
-            fp = ctypes.c_void_p(fr.data_ptr())
-            lrp = None if lr_dev is None else ctypes.c_void_p(lr_dev.data_ptr())
-            if K:
-                self._cs_iterate(fp, code, t_frame, tp, cap, lrp, st, W)
-            else:
-                _lib.check(L.v2e_emu_phase_update(h, fp, code, t_frame, tp, lrp, None, cap, 0, st))
-            # the frame-global maximum (emulator.py:773-775): in-place MAX over the ranks
-            mx = torch.as_tensor(_DevView(L.v2e_emu_max_n_dev(h), (1,), "<i4", self), device=self.device)
-            dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=group)
-            shot_pending = shot_on and replay
-            _lib.check(L.v2e_emu_phase_filter(h, t_frame, tp, cap, 0 if shot_pending else 1, st))
-            m, counts = 0, None
-            if replay or not return_device:
-                # per-(iteration, polarity) counts on the host: the replayed randperm draws and the canonical row
-                # order need them (one synchronisation); the device-RNG batch path skips this
-                max_n = ctypes.c_int32(0)
-                counts = np.zeros(2 * self.iter_cap, np.uint32)
-                _lib.check(L.v2e_emu_read_counts(h, ctypes.byref(max_n), counts.ctypes.data_as(ctypes.c_void_p),
-                                                 counts.size, st))
-                m = max_n.value
-                counts = counts[:2 * m].astype(np.int64)
-            if replay:
-                # keep the seeded generator aligned with an unsharded run: the reference draws one
-                # randperm(n_i) per iteration with n_i = events of the WHOLE frame (emulator.py:868)
-                tot = torch.from_numpy(counts.copy()).to(self.device)
-                if m > 0:
-                    dist.all_reduce(tot, op=dist.ReduceOp.SUM, group=group)
-                tot = tot.cpu().numpy()
-                for it in range(m):
-                    k = int(tot[2 * it] + tot[2 * it + 1])
-                    if k > 0:
-                        self.rng.randperm(k)
-            if shot_pending:
-                sr_dev = self._full_then_band(self.rng.rand, H, W, ye0, ye1).to(self.device)
-                _lib.check(L.v2e_emu_phase_shot(h, fp, code, t_frame, tp, ctypes.c_void_p(sr_dev.data_ptr()), cap, st))
-            _lib.check(L.v2e_emu_phase_emit(h, t_frame, tp, ctypes.c_void_p(self._ev_dev.data_ptr()), cap, st))
-            fi = self._collect_one(fp, code, t_frame, tp, st)
-            self.last_frame_info = fi
-            if return_device and not replay:
-                self._account(fi)
-                self.t_previous = t_frame
-                if fi.n_events == 0:
-                    return None
-                evd = self._ev_dev[:int(fi.n_events)].clone()
-                evd[:, 2] += ye0
-                return evd
-            ev = self._rows_to_host(int(fi.n_events))
-        self._account(fi)
+        ev = self._phase_frame(fr, code, t_frame, return_device)
         self.t_previous = t_frame
-        if fi.n_events == 0:
-            return None
-        saved, self.exact_order = self.exact_order, False
-        try:
-            ev = self._canonical_then_shuffle(ev, counts, [None] * m, int(fi.n_shot_on), int(fi.n_shot_off))
-        finally:
-            self.exact_order = saved
-        ev[:, 2] += ye0
-        return torch.from_numpy(ev).to(self.device) if return_device else ev
+        return ev
 
     def _cs_iterate(self, fp, code, t_frame, tp, cap, lrp, st, W):
         """Centre-surround model over row bands (emulator.py:1061-1124; BASELINE config 5): the Euler iteration in
@@ -807,13 +752,8 @@ class EventEmulator(object):
         y0, y1 = self.ext_band(H)        # = the band, unless the centre-surround model adds halo rows
         if fr.dim() != 3 or fr.shape[1] != y1 - y0:
             raise ValueError("band_frames must be [T, %d, W]: rows [%d, %d) of every frame" % (y1 - y0, y0, y1))
-        t_frames = [float(t) for t in t_frames]
         T = fr.shape[0]
-        if len(t_frames) != T:
-            raise ValueError("t_frames length mismatch")
-        for a, b in zip([self.t_previous] + t_frames[:-1], t_frames):
-            if b < a:
-                raise ValueError("this frame time={} must be later than previous frame time={}".format(b, a))
+        t_frames = self._frame_times(t_frames, T)
         L = self._lib
         out, offs = [], [0]
         state = {"total": 0}
@@ -827,7 +767,7 @@ class EventEmulator(object):
             ts = (ctypes.c_double * Tc)(*t_frames[a:b])
             with torch.cuda.device(self.device):
                 st = self._stream()
-                self._ensure_event_buffers(self.event_rows_hint or max(2 * n, 1 << 16))
+                self._grow_event_buffer(self.event_rows_hint or max(2 * n, 1 << 16))
                 rc = L.v2e_emu_fused_count(self._h, ctypes.c_void_p(chunk.data_ptr()), code, Tc, ts,
                                            float(self.t_previous), st)
                 if rc == _lib.V2E_E_UNSUPPORTED:
@@ -845,8 +785,7 @@ class EventEmulator(object):
                     if rc != _lib.V2E_E_CAPACITY:
                         break
                     need = max(int(info[k].ev_base) + int(info[k].n_events) for k in range(Tc))
-                    self._ev_dev = None
-                    self._ensure_event_buffers(2 * need)
+                    self._grow_event_buffer(2 * need)
                 if rc == _lib.V2E_E_FALLBACK:
                     return int(done.value)
                 _lib.check(rc)
@@ -866,7 +805,7 @@ class EventEmulator(object):
         def frame_by_frame(a, b):
             for k in range(a, b):
                 self.frame_counter += 1
-                evk = self._generate_sharded(fr[k], code, t_frames[k], full_height=H, return_device=True)
+                evk = self._generate_band(fr[k], code, t_frames[k], H, return_device=True)
                 if evk is not None:
                     out.append(evk)
                     state["total"] += len(evk)
@@ -898,11 +837,12 @@ class EventEmulator(object):
     def _canonical_then_shuffle(self, ev, counts, perms, shot_on, shot_off):
         """Device rows of one (iteration, polarity) group come in no particular order. The reference
         builds each iteration as ON rows then OFF rows in row-major pixel order and shuffles it with
-        randperm (emulator.py:861-870, 1024-1059); shot rows are appended unshuffled (:906-919)."""
+        randperm (emulator.py:861-870, 1024-1059); shot rows are appended unshuffled (:906-919).
+        perms: the replayed permutation of every iteration, or None to keep the rows in that canonical order."""
         W = self._W
         out = np.empty_like(ev)
         off = 0
-        for it in range(len(perms)):
+        for it in range(len(counts) // 2):
             c_on, c_off = int(counts[2 * it]), int(counts[2 * it + 1])
             k = c_on + c_off
             if k == 0:
@@ -911,7 +851,7 @@ class EventEmulator(object):
             key = blk[:, 2].astype(np.int64) * W + blk[:, 1].astype(np.int64)
             key[c_on:] += (1 << 40)   # keep OFF rows after ON rows
             blk = blk[np.argsort(key, kind="stable")]
-            out[off:off + k] = blk[perms[it]] if self.exact_order else blk
+            out[off:off + k] = blk if perms is None else blk[perms[it]]
             off += k
         for c in (shot_on, shot_off):
             if c:
@@ -939,8 +879,7 @@ class EventEmulator(object):
         ts = (ctypes.c_double * T)(*[float(t) for t in t_frames])
         with torch.cuda.device(self.device):
             st = self._stream()
-            if self._ev_dev is None:
-                self._ensure_event_buffers(self.event_rows_hint or max(2 * n, 1 << 16))
+            self._grow_event_buffer(self.event_rows_hint or max(2 * n, 1 << 16))
             info = (_lib.V2eFrameInfo * T)()
             done, rows = ctypes.c_int(0), ctypes.c_uint64(0)
             first, resume, base = 0, 0, int(base_row)
@@ -964,11 +903,7 @@ class EventEmulator(object):
                 # a multi-frame (fused) step reports the rows of every frame of the chunk; the frame-by-frame
                 # kernels only those up to the frame that did not fit
                 need = max(int(info[f].ev_base) + int(info[f].n_events) for f in range(first, T))
-                old = self._ev_dev
-                self._ev_dev = None
-                self._ensure_event_buffers(max(2 * need, 2 * old.shape[0]))
-                self._ev_dev[:base].copy_(old[:base])
-                del old
+                self._grow_event_buffer(max(2 * need, 2 * self._ev_dev.shape[0]), keep=base)
             total = int(rows.value)
             offsets = np.array([int(info[f].ev_base) for f in range(T)] + [total], np.int64)
             for f in range(T):
@@ -987,20 +922,18 @@ class EventEmulator(object):
                                           self.photoreceptor_noise):
             raise RuntimeError("generate_events_batch with per-frame noise needs rng_mode='device' "
                                "(replay mode must interleave host draws frame by frame)")
+        if self.shard is not None:
+            raise RuntimeError("generate_events_batch runs whole frames; a sharded emulator takes "
+                               "generate_events_band_batch")
         fr, code = self._to_device_frames(frames)
         if fr.dim() != 3:
             raise ValueError("frames must be [T, height, width]")
-        t_frames = [float(t) for t in t_frames]
         T = fr.shape[0]
-        if len(t_frames) != T:
-            raise ValueError("t_frames length mismatch")
-        for a, b in zip([self.t_previous] + t_frames[:-1], t_frames):
-            if b < a:
-                raise ValueError("this frame time={} must be later than previous frame time={}".format(b, a))
+        t_frames = self._frame_times(t_frames, T)
         offs = [0]
         start = 0
         if not self._initialized:
-            self._first_frame(fr[0], code, t_frames[0])
+            self._first_frame(fr[0], code, t_frames[0], fr.shape[1])
             self.frame_counter += 1
             offs.append(0)
             start = 1

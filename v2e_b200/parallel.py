@@ -115,11 +115,3 @@ def merge_by_time(streams):
     allr = torch.cat(streams, 0)
     order = torch.argsort(allr[:, 0], stable=True)
     return allr[order]
-
-
-def allreduce_max_int(value, device, group=None):
-    """max over ranks of a small integer (frame-global max_n when one clip is pixel-sharded,
-    emulator.py:773-775)."""
-    t = torch.tensor([int(value)], dtype=torch.int64, device=device)
-    dist.all_reduce(t, op=dist.ReduceOp.MAX, group=group)
-    return int(t.item())
