@@ -54,7 +54,7 @@ typedef struct V2eEmuCfg {
     int32_t hdr;                    /* emulator.py:110 hdr / log_input */
     double pos_thres_nominal;       /* emulator.py:88 */
     double neg_thres_nominal;       /* emulator.py:89 */
-    double cutoff_hz;               /* emulator.py:91 ; >0 (or hdr) makes lp/base float64 */
+    double cutoff_hz;               /* emulator.py:91 ; >0 (or hdr) makes lp/base (and surround) float64 */
     double leak_rate_hz;            /* emulator.py:92 */
     double leak_jitter_fraction;    /* emulator.py:96 */
     double refractory_period_s;     /* emulator.py:93 */
@@ -207,23 +207,24 @@ int32_t *v2e_emu_max_n_dev(V2eEmu *h);
  * function of the frames), the surround on the halo rows comes from the neighbours. Per frame:
  *   v2e_emu_cs_begin      low-pass of the band, Euler-step plan (*num_steps, emulator.py:1076-1078)
  *   for chunks [s0, s1) of at most K steps:
- *       v2e_emu_cs_pack        own edge rows of the current surround -> v2e_emu_cs_send_dev()  [2][K][W] float64
+ *       v2e_emu_cs_pack        own edge rows of the current surround -> v2e_emu_cs_send_dev()  [2][K][W] of the
+ *                              state dtype (float64 when v2e_emu_state_is_f64, else float32)
  *                              ([0] = the top K own rows, [1] = the bottom K)
  *       (caller: exchange with the neighbours, e.g. one all-gather of every rank's send buffer)
  *       v2e_emu_cs_unpack_from the neighbours' rows -> halo rows, read where the exchange left them:
  *                              rows_above_dev = the upper neighbour's bottom K rows [K][W], rows_below_dev = the lower
- *                              neighbour's top K rows; NULL at the image border
+ *                              neighbour's top K rows (state dtype); NULL at the image border
  *       v2e_emu_cs_chunk      steps s0 .. s1-1 (each into its own ring buffer; maxima over the own rows)
  *       (caller: all-reduce MAX of the uint64 at v2e_emu_cs_max_dev()[s0 .. s1) -- non-negative doubles order
- *        like their bit patterns)
+ *        like their bit patterns; a float32 state's maxima are float32 magnitudes widened to double, exactly)
  *       v2e_emu_cs_advance     first step with max|change| <= 1e-5 ends the iteration (device side, no host sync)
  *   v2e_emu_cs_update     the update kernel on the converged surround (then v2e_emu_max_n_dev ... as above)
  * Everything is enqueued on `stream`; nothing synchronises. */
 int v2e_emu_cs_begin(V2eEmu *h, const void *frame_dev, int frame_dtype, double t_frame, double t_previous,
                      uint64_t capacity, uint64_t ev_base_start, int *num_steps, void *stream);
 int v2e_emu_cs_pack(V2eEmu *h, void *stream);
-int v2e_emu_cs_unpack_from(V2eEmu *h, const double *rows_above_dev, const double *rows_below_dev, void *stream);
-double *v2e_emu_cs_send_dev(V2eEmu *h);
+int v2e_emu_cs_unpack_from(V2eEmu *h, const void *rows_above_dev, const void *rows_below_dev, void *stream);
+void *v2e_emu_cs_send_dev(V2eEmu *h);
 int v2e_emu_cs_chunk(V2eEmu *h, int s0, int s1, void *stream);
 uint64_t *v2e_emu_cs_max_dev(V2eEmu *h);
 int v2e_emu_cs_advance(V2eEmu *h, int s0, int s1, void *stream);
@@ -259,9 +260,9 @@ int v2e_emu_profile_read4(V2eEmu *h, float *ms_sum4, int *launches4, void *strea
 /* State access for parity probes (emulator.py:756-764 reads them by name): the device pointer of a state
  * array, for zero-copy views, or NULL when this configuration has none. which:
  * 0 lp_log_frame, 1 base_log_frame, 2 pos_thres, 3 neg_thres, 4 noise_rate_array,
- * 5 timestamp_mem, 6 cs_surround_frame (float64), 7 scidvs_highpass (state dtype), 8 photoreceptor_noise_arr
- * (float32), 9 scidvs_tau_arr (float32). lp, base and the high-pass have the state dtype: float64 when
- * v2e_emu_state_is_f64, else float32; the others are float32. */
+ * 5 timestamp_mem, 6 cs_surround_frame (state dtype), 7 scidvs_highpass (state dtype), 8 photoreceptor_noise_arr
+ * (float32), 9 scidvs_tau_arr (float32). lp, base, the surround and the high-pass have the state dtype: float64 when
+ * v2e_emu_state_is_f64, else float32 (cutoff_hz == 0 without hdr, as in the reference); the others are float32. */
 int v2e_emu_state_is_f64(V2eEmu *h);
 void *v2e_emu_state_ptr(V2eEmu *h, int which);
 

@@ -74,6 +74,7 @@ _SIGS = {
     "v2e_emu_max_n_dev": (_vp, [_vp]),
     "v2e_emu_cs_begin": (_i, [_vp, _vp, _i, _d, _d, _u64, _u64, ctypes.POINTER(_i), _vp]),
     "v2e_emu_cs_pack": (_i, [_vp, _vp]),
+    # the halo exchange buffers (send, rows above / below) hold the state dtype: float64, or float32 at cutoff_hz = 0
     "v2e_emu_cs_unpack_from": (_i, [_vp, _vp, _vp, _vp]),
     "v2e_emu_cs_send_dev": (_vp, [_vp]),
     "v2e_emu_cs_chunk": (_i, [_vp, _i, _i, _vp]),

@@ -65,8 +65,8 @@ struct EmuDev {                         // passed by value to every kernel
     uint64_t seed;
     void *lp, *base;
     float *pos_thres, *neg_thres, *noise_rate, *tmem;
-    double *surround;                   // CSDVS h, ping buffer (cs_cur == 0)
-    double *surround2;                  // pong buffer
+    void *surround;                     // CSDVS h, ping buffer (cs_cur == 0); state dtype, like lp
+    void *surround2;                    // pong buffer
     int32_t *cs_cur;                    // which buffer holds the current surround
     unsigned long long *cs_max;         // [cs_cap] max|change| of every Euler step of the current frame (double bits)
     int32_t cs_cap;
@@ -76,7 +76,8 @@ struct EmuDev {                         // passed by value to every kernel
     int32_t own_lo, own_hi;             // pixels [own_lo, own_hi) emit events (a sharded centre-surround handle also
                                         // carries halo rows above / below its own rows); 0 / n otherwise
     int32_t *cs_done;                   // sharded: the Euler iteration of this frame ended in an earlier chunk
-    double *cs_bufs;                    // sharded: ring of cs_ring buffers of cs_stride doubles (replaces surround / surround2)
+    void *cs_bufs;                      // sharded: ring of cs_ring buffers of cs_stride state values (replaces surround /
+                                        // surround2)
     size_t cs_stride;
     int16_t *rec;
     uint32_t *act_list;                 // [n_pad] pixel indices with a non-zero record (built by the update kernel)
@@ -469,7 +470,7 @@ __global__ void __launch_bounds__(kThreads) emu_first_frame_kernel(EmuDev d, Fra
     load_frame4<FT>(frame, i0, d.n, x);
     S lp[4], base[4];
     float tm[4];
-    double su[4];
+    S su[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) {
         double xv = x[k];
@@ -484,26 +485,32 @@ __global__ void __launch_bounds__(kThreads) emu_first_frame_kernel(EmuDev d, Fra
                 v = (1.0 - eps) * ln + eps * ln;      // lp seeded with log_new, still filtered once
             }
             lp[k] = (S)v;
-            su[k] = v;
+            su[k] = (S)v;
             base[k] = (S)(d.csdvs ? v - v : v);      // emulator.py:714
         } else {
             lp[k] = (S)lnf;
-            base[k] = (S)lnf;
-            su[k] = 0.0;
+            su[k] = (S)lnf;
+            base[k] = (S)(d.csdvs ? lnf - lnf : lnf);
         }
         tm[k] = 0.0f - d.refr_f;                     // emulator.py:508-511
     }
     st4((S *)d.lp, i0, lp);
     st4((S *)d.base, i0, base);
     if (d.refr_on) st4(d.tmem, i0, tm);
-    if (d.csdvs) st4(d.cs_bufs ? d.cs_bufs : d.surround, i0, su);     // v2e_emu_first_frame resets cs_cur to 0
+    if (d.csdvs) st4(d.cs_bufs ? (S *)d.cs_bufs : (S *)d.surround, i0, su);     // v2e_emu_first_frame resets cs_cur to 0
 }
 
 // ---------------------------------------------------------------------------------------------
 // centre-surround model (emulator.py:1061-1124), only when cs_lambda_pixels is set
 // ---------------------------------------------------------------------------------------------
-// photoreceptor low-pass alone: the surround diffusion needs the whole new lp field first
-template <int FT>
+// ring buffer k of the surround (the ping-pong pair unless pixel-sharded)
+template <typename S> __device__ __forceinline__ S *cs_buf(const EmuDev &d, int k) {
+    return d.cs_bufs ? (S *)d.cs_bufs + (size_t)k * d.cs_stride : (S *)(k ? d.surround2 : d.surround);
+}
+
+// photoreceptor low-pass alone: the surround diffusion needs the whole new lp field first. A float32 state has no
+// low-pass (cutoff_hz == 0): lp is the float32 lin-log value (emulator_utils.py:75-77)
+template <typename S, int FT>
 __global__ void __launch_bounds__(kThreads) emu_lp_kernel(EmuDev d, FrameParams p, const void *frame) {
     __shared__ float s_lut[256];
     if (*(volatile int32_t *)d.abort_flag) return;
@@ -511,29 +518,41 @@ __global__ void __launch_bounds__(kThreads) emu_lp_kernel(EmuDev d, FrameParams 
     __syncthreads();
     const int i0 = (blockIdx.x * kThreads + threadIdx.x) * kVec;
     if (i0 >= d.n) return;
-    double x[4], lp[4];
+    double x[4];
+    S lp[4];
     load_frame4<FT>(frame, i0, d.n, x);
-    ld4((const double *)d.lp, i0, lp);
+    if (sizeof(S) == 8) ld4((const S *)d.lp, i0, lp);
 #pragma unroll
     for (int k = 0; k < 4; k++) {
         const double xv = x[k];
         double ln;
         if (d.hdr) ln = xv;
         else ln = (double)((FT == V2E_U8 || (xv >= 0.0 && xv <= 255.0 && xv == floor(xv))) ? s_lut[(int)xv] : lin_log_eval(xv));
-        if (d.lowpass_on) {
+        if (sizeof(S) == 8 && d.lowpass_on) {
             double eps = ((xv + 20.0) / 275.0) * p.eps_scale;
             if (eps > 1.0) eps = 1.0;
-            lp[k] = (1.0 - eps) * lp[k] + eps * ln;
+            lp[k] = (S)((1.0 - eps) * (double)lp[k] + eps * ln);
         } else {
-            lp[k] = ln;
+            lp[k] = (S)ln;                          // float32 state: exact, ln is a widened float32
         }
     }
-    st4((double *)d.lp, i0, lp);
+    st4((S *)d.lp, i0, lp);
+}
+
+// change = alpha_p*(p - h) + h_term of one pixel (emulator.py:1111-1117). float64 state: p_term and change are float64,
+// h_term is promoted. float32 state (cutoff_hz == 0): every op is float32, alpha_p a Python float rounded to float32.
+__device__ __forceinline__ double cs_change(double alpha_p, double p, double h, float h_term) {
+    return alpha_p * (p - h) + (double)h_term;
+}
+__device__ __forceinline__ float cs_change(double alpha_p, float p, float h, float h_term) {
+    const float p_term = (float)alpha_p * (p - h);
+    return p_term + h_term;
 }
 
 // One Euler step h += alpha_p*(p - h) + alpha_h*lap(float32(h)) with replicate padding
-// (emulator.py:1105-1121). p, h float64; the 3x3 stencil is a float32 conv2d whose summation order is the
-// reference's CPU backend's (see oracle/emu_oracle.c); alpha_h meets a float32 tensor -> float32 product.
+// (emulator.py:1105-1121). p, h in the state dtype S; the 3x3 stencil is a float32 conv2d whose summation order is the
+// reference's CPU backend's (see oracle/emu_oracle.c); alpha_h meets a float32 tensor -> float32 product. max|change|
+// goes through cs_max as a double (a float32 magnitude widens exactly).
 // Step k runs only if every earlier step changed some pixel by more than 1e-5 (the reference's while
 // condition); the maxima are exchanged through cs_max.
 // Ring form: step `step` of the frame is step `i` of its chunk; it reads ring buffer (cs_cur + i) % cs_ring and writes
@@ -543,6 +562,7 @@ __global__ void __launch_bounds__(kThreads) emu_lp_kernel(EmuDev d, FrameParams 
 // over the rank's own rows only and reduced over the ranks after the chunk, so the steps of a chunk run without
 // knowing whether an earlier step of the same chunk ended the iteration -- the ring (K + 1 buffers) keeps every
 // step's result and emu_csdvs_advance_kernel picks the right one.
+template <typename S>
 __global__ void __launch_bounds__(kThreads)
 emu_csdvs_step_kernel(EmuDev d, double alpha_p, float alpha_h, int step, int i, int sharded) {
     if (*(volatile int32_t *)d.abort_flag) return;
@@ -550,23 +570,23 @@ emu_csdvs_step_kernel(EmuDev d, double alpha_p, float alpha_h, int step, int i, 
     else if (step > 0 && __longlong_as_double((long long)d.cs_max[step - 1]) <= 1e-5) return;
     const int cur = (*(volatile int32_t *)d.cs_cur + i) % d.cs_ring;
     const int nxt = (cur + 1) % d.cs_ring;
-    const double *h = d.cs_bufs ? d.cs_bufs + (size_t)cur * d.cs_stride : (cur ? d.surround2 : d.surround);
-    double *hn = d.cs_bufs ? d.cs_bufs + (size_t)nxt * d.cs_stride : (nxt ? d.surround2 : d.surround);
-    const double *pp = (const double *)d.lp;
+    const S *h = cs_buf<S>(d, cur);
+    S *hn = cs_buf<S>(d, nxt);
+    const S *pp = (const S *)d.lp;
     const int idx = blockIdx.x * kThreads + threadIdx.x;
     double a = 0.0;
     if (idx < d.n) {
         const int y = idx / d.W, x = idx - y * d.W;
         const int ym = y > 0 ? y - 1 : 0, yp = y < d.H - 1 ? y + 1 : d.H - 1;
         const int xm = x > 0 ? x - 1 : 0, xp = x < d.W - 1 ? x + 1 : d.W - 1;
-        const double hc = h[idx];
+        const S hc = h[idx];
         const float uu = (float)h[ym * d.W + x], ll = (float)h[y * d.W + xm], cc = -4.0f * (float)hc;
         const float rr = (float)h[y * d.W + xp], dd = (float)h[yp * d.W + x];
         const float acc = idx >= d.cs_seq_from ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
         const float h_term = alpha_h * acc;
-        const double chg = alpha_p * (pp[idx] - hc) + (double)h_term;
+        const S chg = cs_change(alpha_p, pp[idx], hc, h_term);
         hn[idx] = hc + chg;
-        if (y >= d.cs_y_lo && y < d.cs_y_hi) a = fabs(chg);
+        if (y >= d.cs_y_lo && y < d.cs_y_hi) a = fabs((double)chg);
     }
     // block max of |change| -> one atomicMax (non-negative doubles order like their bit patterns)
     unsigned long long bits = (unsigned long long)__double_as_longlong(a);
@@ -591,6 +611,7 @@ emu_csdvs_step_kernel(EmuDev d, double alpha_p, float alpha_h, int step, int i, 
 // Sharded: a chunk of K steps between two halo exchanges, no early exit inside (the maxima are reduced over the ranks
 // after the chunk; emu_csdvs_advance_kernel picks the step).
 constexpr int kCsThreads = 512;
+template <typename S>
 __global__ void __launch_bounds__(kCsThreads)
 emu_csdvs_iter_kernel(EmuDev d, double alpha_p, float alpha_h, int s0, int s1, int sharded, int slot) {
     namespace cg = cooperative_groups;
@@ -600,26 +621,26 @@ emu_csdvs_iter_kernel(EmuDev d, double alpha_p, float alpha_h, int s0, int s1, i
     if (*(volatile int32_t *)d.abort_flag) return;
     if (sharded && *(volatile int32_t *)d.cs_done) return;
     const int cur0 = *(volatile int32_t *)d.cs_cur;
-    const double *pp = (const double *)d.lp;
+    const S *pp = (const S *)d.lp;
     const int stride = gridDim.x * kCsThreads;
     int taken = s1 - s0;
     for (int s = s0; s < s1; s++) {
         const int cur = (cur0 + (s - s0)) % d.cs_ring, nxt = (cur + 1) % d.cs_ring;
-        const double *h = d.cs_bufs ? d.cs_bufs + (size_t)cur * d.cs_stride : (cur ? d.surround2 : d.surround);
-        double *hn = d.cs_bufs ? d.cs_bufs + (size_t)nxt * d.cs_stride : (nxt ? d.surround2 : d.surround);
+        const S *h = cs_buf<S>(d, cur);
+        S *hn = cs_buf<S>(d, nxt);
         double a = 0.0;
         for (int idx = blockIdx.x * kCsThreads + threadIdx.x; idx < d.n; idx += stride) {
             const int y = idx / d.W, x = idx - y * d.W;
             const int ym = y > 0 ? y - 1 : 0, yp = y < d.H - 1 ? y + 1 : d.H - 1;
             const int xm = x > 0 ? x - 1 : 0, xp = x < d.W - 1 ? x + 1 : d.W - 1;
-            const double hc = h[idx];
+            const S hc = h[idx];
             const float uu = (float)h[ym * d.W + x], ll = (float)h[y * d.W + xm], cc = -4.0f * (float)hc;
             const float rr = (float)h[y * d.W + xp], dd = (float)h[yp * d.W + x];
             const float acc = idx >= d.cs_seq_from ? ((((uu + ll) + cc) + rr) + dd) : (uu + ll) + (cc + (rr + dd));
             const float h_term = alpha_h * acc;
-            const double chg = alpha_p * (pp[idx] - hc) + (double)h_term;
+            const S chg = cs_change(alpha_p, pp[idx], hc, h_term);
             hn[idx] = hc + chg;
-            if (y >= d.cs_y_lo && y < d.cs_y_hi) a = fmax(a, fabs(chg));
+            if (y >= d.cs_y_lo && y < d.cs_y_hi) a = fmax(a, fabs((double)chg));
         }
         unsigned long long bits = (unsigned long long)__double_as_longlong(a);
 #pragma unroll
@@ -658,8 +679,9 @@ __global__ void emu_csdvs_advance_kernel(EmuDev d, int s0, int s1, int slot) {
 }
 // sharded halo exchange: the K own rows next to each band edge of the current surround buffer -> send[2][K][W];
 // recv[2][K][W] (the neighbours' rows) -> the halo rows of the current buffer
-__global__ void emu_csdvs_pack_kernel(EmuDev d, double *send, int K) {
-    const double *h = d.cs_bufs + (size_t)(*d.cs_cur) * d.cs_stride;
+template <typename S>
+__global__ void emu_csdvs_pack_kernel(EmuDev d, S *send, int K) {
+    const S *h = (const S *)d.cs_bufs + (size_t)(*d.cs_cur) * d.cs_stride;
     const int per = K * d.W;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * per; i += gridDim.x * blockDim.x) {
         const int side = i / per, r = (i - side * per) / d.W, x = i % d.W;
@@ -669,8 +691,9 @@ __global__ void emu_csdvs_pack_kernel(EmuDev d, double *send, int K) {
 }
 // recv_above / recv_below: [K][W] rows of the neighbour above (its bottom edge) / below (its top edge); null at the
 // image border
-__global__ void emu_csdvs_unpack_kernel(EmuDev d, const double *recv_above, const double *recv_below, int K) {
-    double *h = d.cs_bufs + (size_t)(*d.cs_cur) * d.cs_stride;
+template <typename S>
+__global__ void emu_csdvs_unpack_kernel(EmuDev d, const S *recv_above, const S *recv_below, int K) {
+    S *h = (S *)d.cs_bufs + (size_t)(*d.cs_cur) * d.cs_stride;
     const int per = K * d.W;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * per; i += gridDim.x * blockDim.x) {
         const int side = i / per, r = (i - side * per) / d.W, x = i % d.W;
@@ -918,11 +941,8 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
     }
     FrameCtrl *c = d.ctrl + slot;
     uint32_t *hist = d.hist_pre + (size_t)slot * d.seg_stride;
-    const double *su_ptr = nullptr;
-    if (f_cs) {
-        const int cur = *(volatile int32_t *)d.cs_cur;
-        su_ptr = d.cs_bufs ? d.cs_bufs + (size_t)cur * d.cs_stride : (cur ? d.surround2 : d.surround);
-    }
+    const S *su_ptr = nullptr;
+    if (f_cs) su_ptr = cs_buf<S>(d, *(volatile int32_t *)d.cs_cur);
     const bool shot_here = f_shot && (RNG == 1 || shot_rand != nullptr);
     const uint32_t seg_base = (uint32_t)blockIdx.x * (uint32_t)d.seg_px;
     const int so = lane * kVec;                          // element offset inside the stage arrays
@@ -950,7 +970,7 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
         const uint32_t codes = codes_next;
         if (FT == V2E_U8 && j + 1 < nj) codes_next = load_codes(i0 + kWarps * kUnitPx);
         float lr[4], sr[4];
-        double su[4];
+        S su[4];
         if (t_on) {
             if (FT != V2E_U8) load_frame4<FT>(frame, i0, d.n, x);
             if (f_cs) ld4(su_ptr, i0, su);
@@ -1014,7 +1034,8 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
                 }
                 // difference and event counts (emulator.py:748-772, emulator_utils.py:137-173)
                 S diff;
-                if (sizeof(S) == 8 && f_cs) diff = (S)(((double)lp[k] - su[k]) - (double)base[k]);
+                // centre-surround: c_minus_s = photoreceptor - surround, diff = c_minus_s - base (emulator.py:751-752)
+                if (f_cs) diff = (lp[k] - su[k]) - base[k];
                 else diff = lp[k] - base[k];
                 S tp, tn;
                 if (sizeof(S) == 8 && !f_pp) { tp = (S)d.pos_nom; tn = (S)d.neg_nom; }
@@ -1927,7 +1948,7 @@ struct V2eEmu {
     int fused_skip, fused_penalty;                 // back-off: chunks to run frame by frame before the next attempt
     // pixel-sharded centre-surround model: plan of the current frame (v2e_emu_cs_begin) and the exchange buffers
     int cs_K;                   // halo rows = Euler steps per chunk (0: not sharded)
-    double *cs_send;            // [2][K][W]
+    void *cs_send;              // [2][K][W], state dtype
     int cs_num_steps;
     double cs_alpha_p; float cs_alpha_h;
     FrameParams cs_p;
@@ -2008,8 +2029,6 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
     if ((int64_t)cfg->width * cfg->height > (1ll << 30)) return fail(V2E_E_INVALID, "frame too large");
     if (cfg->iter_cap < 1 || cfg->iter_cap > kRecMaxCount) return fail(V2E_E_INVALID, "iter_cap out of range");
     if (cfg->max_frames_per_step < 1) return fail(V2E_E_INVALID, "max_frames_per_step < 1");
-    if (cfg->csdvs && !(cfg->cutoff_hz > 0 || cfg->hdr))
-        return fail(V2E_E_UNSUPPORTED, "csdvs needs a float64 photoreceptor state (cutoff_hz > 0)");
     if (cfg->csdvs && !(cfg->cs_tau_p_s > 0 && cfg->cs_tau_h_s > 0)) return fail(V2E_E_INVALID, "csdvs time constants must be positive");
     if (cfg->photoreceptor_noise && !(cfg->shot_noise_rate_hz > 0 && cfg->cutoff_hz > 0))   // emulator.py:196-204
         return fail(V2E_E_INVALID, "photoreceptor_noise needs shot_noise_rate_hz > 0 and cutoff_hz > 0");
@@ -2102,12 +2121,12 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
             h->cs_K = K;
             d.cs_ring = K + 1;
             d.cs_stride = np;
-            ALLOC(d.cs_bufs, (size_t)d.cs_ring * np * 8);
+            ALLOC(d.cs_bufs, (size_t)d.cs_ring * np * h->state_elem);
             ALLOC(d.cs_done, sizeof(int32_t));
-            ALLOC(h->cs_send, (size_t)2 * K * d.W * 8);
+            ALLOC(h->cs_send, (size_t)2 * K * d.W * h->state_elem);
         } else {
-            ALLOC(d.surround, np * 8);
-            ALLOC(d.surround2, np * 8);
+            ALLOC(d.surround, np * h->state_elem);
+            ALLOC(d.surround2, np * h->state_elem);
         }
     }
     ALLOC(h->lut_dev, 256 * 4);
@@ -2300,8 +2319,10 @@ struct ProfScope {
 
 static size_t frame_elem(int dt) { return dt == V2E_U8 ? 1 : (dt == V2E_F32 ? 4 : 8); }
 
-// One cooperative launch for Euler steps [s0, s1) (emu_csdvs_iter_kernel). Returns false when the device / occupancy
-// does not allow a cooperative grid (the per-step kernels are used then).
+// One cooperative launch for Euler steps [s0, s1) (emu_csdvs_iter_kernel<S>). Returns false when the device / occupancy
+// does not allow a cooperative grid (the per-step kernels are used then). The grid is sized from the occupancy of the
+// instantiation that runs: one query per state dtype.
+template <typename S>
 static bool cs_launch_iter(V2eEmu *h, double alpha_p, float alpha_h, int s0, int s1, int sharded, int slot, cudaStream_t st) {
     static int coop = -1, blocks_per_sm = 0, sms = 132;
     if (coop < 0) {
@@ -2309,7 +2330,7 @@ static bool cs_launch_iter(V2eEmu *h, double alpha_p, float alpha_h, int s0, int
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, emu_csdvs_iter_kernel, kCsThreads, 0) != cudaSuccess)
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, emu_csdvs_iter_kernel<S>, kCsThreads, 0) != cudaSuccess)
             blocks_per_sm = 0;
         const char *e = getenv("V2E_CS_COOP");
         if (e && atoi(e) == 0) coop = 0;
@@ -2321,11 +2342,47 @@ static bool cs_launch_iter(V2eEmu *h, double alpha_p, float alpha_h, int s0, int
     if (grid > need) grid = need;
     EmuDev dd = d;
     void *args[] = {(void *)&dd, (void *)&alpha_p, (void *)&alpha_h, (void *)&s0, (void *)&s1, (void *)&sharded, (void *)&slot};
-    if (cudaLaunchCooperativeKernel((const void *)emu_csdvs_iter_kernel, dim3(grid), dim3(kCsThreads), args, 0, st) == cudaSuccess)
+    if (cudaLaunchCooperativeKernel((const void *)emu_csdvs_iter_kernel<S>, dim3(grid), dim3(kCsThreads), args, 0, st) == cudaSuccess)
         return true;
     cudaGetLastError();         // clear; fall back to one launch per step from now on
     coop = 0;
     return false;
+}
+
+// Euler steps [s0, s1) of the current frame: one cooperative launch, else one kernel per step (single GPU: then
+// emu_csdvs_finish_kernel records the steps taken; sharded: emu_csdvs_advance_kernel does after the all-reduce)
+template <typename S>
+static void cs_run_steps(V2eEmu *h, double alpha_p, float alpha_h, int s0, int s1, int sharded, int slot, cudaStream_t st) {
+    if (cs_launch_iter<S>(h, alpha_p, alpha_h, s0, s1, sharded, slot, st)) {
+        h->n_cs_coop++;
+        return;
+    }
+    const EmuDev &d = h->d;
+    const int gs = (d.n + kThreads - 1) / kThreads;
+    for (int s = s0; s < s1; s++)
+        emu_csdvs_step_kernel<S><<<gs, kThreads, 0, st>>>(d, alpha_p, alpha_h, s, s - s0, sharded);
+    if (!sharded) emu_csdvs_finish_kernel<<<1, 1, 0, st>>>(d, s1, slot);
+    h->n_cs_step++;
+}
+static void cs_steps(V2eEmu *h, double alpha_p, float alpha_h, int s0, int s1, int sharded, int slot, cudaStream_t st) {
+    if (h->d.state_f64) cs_run_steps<double>(h, alpha_p, alpha_h, s0, s1, sharded, slot, st);
+    else cs_run_steps<float>(h, alpha_p, alpha_h, s0, s1, sharded, slot, st);
+}
+
+// photoreceptor low-pass of the centre-surround model, ahead of the Euler steps
+template <typename S>
+static int launch_lp_s(const EmuDev &d, const FrameParams &p, const void *frame, int dtype, cudaStream_t st) {
+    const int g = grid_for(d);
+    switch (dtype) {
+        case V2E_U8: emu_lp_kernel<S, V2E_U8><<<g, kThreads, 0, st>>>(d, p, frame); break;
+        case V2E_F32: emu_lp_kernel<S, V2E_F32><<<g, kThreads, 0, st>>>(d, p, frame); break;
+        case V2E_F64: emu_lp_kernel<S, V2E_F64><<<g, kThreads, 0, st>>>(d, p, frame); break;
+        default: return fail(V2E_E_INVALID, "bad frame dtype");
+    }
+    return V2E_OK;
+}
+static int launch_lp(const EmuDev &d, const FrameParams &p, const void *frame, int dtype, cudaStream_t st) {
+    return d.state_f64 ? launch_lp_s<double>(d, p, frame, dtype, st) : launch_lp_s<float>(d, p, frame, dtype, st);
 }
 
 // Euler-step plan of one frame of the centre-surround model (emulator.py:1068-1096)
@@ -2359,13 +2416,7 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
     int lp_done = 0;
     if (d.csdvs) {
         // emulator.py:686-708: low-pass for the whole field, then the surround's Euler steps
-        const int g = grid_for(d);
-        switch (dtype) {
-            case V2E_U8: emu_lp_kernel<V2E_U8><<<g, kThreads, 0, st>>>(d, p, frame); break;
-            case V2E_F32: emu_lp_kernel<V2E_F32><<<g, kThreads, 0, st>>>(d, p, frame); break;
-            case V2E_F64: emu_lp_kernel<V2E_F64><<<g, kThreads, 0, st>>>(d, p, frame); break;
-            default: return fail(V2E_E_INVALID, "bad frame dtype");
-        }
+        if ((rc = launch_lp(d, p, frame, dtype, st))) return rc;
         lp_done = 1;
     }
     if (d.scidvs || d.pr_noise) {
@@ -2389,15 +2440,7 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
         float alpha_h = 0;
         if ((rc = cs_plan(h, p, &num_steps, &alpha_p, &alpha_h))) return rc;
         CU(cudaMemsetAsync(d.cs_max, 0, (size_t)num_steps * sizeof(unsigned long long), st));
-        if (cs_launch_iter(h, alpha_p, alpha_h, 0, num_steps, 0, slot, st)) {
-            h->n_cs_coop++;
-        } else {
-            const int gs = (d.n + kThreads - 1) / kThreads;
-            for (int k = 0; k < num_steps; k++)
-                emu_csdvs_step_kernel<<<gs, kThreads, 0, st>>>(d, alpha_p, alpha_h, k, k, 0);
-            emu_csdvs_finish_kernel<<<1, 1, 0, st>>>(d, num_steps, slot);
-            h->n_cs_step++;
-        }
+        cs_steps(h, alpha_p, alpha_h, 0, num_steps, 0, slot, st);
     }
     {
         ProfScope ps(h, slot, 0, st);
@@ -3052,13 +3095,7 @@ extern "C" int v2e_emu_cs_begin(V2eEmu *h, const void *frame, int dtype, double 
     FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
     h->last_dt = p.dt;
     if ((rc = cs_plan(h, p, &h->cs_num_steps, &h->cs_alpha_p, &h->cs_alpha_h))) return rc;
-    const int g = grid_for(d);
-    switch (dtype) {
-        case V2E_U8: emu_lp_kernel<V2E_U8><<<g, kThreads, 0, st>>>(d, p, frame); break;
-        case V2E_F32: emu_lp_kernel<V2E_F32><<<g, kThreads, 0, st>>>(d, p, frame); break;
-        case V2E_F64: emu_lp_kernel<V2E_F64><<<g, kThreads, 0, st>>>(d, p, frame); break;
-        default: return fail(V2E_E_INVALID, "bad frame dtype");
-    }
+    if ((rc = launch_lp(d, p, frame, dtype, st))) return rc;
     CU(cudaMemsetAsync(d.cs_max, 0, (size_t)h->cs_num_steps * sizeof(unsigned long long), st));
     CU(cudaMemsetAsync(d.cs_done, 0, sizeof(int32_t), st));
     CU(cudaGetLastError());
@@ -3069,32 +3106,29 @@ extern "C" int v2e_emu_cs_begin(V2eEmu *h, const void *frame, int dtype, double 
     h->last_fused = 0;
     return V2E_OK;
 }
-extern "C" double *v2e_emu_cs_send_dev(V2eEmu *h) { return h ? h->cs_send : nullptr; }
+extern "C" void *v2e_emu_cs_send_dev(V2eEmu *h) { return h ? h->cs_send : nullptr; }
 extern "C" uint64_t *v2e_emu_cs_max_dev(V2eEmu *h) { return h ? (uint64_t *)h->d.cs_max : nullptr; }
 extern "C" int v2e_emu_cs_pack(V2eEmu *h, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
-    emu_csdvs_pack_kernel<<<132, 256, 0, (cudaStream_t)stream>>>(h->d, h->cs_send, h->cs_K);
+    if (h->d.state_f64) emu_csdvs_pack_kernel<double><<<132, 256, 0, (cudaStream_t)stream>>>(h->d, (double *)h->cs_send, h->cs_K);
+    else emu_csdvs_pack_kernel<float><<<132, 256, 0, (cudaStream_t)stream>>>(h->d, (float *)h->cs_send, h->cs_K);
     CU(cudaGetLastError());
     return V2E_OK;
 }
-extern "C" int v2e_emu_cs_unpack_from(V2eEmu *h, const double *rows_above_dev, const double *rows_below_dev, void *stream) {
+extern "C" int v2e_emu_cs_unpack_from(V2eEmu *h, const void *rows_above_dev, const void *rows_below_dev, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
-    emu_csdvs_unpack_kernel<<<132, 256, 0, (cudaStream_t)stream>>>(h->d, rows_above_dev, rows_below_dev, h->cs_K);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (h->d.state_f64)
+        emu_csdvs_unpack_kernel<double><<<132, 256, 0, st>>>(h->d, (const double *)rows_above_dev, (const double *)rows_below_dev, h->cs_K);
+    else
+        emu_csdvs_unpack_kernel<float><<<132, 256, 0, st>>>(h->d, (const float *)rows_above_dev, (const float *)rows_below_dev, h->cs_K);
     CU(cudaGetLastError());
     return V2E_OK;
 }
 extern "C" int v2e_emu_cs_chunk(V2eEmu *h, int s0, int s1, void *stream) {
     if (!h || !h->cs_pending) return fail(V2E_E_STATE, "v2e_emu_cs_begin must precede v2e_emu_cs_chunk");
     if (s0 < 0 || s1 <= s0 || s1 > h->cs_num_steps || s1 - s0 > h->cs_K) return fail(V2E_E_INVALID, "bad chunk of Euler steps");
-    const EmuDev &d = h->d;
-    if (cs_launch_iter(h, h->cs_alpha_p, h->cs_alpha_h, s0, s1, 1, 0, (cudaStream_t)stream)) {
-        h->n_cs_coop++;
-    } else {
-        const int gs = (d.n + kThreads - 1) / kThreads;
-        for (int s = s0; s < s1; s++)
-            emu_csdvs_step_kernel<<<gs, kThreads, 0, (cudaStream_t)stream>>>(d, h->cs_alpha_p, h->cs_alpha_h, s, s - s0, 1);
-        h->n_cs_step++;
-    }
+    cs_steps(h, h->cs_alpha_p, h->cs_alpha_h, s0, s1, 1, 0, (cudaStream_t)stream);
     CU(cudaGetLastError());
     return V2E_OK;
 }
@@ -3223,7 +3257,7 @@ extern "C" void *v2e_emu_state_ptr(V2eEmu *h, int which) {
             int32_t cur = 0;
             cudaDeviceSynchronize();
             cudaMemcpy(&cur, h->d.cs_cur, sizeof(cur), cudaMemcpyDeviceToHost);
-            if (h->d.cs_bufs) return h->d.cs_bufs + (size_t)cur * h->d.cs_stride;
+            if (h->d.cs_bufs) return (char *)h->d.cs_bufs + (size_t)cur * h->d.cs_stride * h->state_elem;
             return cur ? h->d.surround2 : h->d.surround;
         }
         case 7: return h->d.hp;

@@ -709,17 +709,18 @@ class EventEmulator(object):
         _lib.check(L.v2e_emu_cs_begin(h, fp, code, t_frame, tp, cap, 0, ctypes.byref(ns), st))
         ns = ns.value
         c = getattr(self, "_cs_cache", None)
-        if c is None:                # views of the library's exchange buffers, made once per handle
+        if c is None:                # views of the library's exchange buffers (state dtype), made once per handle
             nccl = dist.get_backend(group) == "nccl"
+            dtype, typestr = (torch.float64, "<f8") if self._state_f64 else (torch.float32, "<f4")
             c = self._cs_cache = dict(
                 nccl=nccl,
-                send=torch.as_tensor(_DevView(L.v2e_emu_cs_send_dev(h), (2, K, W), "<f8", self), device=self.device),
+                send=torch.as_tensor(_DevView(L.v2e_emu_cs_send_dev(h), (2, K, W), typestr, self), device=self.device),
                 mxv=torch.as_tensor(_DevView(L.v2e_emu_cs_max_dev(h), (8192,), "<i8", self), device=self.device),
-                gathered=torch.empty((world, 2, K, W), dtype=torch.float64, device=self.device))
+                gathered=torch.empty((world, 2, K, W), dtype=dtype, device=self.device))
         send, mxv, gathered = c["send"], c["mxv"], c["gathered"]
-        row_bytes = 2 * K * W * 8
+        row_bytes = 2 * K * W * gathered.element_size()
         # the upper neighbour's bottom edge / the lower neighbour's top edge, where the all-gather leaves them
-        above = ctypes.c_void_p(gathered.data_ptr() + (rank - 1) * row_bytes + K * W * 8) if rank > 0 else None
+        above = ctypes.c_void_p(gathered.data_ptr() + (rank - 1) * row_bytes + row_bytes // 2) if rank > 0 else None
         below = ctypes.c_void_p(gathered.data_ptr() + (rank + 1) * row_bytes) if rank < world - 1 else None
         for s0 in range(0, ns, K):
             s1 = min(ns, s0 + K)
@@ -960,7 +961,7 @@ class EventEmulator(object):
         ptr = self._lib.v2e_emu_state_ptr(self._h, which)
         if not ptr:
             return None
-        f64 = (which in (0, 1, 7) and self._state_f64) or which == 6
+        f64 = which in (0, 1, 6, 7) and self._state_f64      # lp, base, surround, high-pass: the state dtype
         view = _DevView(ptr, (self._H, self._W), "<f8" if f64 else "<f4", self)
         torch.cuda.current_stream(self.device).synchronize()
         # a copy: the library owns the memory and frees it at reset() / cleanup()
