@@ -420,13 +420,37 @@ int v2e_prep_run(V2ePrep *h, const uint8_t *src_dev, int n_images, uint8_t *dst_
 /* HDF5 "events" dataset rows (emulator.py:953-959): rows_dev [n][4] uint32 = [t * 1e6 (float32 product,
  * truncated), x, y, p with -1 -> 0]. */
 int v2e_events_to_h5_rows(const float *events_dev, uint64_t n, uint32_t *rows_dev, void *stream);
-/* AEDAT-2.0 body (v2ecore/output/aedat2_output.py:133-165): words_dev [2n] uint32 = per event the address
+/* AEDAT-2.0 body (v2ecore/output/aedat2_output.py:133-168): words_dev [2n] uint32 = per event the address
  * x << x_shift | y << y_shift | p01 << pol_shift (x, y flipped about size-1 when asked) and the int32 microsecond
  * timestamp, both big endian, ready for file.write(). The shifts / flips of the three supported cameras are in
- * aedat2_output.py:38-60. n_on_dev (nullable): += number of ON events (numOnEvents, :176). */
+ * aedat2_output.py:38-60. labels_dev (nullable): [n] uint8, 0 = shot noise; a noise row's address ORs in the
+ * special-event bit 1 << 10 (label_signal_noise, :154-158), even where that bit overlaps x (640x480).
+ * n_on_dev (nullable): += number of ON events (numOnEvents, :176). */
 int v2e_events_to_aedat2(const float *events_dev, uint64_t n, int size_x, int size_y, int x_shift, int y_shift,
-                         int pol_shift, int flip_x, int flip_y, uint32_t *words_dev, uint64_t *n_on_dev,
-                         void *stream);
+                         int pol_shift, int flip_x, int flip_y, const uint8_t *labels_dev, uint32_t *words_dev,
+                         uint64_t *n_on_dev, void *stream);
+/* DVS text body (RPG events.txt, v2ecore/output/ae_text_output.py:89-101), one line per row:
+ *   '{} {} {} {}\n'.format(float(t), int(x), int(y), int((p + 1) / 2))
+ * where float(t) is Python's repr() of the float32 timestamp widened to double (shortest round trip: "0.1000000015"
+ * style 17 digits, "4.8999998398358e-05" below 1e-4, "1e+16" from 1e16 up, "0.0", "inf", "nan"), x, y and p are cast
+ * to int32 by truncation and (p + 1) / 2 is evaluated in float32. labels_dev (nullable): [n] uint8; when given, each
+ * line ends ' {label}' before the newline (label_signal_noise: 1 = signal, 0 = shot noise). Lines are at most 64 bytes.
+ * Two calls:
+ *   v2e_events_to_text_layout: block_offsets_dev [v2e_events_to_text_scratch(n)] uint64 receives the byte offset of
+ *     every 256-row block and, in its last entry, the total length of the body. Read that entry (the only
+ *     synchronisation) to size text_dev.
+ *   v2e_events_to_text: writes the body, total bytes, to text_dev (no alignment needed).  */
+uint64_t v2e_events_to_text_scratch(uint64_t n);
+int v2e_events_to_text_layout(const float *events_dev, uint64_t n, const uint8_t *labels_dev,
+                              uint64_t *block_offsets_dev, void *stream);
+int v2e_events_to_text(const float *events_dev, uint64_t n, const uint8_t *labels_dev,
+                       const uint64_t *block_offsets_dev, uint8_t *text_dev, void *stream);
+/* Signal / shot-noise labels of a chunk of frames (emulator.py:889-923): frame f holds rows
+ * [offsets_dev[f], offsets_dev[f + 1]) and its last n_noise_dev[f] rows are shot noise (V2eFrameInfo n_shot_on +
+ * n_shot_off: every path emits them after the frame's signal rows). labels_dev [n_rows] uint8 = 1 for signal, 0 for
+ * noise; n_rows = offsets_dev[n_frames]. */
+int v2e_signnoise_labels(const int64_t *offsets_dev, const uint32_t *n_noise_dev, int n_frames, uint64_t n_rows,
+                         uint8_t *labels_dev, void *stream);
 
 /* ------------------------------------------------------------------------- */
 /* DVS frame rendering (SURVEY.md 8f rank 4): the histogram of EventRenderer.render_events_to_frames

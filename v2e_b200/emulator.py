@@ -17,11 +17,13 @@ Two RNG modes:
 Extra keywords (not in the reference): rng_mode, rng (draw source object), iter_cap,
 max_frames_per_step, exact_order, shard, fused.
 
-Sink keywords (dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text; emulator.py:325-357): file writers are out of
-scope here, so they are DELEGATED to the reference's own writer classes (v2ecore.output.*, h5py) when
-those import, exactly as the reference drives them (emulator.py:953-975); when they do not import the
-keyword is ignored with a warning. show_dvs_model_state / record_single_pixel_states (GUI / debug
-probes) are ignored with a warning.
+Sink keywords (dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text; emulator.py:325-357): the files are opened by the
+reference's own writer classes (v2ecore.output.*, h5py) when those import, and fed the way the reference feeds
+them (emulator.py:953-975); when they do not import the keyword is ignored with a warning. The DVS text body is
+formatted on the device (v2e_b200.sinks.events_to_text) and written to the writer's file. label_signal_noise
+labels every returned row signal (1) or shot noise (0) -- `last_signnoise_label`, generate_events_batch(...,
+return_labels=True) -- and passes the labels to the text and AEDAT-2.0 sinks; pixel-sharded emulators ignore it.
+show_dvs_model_state / record_single_pixel_states (GUI / debug probes) are ignored with a warning.
 """
 import ctypes
 import logging
@@ -75,9 +77,10 @@ class _Sinks:
     """The reference's event writers, driven the way emulator.py:325-357 / :953-975 / :401-421 drives them."""
 
     def __init__(self, output_folder, dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text, output_width, output_height,
-                 label_signal_noise):
+                 label_signal_noise, device):
         self.h5 = self.h5_dataset = self.aedat2 = self.aedat4 = self.text = None
         self.label_signal_noise = label_signal_noise
+        self.device = device
         folder = output_folder if output_folder is not None else "."
 
         def suffix(path, sfx):        # v2e_utils.checkAddSuffix
@@ -115,10 +118,12 @@ class _Sinks:
     def any(self):
         return any(x is not None for x in (self.h5, self.aedat2, self.aedat4, self.text))
 
-    def append(self, events):
-        """emulator.py:953-975 (rows are a host float32 [N,4] array)."""
+    def append(self, events, signnoise_label=None):
+        """emulator.py:953-975 (rows are a host float32 [N,4] array; signnoise_label a bool [N] array or None)."""
         if events is None or len(events) == 0:
             return
+        if not self.label_signal_noise:
+            signnoise_label = None
         if self.h5 is not None:
             tmp = np.array(events, dtype=np.float32)
             tmp[:, 0] = tmp[:, 0] * 1e6
@@ -127,11 +132,18 @@ class _Sinks:
             self.h5_dataset.resize(self.h5_dataset.shape[0] + tmp.shape[0], axis=0)
             self.h5_dataset[-tmp.shape[0]:] = tmp
         if self.aedat2 is not None:
-            self.aedat2.appendEvents(events, signnoise_label=None)
+            self.aedat2.appendEvents(events, signnoise_label=signnoise_label)
         if self.aedat4 is not None:
             self.aedat4.appendEvents(events, signnoise_label=None)
         if self.text is not None:
-            self.text.appendEvents(events)
+            # DVSTextOutput.appendEvents (ae_text_output.py:68-101) formats one line per Python call; the same lines
+            # come from the device, one copy and one write for the frame
+            if self.text.file is None:
+                raise Exception('output file closed already')
+            from . import sinks
+            ev = torch.from_numpy(np.ascontiguousarray(events, dtype=np.float32)).to(self.device)
+            lab = None if signnoise_label is None else torch.from_numpy(np.asarray(signnoise_label, np.uint8))
+            self.text.numEventsWritten += sinks.write_text(self.text.file, ev, lab)
 
     def close(self):
         for w in (self.h5, self.aedat2, self.aedat4, self.text):
@@ -252,6 +264,9 @@ class EventEmulator(object):
         self.output_width = output_width
         self.output_height = output_height
         self.label_signal_noise = label_signal_noise
+        if label_signal_noise and shard is not None:
+            logger.warning("label_signal_noise is ignored by a pixel-sharded emulator: its rows are not labelled")
+        self.last_signnoise_label = None     # label_signal_noise: labels of the rows generate_events last returned
         self.log_input = hdr
         self.scidvs = scidvs
         self.cs_lambda_pixels = cs_lambda_pixels
@@ -287,7 +302,7 @@ class EventEmulator(object):
         self._sinks = None
         if dvs_h5 or dvs_aedat2 or dvs_aedat4 or dvs_text:
             sk = _Sinks(output_folder, dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text, output_width, output_height,
-                        label_signal_noise)
+                        label_signal_noise, self.device)
             if sk.any():
                 self._sinks = sk
                 self.dvs_h5, self.dvs_aedat2, self.dvs_aedat4, self.dvs_text = sk.h5, sk.aedat2, sk.aedat4, sk.text
@@ -505,6 +520,7 @@ class EventEmulator(object):
         if self.shard is not None:
             ye0, ye1 = self.ext_band(fr.shape[0])
             return self._generate_band(fr[ye0:ye1], code, t_frame, fr.shape[0])
+        self.last_signnoise_label = None
         if not self._initialized:
             self._first_frame(fr, code, t_frame, fr.shape[0])
             return None
@@ -514,12 +530,20 @@ class EventEmulator(object):
         if self.rng_mode == "replay" and (per_frame_rng or self.exact_order):
             ev = self._phase_frame(fr, code, t_frame)
         else:
-            total, _ = self._run_step(fr.unsqueeze(0), code, [t_frame])
+            total, _, _ = self._run_step(fr.unsqueeze(0), code, [t_frame])
             ev = self._rows_to_host(total)
         self.t_previous = t_frame
         if ev is not None and len(ev) > 0:
+            label = None
+            if self.label_signal_noise:
+                # emulator.py:889-923: signal rows (leak included) first, labelled 1; the frame's shot-noise rows are
+                # its last n_shot_on + n_shot_off rows, labelled 0
+                fi = self.last_frame_info
+                label = np.ones(len(ev), dtype=bool)
+                label[len(ev) - (int(fi.n_shot_on) + int(fi.n_shot_off)):] = False
+                self.last_signnoise_label = label
             if self._sinks is not None:
-                self._sinks.append(ev)
+                self._sinks.append(ev, label)
             return ev
         return None
 
@@ -873,7 +897,7 @@ class EventEmulator(object):
     # batched path ------------------------------------------------------------------------------
     def _run_step(self, frames_dev, code, t_frames, base_row=0):
         """frames_dev: [T,H,W] device tensor, T <= max_frames_per_step. Appends this chunk's rows to the
-        device event buffer starting at base_row; returns (end_row, absolute offsets[T+1])."""
+        device event buffer starting at base_row; returns (end_row, absolute offsets[T+1], shot-noise rows [T])."""
         T = frames_dev.shape[0]
         L, h = self._lib, self._h
         n = self._H * self._W
@@ -907,18 +931,23 @@ class EventEmulator(object):
                 self._grow_event_buffer(max(2 * need, 2 * self._ev_dev.shape[0]), keep=base)
             total = int(rows.value)
             offsets = np.array([int(info[f].ev_base) for f in range(T)] + [total], np.int64)
+            n_shot = np.array([int(info[f].n_shot_on) + int(info[f].n_shot_off) for f in range(T)], np.int64)
             for f in range(T):
                 self._account(info[f])
             self.last_frame_info = info[T - 1]
-            return total, offsets
+            return total, offsets, n_shot
 
-    def generate_events_batch(self, frames, t_frames, return_device=False, copy=True):
+    def generate_events_batch(self, frames, t_frames, return_device=False, copy=True, return_labels=False):
         """Fast path (not in the reference): all frames of a clip in a few launches per frame and no
         per-frame host synchronisation. frames: [T,H,W]; t_frames: [T] seconds, non-decreasing.
         Returns (rows [N,4] float32, offsets [T+1]) -- rows of frame f are rows[offsets[f]:offsets[f+1]].
         With return_device=True rows is a view of the emulator's device buffer (valid until the next
         call); with copy=False the host rows are a view of the pinned staging buffer (same lifetime). The first frame of a fresh emulator only initialises state (zero rows), as in the
-        reference. Needs rng_mode="device" when leak or shot noise is on."""
+        reference. Needs rng_mode="device" when leak or shot noise is on.
+        return_labels=True (needs label_signal_noise=True) returns (rows, offsets, labels): labels [N], 1 for a signal
+        row and 0 for a shot-noise row, as a uint8 CUDA tensor with return_device, else a bool ndarray."""
+        if return_labels and not self.label_signal_noise:
+            raise ValueError("return_labels=True needs label_signal_noise=True")
         if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
                                           self.photoreceptor_noise):
             raise RuntimeError("generate_events_batch with per-frame noise needs rng_mode='device' "
@@ -931,27 +960,38 @@ class EventEmulator(object):
             raise ValueError("frames must be [T, height, width]")
         T = fr.shape[0]
         t_frames = self._frame_times(t_frames, T)
-        offs = [0]
+        offs, n_shot = [0], []
         start = 0
         if not self._initialized:
             self._first_frame(fr[0], code, t_frames[0], fr.shape[1])
             self.frame_counter += 1
             offs.append(0)
+            n_shot.append(0)
             start = 1
         f, row = start, 0
         while f < T:
             e = min(T, f + self.max_frames_per_step)
-            row, o = self._run_step(fr[f:e], code, t_frames[f:e], base_row=row)
+            row, o, s = self._run_step(fr[f:e], code, t_frames[f:e], base_row=row)
             offs.extend(o[1:].tolist())
+            n_shot.extend(s.tolist())
             self.t_previous = t_frames[e - 1]
             self.frame_counter += e - f
             f = e
         offs = np.asarray(offs, np.int64)
+        labels = None
+        if return_labels:
+            from .sinks import signnoise_labels
+            labels = signnoise_labels(offs, n_shot, self.device)
+            if not return_device:
+                labels = labels.cpu().numpy().astype(bool)
         if return_device:
             if self._ev_dev is None:
-                return torch.zeros((0, 4), dtype=torch.float32, device=self.device), offs
-            return self._ev_dev[:row], offs
-        return self._rows_to_host(row, copy=copy), offs
+                rows = torch.zeros((0, 4), dtype=torch.float32, device=self.device)
+            else:
+                rows = self._ev_dev[:row]
+        else:
+            rows = self._rows_to_host(row, copy=copy)
+        return (rows, offs, labels) if return_labels else (rows, offs)
 
     # state tensors by the reference's attribute names (emulator.py:756-764 reads them via getattr)
     def _state(self, name):
