@@ -186,12 +186,13 @@ constexpr int kRowTile = 128;
 // tap (r, s) is a descriptor offset: ring slot of input row y+r-ph, start + s pixels.
 //   warp 8     : TMA producer: the weights once per CTA, then one row (all slabs) per ring slot.
 //   warps 0..7 : two consumer warpgroups, taking turns over PAIRS of output rows of an item (warpgroup g:
-//                pairs g, g+2, ...). A row is 2 x (M=64) wgmma tiles over the 128 pixels, N = BN, accumulated
-//                in registers; then bias, LeakyReLU and the store. A ring slot is released by both
-//                warpgroups (every row of the item exactly once each) when neither needs it any more.
+//                pairs g, g+2, ...). Per 64-pixel half of the strip, the pair's wgmmas (M = 64, N = BN, both rows)
+//                are one asynchronous chain over the KH+1 input rows (strip_pair_mma); then bias, LeakyReLU and
+//                the store. A ring slot is released by both warpgroups (every row of the item exactly once each)
+//                when neither needs it any more.
 // POOL: F.avg_pool2d(out, 2) written beside the output (model.py:71: the pool that opens a down block). A pair
-// is rows (2k, 2k+1) of the item (items start on even rows), so the 2x2 window is in one warpgroup: the upper
-// row's fp16 activations stay in registers, the horizontal neighbour is the lane 4 apart.
+// is rows (2k, 2k+1) of the item (items start on even rows), so both rows of a 2x2 window are in the same
+// registers; the horizontal neighbour is the lane 4 apart.
 // ---------------------------------------------------------------------------------------------
 struct StripParams {
     int N, H, W;
@@ -206,7 +207,6 @@ struct StripParams {
                                    // (layers whose whole weight tensor does not fit in shared memory)
     int slab_bytes;                // bytes of one row buffer of one slab (1024-aligned)
     int w_bytes;                   // resident weights
-    int w_rows_per_load, w_loads;  // fused up-sampling kernel: weight rows per TMA load, loads
     int out_cstride, out_mode, co_real;
     float slope;
     const float *bias;
@@ -236,6 +236,49 @@ struct RowRing {
             if (lane == 0) mbar_arrive(&empty[slot(released)]);
     }
 };
+
+// One committed wgmma group: output rows (row0, row0+1) of a strip item over one 64-pixel half (a_off: its start in a
+// row buffer). Input row row0+r' (r' = 0..KH) feeds row0 with tap r' and row0+1 with tap r'-1, so the two rows' MMAs
+// interleave in one chain over the KH+1 input rows. An odd last row of an item has no input row row0+KH in the
+// ring: last = KH-1 reads row row0+KH-1 in its place, and the epilogue drops the row row0+1 this makes. Every output
+// element accumulates its terms in the order (r, slab, s, channel).
+// The accumulators are zeroed before the fence and never copied inside the chain: a register move that ptxas places
+// between two wgmmas (zeroing sunk past the fence, a path that skips a loop, accumulators merged from two code
+// paths, or one accumulator used by wgmmas of two widths) makes it wait for each wgmma before the next. Hence the
+// zeroing pinned by wgmma_fence_regs, the slab loop that runs at least once and is never unrolled (its remainder
+// would be a second path), and one code path for both row counts.
+template <int KW, int KC, int BN>
+__device__ __forceinline__ void strip_pair_mma(float (&acc)[2][BN / 2], const RowRing &rr, int row0, int last, int slabs,
+                                               uint64_t dr, uint64_t dw, uint32_t a_off, uint32_t row16, uint32_t slab16) {
+    constexpr int KH = KW, taps = KH * KW;
+    constexpr uint32_t rowb16 = (KC * 2u) >> 4, tile16 = (BN * KC * 2u) >> 4;
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; i++) acc[k][i] = 0.f;
+        wgmma_fence_regs(acc[k]);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int rp = 0; rp <= KH; rp++) {
+        const uint32_t a_row = rr.slot(row0 + (rp < KH ? rp : last)) * row16 + a_off;
+        int sl = 0;
+#pragma unroll 1
+        do {
+            const uint32_t a_lo = a_row + (uint32_t)sl * slab16;
+#pragma unroll
+            for (int s = 0; s < KW; s++) {
+#pragma unroll
+                for (int j = 0; j < KC / 16; j++) {
+                    const uint64_t ad = desc_add(dr, a_lo + (uint32_t)s * rowb16 + 2u * j);
+                    if (rp < KH) wgmma_f16<BN>(acc[0], ad, desc_add(dw, (uint32_t)(sl * taps + rp * KW + s) * tile16 + 2u * j), 1u);
+                    if (rp > 0) wgmma_f16<BN>(acc[1], ad, desc_add(dw, (uint32_t)(sl * taps + (rp - 1) * KW + s) * tile16 + 2u * j), 1u);
+                }
+            }
+        } while (++sl < slabs);
+    }
+    wgmma_commit();
+}
 
 template <int KW, int KC, int BN, bool POOL>
 __global__ void __launch_bounds__(kStripThreads, 1)
@@ -295,10 +338,13 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
     } else {
         // ===== consumer warpgroup g =====
-        const int g = warp >> 2;
-        constexpr uint32_t sbo = 8u * KC * 2u, rowb16 = (KC * 2u) >> 4, half16 = (64u * KC * 2u) >> 4;
-        constexpr uint32_t tile16 = tile_bytes >> 4;
-        constexpr int ksteps = KC / 16;
+        // g broadcast from lane 0: ptxas then sees warp-uniform control flow around the wgmma chains (a chain under
+        // a branch it takes for divergent is serialised, one wait per wgmma)
+        const int g = __shfl_sync(0xffffffffu, warp >> 2, 0);
+        constexpr uint32_t sbo = 8u * KC * 2u, half16 = (64u * KC * 2u) >> 4;
+        // the second 64-pixel half's chain runs during the first half's epilogue where both halves' accumulators
+        // (2 x BN registers) fit within the 168-register budget; BN = 64 runs the halves one after the other
+        constexpr bool kOverlap = BN <= 32;
         const uint64_t dw = make_smem_desc(smem_u32(smem), swizzle_layout(KC), sbo);
         const uint64_t dr = make_smem_desc(smem_u32(ring), swizzle_layout(KC), sbo);
         const uint32_t row16 = row_bytes >> 4, slab16 = (uint32_t)p.slab_bytes >> 4;
@@ -312,68 +358,64 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             rr.waited = 0; rr.released = 0;
             for (int q = g; 2 * q < rows_out; q += 2) {
                 rr.release_upto(2 * q, lane);                   // rows only the other warpgroup needed
-                const int nrows = min(2, rows_out - 2 * q);
-                __half2 prev[2][2][BN / 8];
-                for (int k = 0; k < nrows; k++) {
-                    const int yr = 2 * q + k;                   // output row (relative to the item)
-                    rr.wait_upto(yr + KH);
-                    float acc[2][BN / 2];
-                    uint32_t first = 0;
-                    wgmma_fence();
-                    for (int r = 0; r < KH; r++) {
-                        const uint32_t a_row = rr.slot(yr + r) * row16;
-                        for (int sl = 0; sl < slabs; sl++) {
-                            const uint32_t a_lo = a_row + (uint32_t)sl * slab16;
-                            const uint32_t b_lo = (uint32_t)(sl * taps + r * KW) * tile16;
+                const bool two = 2 * q + 1 < rows_out;          // an odd last row is the pair's upper row alone
+                rr.wait_upto(2 * q + KH + (two ? 1 : 0));
+                float acc[2][2][BN / 2];                        // [64-pixel half][output row 2q, 2q+1]
+                auto issue = [&](int hf) {
+                    strip_pair_mma<KW, KC, BN>(acc[hf], rr, 2 * q, two ? KH : KH - 1, slabs, dr, dw, hf * half16, row16, slab16);
+                };
+                const int y = ya + 2 * q;
+                auto epilogue = [&](int hf) {
 #pragma unroll
-                            for (int s = 0; s < KW; s++) {
+                    for (int i = 0; i < 2; i++) {
+                        const int m = 64 * hf + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+                        const int px = tx * kRowTile + m;
+                        const bool inb = px < p.W;
+                        const size_t pix = ((size_t)n * p.H + y) * p.W + px;
+                        __half2 h0[BN / 8], h1[BN / 8];
+                        epilogue_row<BN>(acc[hf][0], i, inb, pix, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
+                                         p.out_cstride, co_off, h0);
+                        if (two) {
+                            epilogue_row<BN>(acc[hf][1], i, inb, pix + p.W, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
+                                             p.out_cstride, co_off, h1);
+                            if (POOL) {
+                                // 2x2 average of the stored (fp16) activations; pixel m+1 is the lane 4 apart
+                                __half2 *pl = (__half2 *)((__half *)p.pool_out +
+                                    (((size_t)n * (p.H / 2) + y / 2) * (p.W / 2) + px / 2) * p.pool_cstride + co_off);
 #pragma unroll
-                                for (int j = 0; j < ksteps; j++) {
-                                    const uint64_t bd = desc_add(dw, b_lo + (uint32_t)s * tile16 + 2u * j);
-                                    wgmma_f16<BN>(acc[0], desc_add(dr, a_lo + (uint32_t)s * rowb16 + 2u * j), bd, first);
-                                    wgmma_f16<BN>(acc[1], desc_add(dr, a_lo + half16 + (uint32_t)s * rowb16 + 2u * j), bd, first);
-                                    first = 1;
+                                for (int j = 0; j < BN / 8; j++) {
+                                    const float2 a = __half22float2(h1[j]), b = __half22float2(h0[j]);
+                                    float s0 = a.x + b.x, s1 = a.y + b.y;       // exact: fp16 values in float32
+                                    s0 += __shfl_xor_sync(0xffffffffu, s0, 4);
+                                    s1 += __shfl_xor_sync(0xffffffffu, s1, 4);
+                                    if (inb && (lane & 4) == 0)
+                                        pl[(8 * j + 2 * (lane & 3)) / 2] = __floats2half2_rn(s0 * 0.25f, s1 * 0.25f);
                                 }
                             }
                         }
                     }
-                    wgmma_commit();
+                };
+                if constexpr (kOverlap) {
+                    issue(0);
+                    issue(1);
+                    wgmma_wait<1>();
+                    wgmma_fence_regs(acc[0][0]);
+                    wgmma_fence_regs(acc[0][1]);
+                    epilogue(0);
                     wgmma_wait<0>();
-                    wgmma_fence_regs(acc[0]);
-                    wgmma_fence_regs(acc[1]);
-                    if (k == nrows - 1) rr.release_upto(min(rows_in, 2 * q + 4), lane);   // next pair starts at 2q+4
-                    const int y = ya + yr;
+                    wgmma_fence_regs(acc[1][0]);
+                    wgmma_fence_regs(acc[1][1]);
+                    rr.release_upto(min(rows_in, 2 * q + 4), lane);    // next pair starts at 2q+4
+                    epilogue(1);
+                } else {
 #pragma unroll
                     for (int hf = 0; hf < 2; hf++) {
-#pragma unroll
-                        for (int i = 0; i < 2; i++) {
-                            const int m = 64 * hf + 16 * (warp & 3) + (lane >> 2) + 8 * i;
-                            const int px = tx * kRowTile + m;
-                            const bool inb = px < p.W;
-                            const size_t pix = ((size_t)n * p.H + y) * p.W + px;
-                            __half2 hv[BN / 8];
-                            epilogue_row<BN>(acc[hf], i, inb, pix, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
-                                             p.out_cstride, co_off, hv);
-                            if (POOL) {
-                                if (k == 0) {
-#pragma unroll
-                                    for (int j = 0; j < BN / 8; j++) prev[hf][i][j] = hv[j];
-                                } else {
-                                    // 2x2 average of the stored (fp16) activations; pixel m+1 is the lane 4 apart
-                                    __half2 *pl = (__half2 *)((__half *)p.pool_out +
-                                        (((size_t)n * (p.H / 2) + y / 2) * (p.W / 2) + px / 2) * p.pool_cstride + co_off);
-#pragma unroll
-                                    for (int j = 0; j < BN / 8; j++) {
-                                        const float2 a = __half22float2(hv[j]), b = __half22float2(prev[hf][i][j]);
-                                        float s0 = a.x + b.x, s1 = a.y + b.y;       // exact: fp16 values in float32
-                                        s0 += __shfl_xor_sync(0xffffffffu, s0, 4);
-                                        s1 += __shfl_xor_sync(0xffffffffu, s1, 4);
-                                        if (inb && (lane & 4) == 0)
-                                            pl[(8 * j + 2 * (lane & 3)) / 2] = __floats2half2_rn(s0 * 0.25f, s1 * 0.25f);
-                                    }
-                                }
-                            }
-                        }
+                        issue(hf);
+                        wgmma_wait<0>();
+                        wgmma_fence_regs(acc[hf][0]);
+                        wgmma_fence_regs(acc[hf][1]);
+                        if (hf == 1) rr.release_upto(min(rows_in, 2 * q + 4), lane);
+                        epilogue(hf);
                     }
                 }
             }
@@ -394,10 +436,12 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // built in float32 on the host). Same MACs as the convolution over the up-sampled tensor, a quarter of the
 // input bytes, no upsample kernel. The kernel walks a strip of 128 low-resolution columns like the strip kernel:
 // a consumer warpgroup takes a pair of output rows (2m, 2m+1), both read low rows m-1..m+1, and each row is
-// two horizontal phases x two 64-pixel halves of wgmma tiles (N = Cout_pad = 32); phase px is written to
-// pixels 2j+px. Only the 2-pixel frame of the image differs (bilinear clamping and the conv's zero padding
-// are not shift-invariant there); a small direct kernel rewrites it afterwards.
-// Folded weight tiles: [slab][px][b][q][Cout_pad][64], q = py + 2*(1-a).
+// one asynchronous wgmma chain per 64-pixel half whose N = 128 columns are the four phases (px, py) x 32 output
+// channels (they read the same low-resolution window); phase px is written to pixels 2j+px. Only the 2-pixel
+// frame of the image differs (bilinear clamping and the conv's zero padding are not shift-invariant there); a
+// small direct kernel rewrites it afterwards.
+// Folded weight tiles in global memory: [slab][px][b][q][Cout_pad][64], q = py + 2*(1-a); in shared memory:
+// [slab][b][a][px][py][Cout_pad][64].
 // ---------------------------------------------------------------------------------------------
 constexpr int kUpBlocks = 6;
 
@@ -427,8 +471,13 @@ conv_up2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         // ===== TMA producer: folded weights (already in tile order), then low-resolution rows =====
         if (lane == 0) {
             mbar_expect_tx(&w_bar, (uint32_t)p.w_bytes);
-            for (int l = 0; l < p.w_loads; l++)
-                tma_load_2d(smem + (size_t)l * p.w_rows_per_load * KC * 2, &tmB, &w_bar, 0, l * p.w_rows_per_load);
+            // blocks [slab][b][t][px] of the tiles py = 0, 1 (adjacent in the host layout: q = py + 2*(2-t)), so
+            // that the four phases of a window (slab, b, t) are 4*BN consecutive rows: one N = 128 B descriptor
+            for (int l = 0; l < slabs * 3 * 3 * 2; l++) {
+                const int sl = l / 18, b = (l / 6) % 3, t = (l / 2) % 3, px = l % 2;
+                tma_load_2d(smem + (size_t)l * 2 * BN * KC * 2, &tmB, &w_bar, 0,
+                            (((sl * 2 + px) * KW + b) * kUpBlocks + 2 * (2 - t)) * BN);
+            }
             uint32_t cnt = 0;
             for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
                 const int tx = item % p.tiles_x, rest = item / p.tiles_x;
@@ -447,9 +496,9 @@ conv_up2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
     } else {
         // ===== consumer warpgroup g: output row pairs g, g+2, ... of an item =====
-        const int g = warp >> 2;
+        const int g = __shfl_sync(0xffffffffu, warp >> 2, 0);     // warp-uniform to ptxas (see strip_pair_mma)
         constexpr uint32_t sbo = 8u * KC * 2u, rowb16 = (KC * 2u) >> 4, half16 = (64u * KC * 2u) >> 4;
-        constexpr uint32_t tile16 = (BN * KC * 2u) >> 4;
+        constexpr uint32_t blk16 = (2u * BN * KC * 2u) >> 4;      // one weight block (slab, b, t, px)
         const uint64_t dw = make_smem_desc(smem_u32(smem), swizzle_layout(KC), sbo);
         const uint64_t dr = make_smem_desc(smem_u32(ring), swizzle_layout(KC), sbo);
         const uint32_t row16 = row_bytes >> 4, slab16 = (uint32_t)p.slab_bytes >> 4;
@@ -464,50 +513,49 @@ conv_up2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             for (int q = g; q < pairs; q += 2) {
                 rr.release_upto(q, lane);
                 rr.wait_upto(q + 3);                            // low rows ka-1+q .. ka+1+q
-                for (int py = 0; py < 2; py++) {
-                    float acc[2][2][BN / 2];                    // [px][64-pixel half]
-                    uint32_t first = 0;
+#pragma unroll
+                for (int hf = 0; hf < 2; hf++) {
+                    // one 64-pixel half, all four phases: columns [(2 px + py) * BN, +BN) are phase (px, py); every
+                    // output element accumulates its terms in the order (t, slab, b, channel). Zeroed and chained
+                    // as in strip_pair_mma, so that the wgmmas issue back to back.
+                    float acc[4 * BN / 2];
+#pragma unroll
+                    for (int i = 0; i < 4 * BN / 2; i++) acc[i] = 0.f;
+                    wgmma_fence_regs(acc);
                     wgmma_fence();
+#pragma unroll
                     for (int t = 0; t < 3; t++) {
-                        const int qb = py + 2 * (2 - t);
-                        const uint32_t a_row = rr.slot(q + t) * row16;
-                        for (int sl = 0; sl < slabs; sl++) {
+                        const uint32_t a_row = rr.slot(q + t) * row16 + (uint32_t)hf * half16;
+                        int sl = 0;
+#pragma unroll 1
+                        do {
                             const uint32_t a_lo = a_row + (uint32_t)sl * slab16;
 #pragma unroll
                             for (int b = 0; b < KW; b++) {
 #pragma unroll
-                                for (int j = 0; j < KC / 16; j++) {
-                                    const uint64_t a0 = desc_add(dr, a_lo + (uint32_t)b * rowb16 + 2u * j);
-                                    const uint64_t a1 = desc_add(dr, a_lo + half16 + (uint32_t)b * rowb16 + 2u * j);
-#pragma unroll
-                                    for (int px = 0; px < 2; px++) {
-                                        const uint64_t bd = desc_add(dw, (uint32_t)((((sl * 2 + px) * KW + b) * kUpBlocks + qb)) * tile16 + 2u * j);
-                                        wgmma_f16<BN>(acc[px][0], a0, bd, first);
-                                        wgmma_f16<BN>(acc[px][1], a1, bd, first);
-                                    }
-                                    first = 1;
-                                }
+                                for (int j = 0; j < KC / 16; j++)
+                                    wgmma_f16<4 * BN>(acc, desc_add(dr, a_lo + (uint32_t)b * rowb16 + 2u * j),
+                                                      desc_add(dw, (uint32_t)(((sl * KW + b) * 3 + t) * 2) * blk16 + 2u * j), 1u);
                             }
-                        }
+                        } while (++sl < slabs);
                     }
                     wgmma_commit();
                     wgmma_wait<0>();
+                    wgmma_fence_regs(acc);
+                    if (hf == 1) rr.release_upto(min(rows_in, q + 2), lane);        // next pair starts at q+2
 #pragma unroll
-                    for (int px = 0; px < 2; px++) { wgmma_fence_regs(acc[px][0]); wgmma_fence_regs(acc[px][1]); }
-                    if (py == 1) rr.release_upto(min(rows_in, q + 2), lane);        // next pair starts at q+2
-                    const int y = 2 * (ka + q) + py;
+                    for (int ph = 0; ph < 4; ph++) {
+                        const int px = ph >> 1, py = ph & 1;
+                        const float (&d)[BN / 2] = *reinterpret_cast<const float (*)[BN / 2]>(&acc[ph * BN / 2]);
+                        const int y = 2 * (ka + q) + py;
 #pragma unroll
-                    for (int px = 0; px < 2; px++)
-#pragma unroll
-                        for (int hf = 0; hf < 2; hf++)
-#pragma unroll
-                            for (int i = 0; i < 2; i++) {
-                                const int jl = tx * kRowTile + 64 * hf + 16 * (warp & 3) + (lane >> 2) + 8 * i;
-                                const size_t pix = ((size_t)n * p.H + y) * p.W + (size_t)(2 * jl + px);
-                                __half2 hv[BN / 8];
-                                epilogue_row<BN>(acc[px][hf], i, jl < wl, pix, lane, p.bias, p.slope, 0, p.out,
-                                                 p.out_cstride, 0, hv);
-                            }
+                        for (int i = 0; i < 2; i++) {
+                            const int jl = tx * kRowTile + 64 * hf + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+                            const size_t pix = ((size_t)n * p.H + y) * p.W + (size_t)(2 * jl + px);
+                            __half2 hv[BN / 8];
+                            epilogue_row<BN>(d, i, jl < wl, pix, lane, p.bias, p.slope, 0, p.out, p.out_cstride, 0, hv);
+                        }
+                    }
                 }
             }
             rr.release_upto(rows_in, lane);
@@ -1017,8 +1065,6 @@ int v2e_conv_up2_prepare(V2eUpLaunch *L, const void *x_low, int C, const void *w
     p.slab_bytes = (int)(((size_t)(kRowTile + 2) * KC * 2 + 1023) & ~(size_t)1023);
     p.w_bytes = slabs * 2 * 3 * kUpBlocks * Cout_pad * KC * 2;
     const int rows_total = slabs * 2 * 3 * kUpBlocks * Cout_pad;
-    p.w_rows_per_load = kUpBlocks * Cout_pad;                  // 192 rows: one (slab, px, b) stack per load
-    p.w_loads = rows_total / p.w_rows_per_load;
     int ns = (int)((kSmemFull - (size_t)p.w_bytes - 2048) / ((size_t)p.slab_bytes * slabs));
     if (ns > kMaxSlot) ns = kMaxSlot;
     if (ns < 3) return v2e_set_error(V2E_E_INVALID, "fused up-sampling convolution: weights leave no room for the input ring%s", "");
@@ -1031,7 +1077,7 @@ int v2e_conv_up2_prepare(V2eUpLaunch *L, const void *x_low, int C, const void *w
         EncodeTiledFn fn = encode_fn();
         cuuint64_t dims[2] = {(cuuint64_t)KC, (cuuint64_t)rows_total};
         cuuint64_t strides[1] = {(cuuint64_t)KC * 2};
-        cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)p.w_rows_per_load};
+        cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)(2 * Cout_pad)};     // the tiles py = 0, 1 of one (slab, px, b, a)
         cuuint32_t es[2] = {1, 1};
         CUresult r = fn(&L->tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)wgt_fold, dims, strides, box, es,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
