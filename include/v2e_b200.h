@@ -294,6 +294,25 @@ int v2e_conv2d_lrelu_sm100(const void *x1_dev, int C1, const void *x2_dev, int C
                            int N, int H, int W, void *out_dev, int out_cstride, int out_mode,
                            int co_real, float slope, void *stream);
 
+/* Per-tap tiles of v2e_conv2d_lrelu_sm100 (output pixels x output channels per CTA). AUTO: the tile
+ * v2e_conv_pick_tile chooses for the layer on the current device, what v2e_conv2d_lrelu_sm100 and the SloMo
+ * networks run (the multicast argument is then ignored). LEGACY: 128 x min(Cout_pad, 128). The wide tiles need
+ * 64-channel slabs (C1, C2 multiples of 64), fp16 output (out_mode 0) and Cout_pad a multiple of their width; with
+ * multicast != 0 their CTAs run in pairs (clusters of 2) that share one weight slab per stage. Every tile gives the
+ * same output bit for bit. */
+enum {
+    V2E_CONV_TILE_AUTO = -1,
+    V2E_CONV_TILE_LEGACY = 0,
+    V2E_CONV_TILE_256x128 = 1,        /* 16x16 pixels x 128 channels */
+    V2E_CONV_TILE_128x256 = 2         /* 8x16 pixels x 256 channels */
+};
+int v2e_conv2d_lrelu_sm100_tile(const void *x1_dev, int C1, const void *x2_dev, int C2,
+                                const void *wgt_dev, const float *bias_dev, int Cout_pad, int KH, int KW,
+                                int N, int H, int W, void *out_dev, int out_cstride, int out_mode,
+                                int co_real, float slope, int tile, int multicast, void *stream);
+/* The tile AUTO picks for a layer on a device with n_sms SMs (wave-aware cost; no GPU needed). */
+int v2e_conv_pick_tile(int C1, int C2, int Cout_pad, int KH, int KW, int N, int H, int W, int n_sms);
+
 /* Same operation through the strip kernel (full-resolution layers: W >= 128, Cout_pad <= 128, the
  * whole weight tensor resident in shared memory): a CTA walks down a 128-pixel-wide column strip with a
  * ring of input rows in shared memory; one new input row per output row, filter taps are descriptor

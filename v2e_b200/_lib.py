@@ -87,6 +87,9 @@ _SIGS = {
     "v2e_emu_phase_emit": (_i, [_vp, _d, _d, _vp, _u64, _vp]),
     "v2e_conv2d_lrelu_sm100": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
                                     ctypes.c_float, _vp]),
+    "v2e_conv2d_lrelu_sm100_tile": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
+                                         ctypes.c_float, _i, _i, _vp]),
+    "v2e_conv_pick_tile": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _i]),
     "v2e_conv2d_lrelu_sm100_strip": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
                                           ctypes.c_float, _vp]),
     "v2e_conv_strip_pick_kc": (_i, [_i, _i, _i, _i, _i, _i]),

@@ -22,6 +22,7 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -49,6 +50,7 @@ struct ConvParams {
     int stages;                 // depth of the producer / consumer ring (<= kStages)
     int co_fast;                // grid order: 1 = output-channel blocks in gridDim.x
     int tiles_x, tiles_y;
+    int n_tiles;                // pixel tiles (conv_wide_kernel: the grid may hold one padding CTA more)
     int out_cstride;            // channel stride (elements) of the fp16 NHWC output
     int out_mode;               // 0: fp16 NHWC; 1: fp32 [N,H,W,8], first co_real channels
     int co_real;
@@ -172,6 +174,156 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             epilogue_row<BN>(acc, i, inb, pix, lane, p.bias + n0, p.slope, p.out_mode, p.out, p.out_cstride, n0, hv);
         }
     }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Wide per-tap kernel: conv_tc_kernel's producer / two-consumer structure with 128 fp32 accumulators per consumer
+// thread, so that every (tap, slab) stage feeds twice the MMAs of the 128 x 128 tile. The tile is
+//   MH = 1: 128 pixels (8x16) x BN = 256 channels; a warpgroup runs one m64n256 chain over its 64 pixels,
+//   MH = 2: 256 pixels (16x16) x BN = 128 channels; a warpgroup runs two m64n128 chains (its two 64-pixel quarters)
+//           over the same B slab.
+// MC: the CTAs of a cluster pair share the output-channel block and take neighbouring pixel tiles; each producer
+// loads half of the weight slab and multicasts it to both CTAs, so a stage costs A + B/2 bytes from L2 per CTA.
+// A stage is refilled only when the consumers of BOTH CTAs have released it (each consumer warp arrives on its own
+// and on the peer's empty barrier, 16 arrivals), and both CTAs pass a cluster barrier before they exit (the peer's
+// multicasts and remote arrivals target this CTA's shared memory). A grid with an odd pixel-tile count gets one
+// padding CTA, which loads the last tile's window and multicasts its half of the weights but stores nothing.
+// Every output element accumulates its terms in the order (tap, slab, k16) of conv_tc_kernel.
+// ---------------------------------------------------------------------------------------------
+template <int MH, int BN, bool MC>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
+                 const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
+    constexpr int TH = kTileH * MH, BM = kBM * MH;
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t *smem = align1024(smem_raw);
+    const uint32_t a_bytes = BM * p.KC * 2;
+    const uint32_t b_bytes = BN * p.KC * 2;           // a multiple of 1024 (BN >= 128, KC >= 16)
+    const uint32_t stage_bytes = a_bytes + b_bytes;
+    __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages];
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tile_g = p.co_fast ? blockIdx.y : blockIdx.x;
+    const bool live = tile_g < p.n_tiles;             // false: the padding CTA of an odd tile count
+    const int tile = live ? tile_g : p.n_tiles - 1;
+    const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, n = tile / (p.tiles_x * p.tiles_y);
+    const int x0 = tx * kTileW, y0 = ty * TH;
+    const int n0 = (p.co_fast ? blockIdx.x : blockIdx.y) * BN;
+    const int Ctot = p.C1 + p.C2;
+    const int slabs = Ctot / p.KC;
+    const int k_iters = p.KH * p.KW * slabs;
+    const uint32_t crank = MC ? cluster_ctarank() : 0u;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kStages; s++) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], (MC ? 2 : 1) * kConsumerWarps);
+        }
+        fence_barrier_init();
+    }
+    if (warp == kProducerWarp && lane == 0) {
+        prefetch_tmap(&tmA);
+        if (p.C2) prefetch_tmap(&tmA2);
+        prefetch_tmap(&tmB);
+    }
+    // the peer multicasts into this CTA's stages and arrives on its barriers: both CTAs' barriers are initialised first
+    if constexpr (MC) cluster_sync();
+    else __syncthreads();
+
+    if (warp == kProducerWarp) {
+        // ===== TMA producer =====
+        if (lane == 0) {
+            int stage = 0;
+            uint32_t phase = 0;
+            const int ph = p.KH / 2, pw = p.KW / 2;
+            for (int tap = 0; tap < p.KH * p.KW; tap++) {
+                const int r = tap / p.KW, s = tap % p.KW;
+                for (int sl = 0; sl < slabs; sl++) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    uint8_t *sa = smem + stage * stage_bytes, *sb = sa + a_bytes;
+                    mbar_expect_tx(&full_bar[stage], a_bytes + b_bytes);
+                    const int c = sl * p.KC;
+                    if (c < p.C1) tma_load_4d(sa, &tmA, &full_bar[stage], c, x0 + s - pw, y0 + r - ph, n);
+                    else tma_load_4d(sa, &tmA2, &full_bar[stage], c - p.C1, x0 + s - pw, y0 + r - ph, n);
+                    if constexpr (MC)
+                        tma_load_2d_multicast(sb + crank * (b_bytes / 2), &tmB, &full_bar[stage], tap * Ctot + c,
+                                              n0 + (int)crank * (BN / 2), (uint16_t)0x3);
+                    else
+                        tma_load_2d(sb, &tmB, &full_bar[stage], tap * Ctot + c, n0);
+                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+    } else {
+        // ===== consumer warpgroup g: pixels BM/2 * g .. BM/2 * (g+1) - 1 of the tile, MH 64-pixel quarters =====
+        const int g = __shfl_sync(0xffffffffu, warp >> 2, 0);       // warp-uniform to ptxas (see strip_pair_mma)
+        const uint64_t d0 = make_smem_desc(smem_u32(smem), swizzle_layout(p.KC), 8u * p.KC * 2u);
+        const uint32_t stage16 = stage_bytes >> 4, a16 = a_bytes >> 4, q16 = (64u * p.KC * 2u) >> 4;
+        const int ksteps = p.KC / 16;
+        float acc[MH][BN / 2];
+#pragma unroll
+        for (int h = 0; h < MH; h++) {
+#pragma unroll
+            for (int i = 0; i < BN / 2; i++) acc[h][i] = 0.f;
+            wgmma_fence_regs(acc[h]);
+        }
+        int stage = 0, prev = -1;
+        uint32_t phase = 0;
+        for (int it = 0; it < k_iters; it++) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t base = (uint32_t)stage * stage16;
+            wgmma_fence();
+            for (int j = 0; j < ksteps; j++) {
+#pragma unroll
+                for (int h = 0; h < MH; h++)
+                    wgmma_f16<BN>(acc[h], desc_add(d0, base + (uint32_t)(g * MH + h) * q16 + 2u * j),
+                                  desc_add(d0, base + a16 + 2u * j), (uint32_t)((it | j) != 0));
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                 // the stage before this one has been read: hand it back
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) {
+                    mbar_arrive(&empty_bar[prev]);
+                    if constexpr (MC) mbar_arrive_cluster(&empty_bar[prev], crank ^ 1u);
+                }
+            }
+            prev = stage;
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int h = 0; h < MH; h++) wgmma_fence_regs(acc[h]);
+        if (live) {
+            // bias + LeakyReLU + fp16 store of both rows of each 8-column group at once (one bias load per group
+            // keeps the 128 accumulators and the addresses within the register budget)
+            const float *bias = p.bias + n0;
+            __half *out = (__half *)p.out + n0;
+#pragma unroll
+            for (int h = 0; h < MH; h++) {
+                size_t pix[2];
+                bool inb[2];
+#pragma unroll
+                for (int i = 0; i < 2; i++) {
+                    const int m = 64 * (g * MH + h) + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+                    const int py = y0 + m / kTileW, px = x0 + m % kTileW;
+                    inb[i] = py < p.H && px < p.W;
+                    pix[i] = (((size_t)n * p.H + py) * p.W + px) * p.out_cstride;
+                }
+#pragma unroll
+                for (int j = 0; j < BN / 8; j++) {
+                    const int c = 8 * j + 2 * (lane & 3);
+                    const float2 b = __ldg((const float2 *)(bias + c));
+#pragma unroll
+                    for (int i = 0; i < 2; i++)
+                        if (inb[i])
+                            *(__half2 *)(out + pix[i] + c) = __floats2half2_rn(lrelu(acc[h][4 * j + 2 * i] + b.x, p.slope),
+                                                                               lrelu(acc[h][4 * j + 2 * i + 1] + b.y, p.slope));
+                }
+            }
+        }
+    }
+    if constexpr (MC) cluster_sync();
 }
 
 
@@ -677,13 +829,13 @@ static CUtensorMapSwizzle swizzle_for(int kc) {
     return kc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (kc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-// NHWC fp16 activation [N,H,W,C]: box = KC channels x 16 columns x 8 rows x 1 image
-int v2e_make_act_tmap(CUtensorMap *tm, const void *ptr, int N, int H, int W, int C, int KC) {
+// NHWC fp16 activation [N,H,W,C]: box = KC channels x 16 columns x tile_h rows x 1 image
+static int make_act_tmap_h(CUtensorMap *tm, const void *ptr, int N, int H, int W, int C, int KC, int tile_h) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) return v2e_set_error(V2E_E_CUDA, "cuTensorMapEncodeTiled unavailable%s", "");
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)kTileW, (cuuint32_t)kTileH, 1};
+    cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)kTileW, (cuuint32_t)tile_h, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
     CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void *)ptr, dims, strides, box, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -693,6 +845,9 @@ int v2e_make_act_tmap(CUtensorMap *tm, const void *ptr, int N, int H, int W, int
         return v2e_set_error(V2E_E_CUDA, "cuTensorMapEncodeTiled failed: %s", g_conv_err);
     }
     return V2E_OK;
+}
+int v2e_make_act_tmap(CUtensorMap *tm, const void *ptr, int N, int H, int W, int C, int KC) {
+    return make_act_tmap_h(tm, ptr, N, H, W, C, KC, kTileH);
 }
 
 // weights [Cout_pad][Ktot] fp16: box = KC x BN
@@ -719,41 +874,107 @@ int v2e_conv_pick_kc(int C1, int C2) {
 }
 int v2e_conv_pick_bn(int Cout_pad) { return Cout_pad >= 128 ? 128 : Cout_pad; }
 
+// Per-tap tiles (pixels x output channels): V2E_CONV_TILE_LEGACY = 128 x min(Cout_pad, 128) (conv_tc_kernel),
+// V2E_CONV_TILE_256x128 and V2E_CONV_TILE_128x256 (conv_wide_kernel, MH = 2 / 1).
+static void tile_shape(int tile, int Cout_pad, int *mh, int *bn) {
+    *mh = tile == V2E_CONV_TILE_256x128 ? 2 : 1;
+    *bn = tile == V2E_CONV_TILE_128x256 ? 256 : (tile == V2E_CONV_TILE_256x128 ? 128 : v2e_conv_pick_bn(Cout_pad));
+}
+
+// Wave-aware choice of the tile (wide tiles without multicast, the default). A CTA's time per (tap, slab) stage is
+// the larger of its L2-to-shared-memory bytes at ~24 B/clk per SM (6-7 TB/s over 132 SMs, the rate the 128 x 128
+// tile runs at) and its MMAs at 4096 dense fp16 FLOP/clk per SM; every tile runs the same stages per CTA, so a layer
+// costs waves x (time per stage). One CTA per SM (the stages fill the shared memory). Ties go to the 128 x 128 tile.
+// The wide tiles need 64-channel slabs.
+extern "C" int v2e_conv_pick_tile(int C1, int C2, int Cout_pad, int KH, int KW, int N, int H, int W, int n_sms) {
+    (void)KH; (void)KW;
+    const int kc = v2e_conv_pick_kc(C1, C2);
+    if (n_sms < 1) n_sms = 1;
+    int best = V2E_CONV_TILE_LEGACY;
+    double best_cost = 0.0;
+    for (int tile = V2E_CONV_TILE_LEGACY; tile <= V2E_CONV_TILE_128x256; tile++) {
+        int mh, bn;
+        tile_shape(tile, Cout_pad, &mh, &bn);
+        const bool wide = tile != V2E_CONV_TILE_LEGACY;
+        // one wide candidate per layer: 16x16 pixels for Cout_pad = 128, 256 channels from Cout_pad = 256 on
+        if (wide && (kc != 64 || Cout_pad % bn || (tile == V2E_CONV_TILE_256x128) != (Cout_pad == 128))) continue;
+        long tiles = (long)((W + kTileW - 1) / kTileW) * ((H + kTileH * mh - 1) / (kTileH * mh)) * N;
+        const long ctas = tiles * (Cout_pad / bn);
+        const long waves = (ctas + n_sms - 1) / n_sms;
+        const double a_bytes = (double)kBM * mh * kc * 2, b_bytes = (double)bn * kc * 2;
+        const double flops = 2.0 * kBM * mh * bn * kc;
+        const double per_stage = fmax((a_bytes + b_bytes) / 24.0, flops / 4096.0);
+        const double cost = (double)waves * per_stage;
+        if (tile == V2E_CONV_TILE_LEGACY || cost < best_cost) { best = tile; best_cost = cost; }
+    }
+    return best;
+}
+
 struct V2eConvLaunch {
     CUtensorMap tmA, tmA2, tmB;
     ConvParams p;
-    dim3 grid;
+    dim3 grid, cluster;
+    int mh, multicast;
     size_t smem;
 };
 
+// V2E_CONV_TILE (A/B measurements): "legacy" = the 128 x 128 tile for every layer, "multicast" = the picked tiles,
+// the wide ones with weight multicast over CTA pairs; unset = the picked tiles without multicast (on an H100 the
+// pairs took about 1.5x as long as unicast wide tiles, DESIGN.md section 5)
+static int conv_tile_env() {
+    static int v = -1;
+    if (v < 0) {
+        const char *e = getenv("V2E_CONV_TILE");
+        v = !e ? 0 : (!strcmp(e, "legacy") ? 1 : (!strcmp(e, "multicast") ? 2 : 0));
+    }
+    return v;
+}
+
 int v2e_conv_prepare(V2eConvLaunch *L, const void *x1, int C1, const void *x2, int C2, const void *wgt,
                      const float *bias, int Cout_pad, int KH, int KW, int N, int H, int W, void *out,
-                     int out_cstride, int out_mode, int co_real, float slope) {
+                     int out_cstride, int out_mode, int co_real, float slope, int tile, int multicast, int n_sms) {
     if (C1 % 16 || C2 % 16 || !(Cout_pad == 16 || Cout_pad == 32 || Cout_pad == 64 || (Cout_pad > 0 && Cout_pad % 128 == 0)))
         return v2e_set_error(V2E_E_INVALID, "conv: channel counts must be padded to 16 (Cout to 16/32/64/128k)%s", "");
+    if (tile == V2E_CONV_TILE_AUTO) {
+        const int env = conv_tile_env();
+        tile = env == 1 ? V2E_CONV_TILE_LEGACY : v2e_conv_pick_tile(C1, C2, Cout_pad, KH, KW, N, H, W, n_sms);
+        multicast = env == 2;
+    }
+    if (tile < V2E_CONV_TILE_LEGACY || tile > V2E_CONV_TILE_128x256)
+        return v2e_set_error(V2E_E_INVALID, "conv: unknown tile%s", "");
     memset(L, 0, sizeof(*L));
     ConvParams &p = L->p;
+    int mh, bn;
+    tile_shape(tile, Cout_pad, &mh, &bn);
+    const bool wide = tile != V2E_CONV_TILE_LEGACY;
     p.N = N; p.H = H; p.W = W; p.C1 = C1; p.C2 = C2; p.KH = KH; p.KW = KW;
     p.KC = v2e_conv_pick_kc(C1, C2);
-    p.BN = v2e_conv_pick_bn(Cout_pad);
+    p.BN = bn;
+    if (wide && (Cout_pad % bn || out_mode != 0))
+        return v2e_set_error(V2E_E_INVALID, "conv: the wide tiles need fp16 output and Cout_pad a multiple of their width%s", "");
     p.stages = kStages;
     p.tiles_x = (W + kTileW - 1) / kTileW;
-    p.tiles_y = (H + kTileH - 1) / kTileH;
+    p.tiles_y = (H + kTileH * mh - 1) / (kTileH * mh);
+    p.n_tiles = p.tiles_x * p.tiles_y * N;
     p.out_cstride = out_cstride; p.out_mode = out_mode; p.co_real = co_real; p.slope = slope;
     p.bias = bias; p.out = out;
+    L->mh = mh;
+    L->multicast = wide && multicast;
     int rc;
-    if ((rc = v2e_make_act_tmap(&L->tmA, x1, N, H, W, C1, p.KC))) return rc;
-    if (C2) { if ((rc = v2e_make_act_tmap(&L->tmA2, x2, N, H, W, C2, p.KC))) return rc; }
+    if ((rc = make_act_tmap_h(&L->tmA, x1, N, H, W, C1, p.KC, kTileH * mh))) return rc;
+    if (C2) { if ((rc = make_act_tmap_h(&L->tmA2, x2, N, H, W, C2, p.KC, kTileH * mh))) return rc; }
     else L->tmA2 = L->tmA;
-    if ((rc = v2e_make_wgt_tmap(&L->tmB, wgt, Cout_pad, KH * KW * (C1 + C2), p.KC, p.BN))) return rc;
+    if ((rc = v2e_make_wgt_tmap(&L->tmB, wgt, Cout_pad, KH * KW * (C1 + C2), p.KC, L->multicast ? bn / 2 : bn))) return rc;
     {
         static int co_fast = -1;
         if (co_fast < 0) { const char *e = getenv("V2E_CONV_CO_FAST"); co_fast = e ? atoi(e) : 1; }
-        const unsigned tiles = (unsigned)(p.tiles_x * p.tiles_y * N), cob = (unsigned)(Cout_pad / p.BN);
+        // a multicast pair is two neighbouring pixel tiles: an odd count gets one padding CTA
+        const unsigned tiles = (unsigned)(L->multicast ? (p.n_tiles + 1) & ~1 : p.n_tiles), cob = (unsigned)(Cout_pad / p.BN);
         p.co_fast = (co_fast && cob > 1 && tiles <= 65535u) ? 1 : 0;
         L->grid = p.co_fast ? dim3(cob, tiles, 1) : dim3(tiles, cob, 1);
+        L->cluster = !L->multicast ? dim3(1, 1, 1) : (p.co_fast ? dim3(1, 2, 1) : dim3(2, 1, 1));
     }
-    size_t stage = (size_t)kBM * p.KC * 2 + (((size_t)p.BN * p.KC * 2 + 1023) & ~(size_t)1023);
+    size_t stage = (size_t)kBM * mh * p.KC * 2 + (((size_t)p.BN * p.KC * 2 + 1023) & ~(size_t)1023);
     L->smem = stage * p.stages + 1024;
     return V2E_OK;
 }
@@ -766,9 +987,31 @@ static cudaError_t conv_launch_bn(const V2eConvLaunch *L, cudaStream_t st) {
     return cudaGetLastError();
 }
 
+template <int MH, int BN, bool MC>
+static cudaError_t conv_launch_wide(const V2eConvLaunch *L, cudaStream_t st) {
+    static PerDeviceOnce attr_once;
+    if (attr_once.first())
+        cudaFuncSetAttribute(conv_wide_kernel<MH, BN, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = L->grid;
+    cfg.blockDim = dim3(kConvThreads, 1, 1);
+    cfg.dynamicSmemBytes = L->smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = L->cluster.x;
+    attr[0].val.clusterDim.y = L->cluster.y;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, conv_wide_kernel<MH, BN, MC>, L->tmA, L->tmA2, L->tmB, L->p);
+}
+
 int v2e_conv_launch(const V2eConvLaunch *L, cudaStream_t st) {
     cudaError_t e;
-    switch (L->p.BN) {
+    if (L->mh == 2 && L->p.BN == 128) e = L->multicast ? conv_launch_wide<2, 128, true>(L, st) : conv_launch_wide<2, 128, false>(L, st);
+    else if (L->mh == 1 && L->p.BN == 256) e = L->multicast ? conv_launch_wide<1, 256, true>(L, st) : conv_launch_wide<1, 256, false>(L, st);
+    else switch (L->p.BN) {
         case 16: e = conv_launch_bn<16>(L, st); break;
         case 32: e = conv_launch_bn<32>(L, st); break;
         case 64: e = conv_launch_bn<64>(L, st); break;
@@ -782,15 +1025,30 @@ int v2e_conv_launch(const V2eConvLaunch *L, cudaStream_t st) {
 size_t v2e_conv_launch_size(void) { return sizeof(V2eConvLaunch); }
 
 // ---- standalone C-ABI entry (tests, and integrators who bring their own network driver) -------------
+static int device_sms() {
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms;
+}
+
+extern "C" int v2e_conv2d_lrelu_sm100_tile(const void *x1_dev, int C1, const void *x2_dev, int C2,
+                                           const void *wgt_dev, const float *bias_dev, int Cout_pad, int KH, int KW,
+                                           int N, int H, int W, void *out_dev, int out_cstride, int out_mode,
+                                           int co_real, float slope, int tile, int multicast, void *stream) {
+    V2eConvLaunch L;
+    int rc = v2e_conv_prepare(&L, x1_dev, C1, x2_dev, C2, wgt_dev, bias_dev, Cout_pad, KH, KW, N, H, W, out_dev,
+                              out_cstride, out_mode, co_real, slope, tile, multicast, device_sms());
+    if (rc) return rc;
+    return v2e_conv_launch(&L, (cudaStream_t)stream);
+}
+
 extern "C" int v2e_conv2d_lrelu_sm100(const void *x1_dev, int C1, const void *x2_dev, int C2,
                                       const void *wgt_dev, const float *bias_dev, int Cout_pad, int KH, int KW,
                                       int N, int H, int W, void *out_dev, int out_cstride, int out_mode,
                                       int co_real, float slope, void *stream) {
-    V2eConvLaunch L;
-    int rc = v2e_conv_prepare(&L, x1_dev, C1, x2_dev, C2, wgt_dev, bias_dev, Cout_pad, KH, KW, N, H, W, out_dev,
-                              out_cstride, out_mode, co_real, slope);
-    if (rc) return rc;
-    return v2e_conv_launch(&L, (cudaStream_t)stream);
+    return v2e_conv2d_lrelu_sm100_tile(x1_dev, C1, x2_dev, C2, wgt_dev, bias_dev, Cout_pad, KH, KW, N, H, W, out_dev,
+                                       out_cstride, out_mode, co_real, slope, V2E_CONV_TILE_AUTO, 0, stream);
 }
 
 // ---- strip kernel host side ------------------------------------------------------------------------

@@ -28,7 +28,7 @@
 struct V2eConvLaunch;
 int v2e_conv_prepare(V2eConvLaunch *L, const void *x1, int C1, const void *x2, int C2, const void *wgt,
                      const float *bias, int Cout_pad, int KH, int KW, int N, int H, int W, void *out,
-                     int out_cstride, int out_mode, int co_real, float slope);
+                     int out_cstride, int out_mode, int co_real, float slope, int tile, int multicast, int n_sms);
 int v2e_conv_launch(const V2eConvLaunch *L, cudaStream_t st);
 size_t v2e_conv_launch_size(void);
 struct V2eStripLaunch;
@@ -521,7 +521,8 @@ static int conv(V2eSlomo *h, const UNet &u, int li, const __half *x1, const __ha
                                pool_out, u.cout_pad[li]);
     else
         rc = v2e_conv_prepare(L, x1, u.c1p[li], x2, x2 ? u.c2p[li] : 0, u.w[li], u.b[li], u.cout_pad[li], u.L[li].k,
-                              u.L[li].k, B, H, W, out, u.cout_pad[li], out_mode, u.L[li].cout, kSlope);
+                              u.L[li].k, B, H, W, out, u.cout_pad[li], out_mode, u.L[li].cout, kSlope,
+                              V2E_CONV_TILE_AUTO, 0, h->n_sms);
     if (rc) return rc;
     if (h->profile) {
         if (h->ev_used + 2 > h->ev.size()) {
