@@ -152,7 +152,10 @@ int v2e_emu_step(V2eEmu *h, const void *frames_dev, int frame_dtype, int T,
  * rows, counters and state are identical to the frame-by-frame kernels'. It relies on the refractory filter not
  * running (refractory_period_s <= dt / max_n in every frame, emulator.py:830) and on max_n <= 31; a chunk that
  * breaks this is rejected on the device (nothing emitted, state untouched) and v2e_emu_collect replays it frame by
- * frame before it returns. option 0 of v2e_emu_set_option: 0 = never take the fast path (A/B tests), 1 = default. */
+ * frame before it returns. option 0 of v2e_emu_set_option: 0 = never take the fast path (A/B tests), 1 = default.
+ * option 1: 1 = the photoreceptor-noise Philox counters (rng_mode 1) use rng_pixel_offset + pixel like the leak and
+ * shot counters, so that a row band of a pixel-sharded clip draws what one GPU draws; 0 = the handle's own pixel index
+ * (default). */
 int v2e_emu_set_option(V2eEmu *h, int option, int value);
 /* The fast path in two halves for a pixel-sharded clip (SURVEY.md 8e): v2e_emu_fused_count enqueues the register-
  * resident update of the T frames and the per-frame counts; the caller all-reduces (MAX) the T int32 at
@@ -270,7 +273,8 @@ void *v2e_emu_state_ptr(V2eEmu *h, int which);
  * for every pixel of the handle, from the same device functions the kernels use. Each non-null output is a device
  * array of H*W float32 indexed by the handle's pixel index: leak_randn the leak-jitter normal, shot_u01 the full
  * shot-noise uniform (the kernels only complete it for prefix candidates), pr_randn the photoreceptor-noise normal.
- * Leak and shot counters use rng_pixel_offset + pixel, like the kernels. Frame k >= 1 of a clip (frame 0 only
+ * Leak and shot counters use rng_pixel_offset + pixel, like the kernels; the photoreceptor counters too after
+ * v2e_emu_set_option(h, 1, 1), else the handle's pixel. Frame k >= 1 of a clip (frame 0 only
  * initialises) is drawn with frame_index k - 1. Asynchronous on `stream`. */
 int v2e_emu_draw_noise(V2eEmu *h, uint32_t frame_index, float *leak_randn, float *shot_u01, float *pr_randn,
                        void *stream);

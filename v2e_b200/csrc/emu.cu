@@ -88,6 +88,8 @@ struct EmuDev {                         // passed by value to every kernel
     int32_t units;                      // ceil(n / 128)
     uint32_t px_off;                    // global index of this handle's pixel 0 (row band of a pixel-sharded clip):
                                         // Philox counters use global pixel indices
+    uint32_t pr_off;                    // offset of the photoreceptor-noise counters: 0 (the handle's own pixel index,
+                                        // the default), or px_off after v2e_emu_set_option(h, 1, 1)
     // optional pixel models (emulator.py:58-80, 694-703, 719-725)
     int32_t scidvs, pr_noise;
     void *hp, *prev_photo;              // scidvs_highpass / scidvs_previous_photo, state dtype
@@ -246,9 +248,9 @@ __device__ __forceinline__ void noise_px4(uint64_t seed, uint32_t g0, uint32_t f
     else noise_px4_unaligned(seed, g0, frame_index, n, pref);
 }
 // Photoreceptor-noise normals (emulator.py:698) of pixels 4q .. 4q+3 from one Philox call; radius and angle from 24
-// bits each. q is the handle's LOCAL quad index, not one offset by px_off like the leak / shot streams: that is safe
-// because a handle with photoreceptor_noise is never a row band (pixel sharding refuses the model: v2e_emu_phase_update,
-// v2e_emu_cs_begin), so its local and whole-frame pixel indices coincide.
+// bits each. The pixel index is the handle's own plus d.pr_off: 0 by default, the handle's rng_pixel_offset once
+// v2e_emu_set_option(h, 1, 1) makes the stream count whole-frame pixels like the leak / shot streams (a row band of
+// a pixel-sharded clip then draws what one GPU draws).
 __device__ __forceinline__ void pr_noise_quad(uint64_t seed, uint32_t quad, uint32_t frame_index, float rn[4]) {
     const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
     const uint4 r = philox4x32<kPhiloxRounds>(make_uint4(quad, frame_index, 2u, 0x70726e7au), key);
@@ -257,6 +259,19 @@ __device__ __forceinline__ void pr_noise_quad(uint64_t seed, uint32_t quad, uint
     __sincosf(6.283185307179586f * u01_half(r.y), &sa, &ca);
     __sincosf(6.283185307179586f * u01_half(r.w), &sb, &cb);
     rn[0] = a * ca; rn[1] = a * sa; rn[2] = b * cb; rn[3] = b * sb;
+}
+// photoreceptor-noise normals of the 4 consecutive pixels starting at GLOBAL index g0 (a row band of a sharded clip
+// may start mid-quad: two calls, out of line)
+__device__ __noinline__ void pr_noise_px4_unaligned(uint64_t seed, uint32_t g0, uint32_t frame_index, float *rn) {
+    const uint32_t q = g0 >> 2, r = g0 & 3u;
+    float ra[8];
+    pr_noise_quad(seed, q, frame_index, ra);
+    pr_noise_quad(seed, q + 1, frame_index, ra + 4);
+    for (int k = 0; k < 4; k++) rn[k] = ra[r + k];
+}
+__device__ __forceinline__ void pr_noise_px4(uint64_t seed, uint32_t g0, uint32_t frame_index, float rn[4]) {
+    if ((g0 & 3u) == 0) pr_noise_quad(seed, g0 >> 2, frame_index, rn);
+    else pr_noise_px4_unaligned(seed, g0, frame_index, rn);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -736,7 +751,7 @@ __global__ void __launch_bounds__(kThreads) emu_front_kernel(EmuDev d, FramePara
     if (d.pr_noise) {
         ld4(d.noise_arr, i0, na);
         if (pr_randn) load_f32x4_any(pr_randn, i0, d.n, rn);
-        else pr_noise_quad(d.seed, (uint32_t)(i0 >> 2), p.frame_index, rn);
+        else pr_noise_px4(d.seed, (uint32_t)i0 + d.pr_off, p.frame_index, rn);
     }
 #pragma unroll
     for (int k = 0; k < 4; k++) {
@@ -1876,7 +1891,7 @@ __global__ void __launch_bounds__(kThreads) emu_plan_kernel(EmuDev d, FrameParam
 }
 
 // v2e_emu_draw_noise: the device-RNG draws of one frame index for EVERY pixel of the handle, through the same
-// functions the update / fused / front kernels call (noise_px4, shot_uniform, pr_noise_quad). Those kernels draw the
+// functions the update / fused / front kernels call (noise_px4, shot_uniform, pr_noise_px4). Those kernels draw the
 // shot uniform's low bits only for prefix candidates; here every pixel gets its full uniform.
 __global__ void __launch_bounds__(kThreads) emu_draw_noise_kernel(EmuDev d, uint32_t frame_index, float *leak_randn,
                                                                   float *shot_u01, float *pr_randn) {
@@ -1886,7 +1901,7 @@ __global__ void __launch_bounds__(kThreads) emu_draw_noise_kernel(EmuDev d, uint
     float lr[4], rn[4];
     uint32_t pref[4];
     noise_px4(d.seed, g0, frame_index, lr, pref);
-    if (pr_randn) pr_noise_quad(d.seed, (uint32_t)(i0 >> 2), frame_index, rn);
+    if (pr_randn) pr_noise_px4(d.seed, (uint32_t)i0 + d.pr_off, frame_index, rn);
     for (int k = 0; k < 4 && i0 + k < d.n; k++) {
         if (leak_randn) leak_randn[i0 + k] = lr[k];
         if (shot_u01) shot_u01[i0 + k] = shot_uniform(d.seed, (g0 + k) >> 2, frame_index, (int)((g0 + k) & 3u), pref[k]);
@@ -2402,6 +2417,34 @@ static int cs_plan(const V2eEmu *h, const FrameParams &p, int *num_steps, double
     return V2E_OK;
 }
 
+// optional front end (SCIDVS / photoreceptor noise) of one frame: low-pass unless lp_done, noise IIR, nonlinear
+// high-pass -> pr_eff, which the update kernel then reads with lp_done = 1
+static int enqueue_front(const EmuDev &d, const FrameParams &p, const void *frame, int dtype, const float *pr_randn,
+                         int lp_done, cudaStream_t st) {
+    const int g = grid_for(d);
+#define FRONT(S_)                                                                                                  \
+    switch (dtype) {                                                                                                \
+        case V2E_U8: emu_front_kernel<S_, V2E_U8><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break;   \
+        case V2E_F32: emu_front_kernel<S_, V2E_F32><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break; \
+        case V2E_F64: emu_front_kernel<S_, V2E_F64><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break; \
+        default: return fail(V2E_E_INVALID, "bad frame dtype");                                                     \
+    }
+    if (d.state_f64) { FRONT(double) } else { FRONT(float) }
+#undef FRONT
+    return V2E_OK;
+}
+
+// the photoreceptor-noise inputs of a single-frame step (v2e_emu_set_pr_noise): amplitude into p, the replay field
+static int take_pr_noise(V2eEmu *h, FrameParams &p, const float **prn, const char *caller) {
+    *prn = nullptr;
+    if (!h->d.pr_noise) return V2E_OK;
+    if (h->pr_T < 1) return fail(V2E_E_STATE, "v2e_emu_set_pr_noise must precede %s", caller);
+    p.pr_vrms_f = (float)h->pr_vrms[0];
+    *prn = h->pr_randn_dev;
+    h->pr_T = 0;
+    return V2E_OK;
+}
+
 // enqueue the counting kernels of one frame into `slot`
 static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int dtype, const float *lr,
                          const float *sr, int shot_pending, int slot, cudaStream_t st, const float *pr_randn = nullptr) {
@@ -2421,16 +2464,7 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
     }
     if (d.scidvs || d.pr_noise) {
         // low-pass (unless the surround path just did it), noise IIR, nonlinear high-pass -> pr_eff
-        const int g = grid_for(d);
-#define FRONT(S_)                                                                                                  \
-        switch (dtype) {                                                                                            \
-            case V2E_U8: emu_front_kernel<S_, V2E_U8><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break;   \
-            case V2E_F32: emu_front_kernel<S_, V2E_F32><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break; \
-            case V2E_F64: emu_front_kernel<S_, V2E_F64><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break; \
-            default: return fail(V2E_E_INVALID, "bad frame dtype");                                                 \
-        }
-        if (d.state_f64) { FRONT(double) } else { FRONT(float) }
-#undef FRONT
+        if ((rc = enqueue_front(d, p, frame, dtype, pr_randn, lp_done, st))) return rc;
         lp_done = 1;
     }
     if (d.csdvs) {
@@ -2686,6 +2720,7 @@ static int run_schedule(V2eEmu *h, int from, cudaStream_t st) {
 extern "C" int v2e_emu_set_option(V2eEmu *h, int option, int value) {
     if (!h) return fail(V2E_E_INVALID, "null handle");
     if (option == 0) { h->fused_enable = value ? 1 : 0; return V2E_OK; }
+    if (option == 1) { h->d.pr_off = value ? h->d.px_off : 0u; return V2E_OK; }
     return fail(V2E_E_INVALID, "unknown option");
 }
 extern "C" int v2e_emu_fused_stats(V2eEmu *h, long long *chunks, long long *rejected) {
@@ -3037,12 +3072,7 @@ extern "C" int v2e_emu_phase_count(V2eEmu *h, const void *frame, int dtype, doub
     FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
     h->last_dt = p.dt;
     const float *prn = nullptr;
-    if (h->d.pr_noise) {
-        if (h->pr_T < 1) return fail(V2E_E_STATE, "v2e_emu_set_pr_noise must precede v2e_emu_phase_count");
-        p.pr_vrms_f = (float)h->pr_vrms[0];
-        prn = h->pr_randn_dev;
-        h->pr_T = 0;
-    }
+    if ((rc = take_pr_noise(h, p, &prn, "v2e_emu_phase_count"))) return rc;
     if ((rc = enqueue_count(h, p, frame, dtype, lr, sr, shot_pending, 0, st, prn))) return rc;
     h->scidvs_started = 1;
     CU(cudaGetLastError());
@@ -3068,11 +3098,19 @@ extern "C" int v2e_emu_phase_update(V2eEmu *h, const void *frame, int dtype, dou
     const EmuDev &d = h->d;
     if (d.rng_mode == 0 && d.leak_on && !lr) return fail(V2E_E_INVALID, "leak_randn field required in replay mode");
     if (d.csdvs) return fail(V2E_E_UNSUPPORTED, "centre-surround model: a pixel-sharded handle is stepped with v2e_emu_cs_* (cs_halo_rows > 0)");
-    if (d.scidvs || d.pr_noise) return fail(V2E_E_UNSUPPORTED, "pixel sharding with scidvs / photoreceptor_noise is not built");
-    rc = d.state_f64 ? launch_update<double>(h, p, frame, dtype, lr, sr, 0, 0, 0, st)
-                     : launch_update<float>(h, p, frame, dtype, lr, sr, 0, 0, 0, st);
+    // SCIDVS / photoreceptor noise: the front end on the band's rows (the noise draws use whole-frame pixel indices)
+    int lp_done = 0;
+    if (d.scidvs || d.pr_noise) {
+        const float *prn = nullptr;
+        if ((rc = take_pr_noise(h, p, &prn, "v2e_emu_phase_update"))) return rc;
+        if ((rc = enqueue_front(d, p, frame, dtype, prn, 0, st))) return rc;
+        lp_done = 1;
+    }
+    rc = d.state_f64 ? launch_update<double>(h, p, frame, dtype, lr, sr, 0, 0, lp_done, st)
+                     : launch_update<float>(h, p, frame, dtype, lr, sr, 0, 0, lp_done, st);
     if (rc) return rc;
     CU(cudaGetLastError());
+    h->scidvs_started = 1;
     h->last_T = 1;
     return V2E_OK;
 }
@@ -3085,7 +3123,6 @@ extern "C" int v2e_emu_cs_begin(V2eEmu *h, const void *frame, int dtype, double 
     if (!h || !frame || !num_steps) return fail(V2E_E_INVALID, "null argument");
     if (!h->first_done) return fail(V2E_E_STATE, "v2e_emu_first_frame must run first");
     if (!h->d.csdvs || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle (cs_halo_rows)");
-    if (h->d.scidvs || h->d.pr_noise) return fail(V2E_E_UNSUPPORTED, "pixel sharding with scidvs / photoreceptor_noise is not built");
     if (t_frame < t_previous) return fail(V2E_E_INVALID, "frame times must be non-decreasing");
     cudaStream_t st = (cudaStream_t)stream;
     const EmuDev &d = h->d;
@@ -3096,6 +3133,14 @@ extern "C" int v2e_emu_cs_begin(V2eEmu *h, const void *frame, int dtype, double 
     h->last_dt = p.dt;
     if ((rc = cs_plan(h, p, &h->cs_num_steps, &h->cs_alpha_p, &h->cs_alpha_h))) return rc;
     if ((rc = launch_lp(d, p, frame, dtype, st))) return rc;
+    if (d.scidvs || d.pr_noise) {
+        // SCIDVS / photoreceptor noise on every row of the handle, halo rows included (computed redundantly, like lp;
+        // the surround reads lp only, and halo rows neither emit nor enter the frame maximum)
+        const float *prn = nullptr;
+        if ((rc = take_pr_noise(h, p, &prn, "v2e_emu_cs_begin"))) return rc;
+        if ((rc = enqueue_front(d, p, frame, dtype, prn, 1, st))) return rc;
+        h->scidvs_started = 1;
+    }
     CU(cudaMemsetAsync(d.cs_max, 0, (size_t)h->cs_num_steps * sizeof(unsigned long long), st));
     CU(cudaMemsetAsync(d.cs_done, 0, sizeof(int32_t), st));
     CU(cudaGetLastError());

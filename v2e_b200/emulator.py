@@ -22,7 +22,8 @@ reference's own writer classes (v2ecore.output.*, h5py) when those import, and f
 them (emulator.py:953-975); when they do not import the keyword is ignored with a warning. The DVS text body is
 formatted on the device (v2e_b200.sinks.events_to_text) and written to the writer's file. label_signal_noise
 labels every returned row signal (1) or shot noise (0) -- `last_signnoise_label`, generate_events_batch(...,
-return_labels=True) -- and passes the labels to the text and AEDAT-2.0 sinks; pixel-sharded emulators ignore it.
+return_labels=True) -- and passes the labels to the text and AEDAT-2.0 sinks. A pixel-sharded emulator labels its own
+rows (generate_events_band(_batch)(..., return_labels=True)) and writes no sink: a file needs the merged stream.
 show_dvs_model_state / record_single_pixel_states (GUI / debug probes) are ignored with a warning.
 """
 import ctypes
@@ -226,8 +227,6 @@ class EventEmulator(object):
             # emulator.py:196-204 logs and calls v2e_quit(1)
             logger.warning("--photoreceptor_noise needs a finite --shot_noise_rate_hz and --cutoff_hz")
             raise SystemExit(1)
-        if (photoreceptor_noise or scidvs) and shard is not None:
-            raise NotImplementedError("pixel sharding with scidvs / photoreceptor_noise is not built")
         if record_single_pixel_states is not None:          # emulator.py:279-290: same argument checks
             if not (type(record_single_pixel_states) is tuple):
                 raise ValueError(f'--record_single_pixel_states {record_single_pixel_states} should be a tuple, e.g. (10,20)')
@@ -264,8 +263,6 @@ class EventEmulator(object):
         self.output_width = output_width
         self.output_height = output_height
         self.label_signal_noise = label_signal_noise
-        if label_signal_noise and shard is not None:
-            logger.warning("label_signal_noise is ignored by a pixel-sharded emulator: its rows are not labelled")
         self.last_signnoise_label = None     # label_signal_noise: labels of the rows generate_events last returned
         self.log_input = hdr
         self.scidvs = scidvs
@@ -432,6 +429,9 @@ class EventEmulator(object):
             self._h = h
             if not self.fused:
                 _lib.check(self._lib.v2e_emu_set_option(h, 0, 0))
+            if self.shard is not None:
+                # a row band's photoreceptor-noise draws count whole-frame pixels, like its leak / shot draws
+                _lib.check(self._lib.v2e_emu_set_option(h, 1, 1))
             lut = _linlog_lut()
             _lib.check(self._lib.v2e_emu_set_linlog_lut(h, ctypes.c_void_p(lut.data_ptr()), self._stream()))
         self._H, self._W = H, W
@@ -550,7 +550,30 @@ class EventEmulator(object):
     def _pr_vrms(self, delta_time):
         """emulator.py:695-697 -> emulator_utils.py:177-295: host-side calibration of the Gaussian noise
         amplitude that gives the requested shot-noise rate after the RC low-pass; cached per sample rate
-        (+-10 %). Like the reference it draws from an unseeded numpy generator."""
+        (+-10 %). Like the reference it draws from an unseeded numpy generator, so a pixel-sharded emulator takes the
+        amplitude of the shard group's first rank, broadcast to every rank (each rank still pops its own tape)."""
+        if self.shard is not None:
+            import torch.distributed as dist
+            group = self.shard[2]
+            first = dist.get_global_rank(group, 0) if group is not None else 0
+            mine = dist.get_rank() == first
+            v = 0.0
+            if mine:
+                v = self._pr_vrms_local(delta_time)
+            elif self._pr_vrms_tape is not None:
+                self._pr_vrms_tape.pop(0)
+            # the amplitude and the first rank's calibration cache (sample rate, amplitude; nan: empty)
+            msg = [v] + [math.nan if c is None else float(c) for c in self._vn_cache]
+            vt = torch.tensor(msg, dtype=torch.float64, device=self.device)
+            dist.broadcast(vt, src=first, group=group)
+            v, rate, cached = vt.tolist()
+            self._vn_cache = [None if math.isnan(rate) else rate, None if math.isnan(cached) else cached]
+        else:
+            v = self._pr_vrms_local(delta_time)
+        self.photoreceptor_noise_vrms = v
+        return v
+
+    def _pr_vrms_local(self, delta_time):
         if self._pr_vrms_tape is not None:
             v = float(self._pr_vrms_tape.pop(0))
         else:
@@ -576,7 +599,6 @@ class EventEmulator(object):
                     rout[i] = acc
                 v = float(np.std(rin) / np.std(rout) * vn)
                 self._vn_cache = [rate, v]
-        self.photoreceptor_noise_vrms = v
         return v
 
     # one frame through the single-frame phase functions, host draws interleaved like the reference's ---------
@@ -602,10 +624,11 @@ class EventEmulator(object):
             return draw((H, W))[ye0:ye0 + self._H].contiguous().to(self.device)
         with torch.cuda.device(self.device):
             st = self._stream()
-            if replay and self.photoreceptor_noise:
-                # emulator.py:694-698: amplitude, then the randn draw, before the leak's
+            if self.photoreceptor_noise:
+                # emulator.py:694-698: amplitude, then the randn draw (replay mode; device mode draws it in the kernel),
+                # before the leak's
                 vr = (ctypes.c_double * 1)(self._pr_vrms(t_frame - tp))
-                pr_dev = field(self.rng.randn)
+                pr_dev = field(self.rng.randn) if replay else None
                 _lib.check(L.v2e_emu_set_pr_noise(h, p(pr_dev), vr, 1))
             lr_dev = field(self.rng.randn) if replay and self.leak_rate_hz > 0 else None
             self._grow_event_buffer(self.event_rows_hint or max(4 * self._H * W, 1 << 16))
@@ -696,12 +719,16 @@ class EventEmulator(object):
         from .parallel import band_with_halo
         return band_with_halo(H, self.shard[0], self.shard[1], self.cs_halo_rows(H))
 
-    def generate_events_band(self, band_frame, t_frame, full_height):
+    def generate_events_band(self, band_frame, t_frame, full_height, return_labels=False):
         """Pixel-sharded operation with the rows already cut: band_frame is [y1-y0, W], this rank's rows
         (v2e_b200.parallel.row_band) of a frame of `full_height` rows -- what the frame exchange of
-        V2EPipeline.run_clip_sharded delivers. Same contract as generate_events otherwise."""
+        V2EPipeline.run_clip_sharded delivers. Same contract as generate_events otherwise.
+        return_labels=True (needs label_signal_noise=True) returns (rows, labels): the band's labels, a bool ndarray
+        aligned with its rows (None with the rows)."""
         if self.shard is None:
             raise RuntimeError("generate_events_band needs shard=(rank, world, group)")
+        if return_labels and not self.label_signal_noise:
+            raise ValueError("return_labels=True needs label_signal_noise=True")
         t_frame = float(t_frame)
         self.frame_counter += 1
         self._frame_times([t_frame], 1)
@@ -709,15 +736,23 @@ class EventEmulator(object):
         y0, y1 = self.ext_band(int(full_height))       # the band (+ halo rows for the centre-surround model)
         if fr.dim() != 2 or fr.shape[0] != y1 - y0:
             raise ValueError("band_frame must hold rows [%d, %d) of the frame" % (y0, y1))
-        return self._generate_band(fr, code, t_frame, int(full_height))
+        ev = self._generate_band(fr, code, t_frame, int(full_height))
+        return (ev, self.last_signnoise_label) if return_labels else ev
 
     def _generate_band(self, fr, code, t_frame, H, return_device=False):
-        """Rows ext_band(H) of one frame of H rows."""
+        """Rows ext_band(H) of one frame of H rows. With label_signal_noise, last_signnoise_label labels the band's
+        rows: its last n_shot_on + n_shot_off rows are the shot noise of the band (emulator.py:889-923)."""
+        self.last_signnoise_label = None
         if not self._initialized:
             self._first_frame(fr, code, t_frame, H)
             return None
         ev = self._phase_frame(fr, code, t_frame, return_device)
         self.t_previous = t_frame
+        if ev is not None and self.label_signal_noise:
+            fi = self.last_frame_info
+            label = np.ones(len(ev), dtype=bool)
+            label[len(ev) - (int(fi.n_shot_on) + int(fi.n_shot_off)):] = False
+            self.last_signnoise_label = label
         return ev
 
     def _cs_iterate(self, fp, code, t_frame, tp, cap, lrp, st, W):
@@ -759,17 +794,22 @@ class EventEmulator(object):
             _lib.check(L.v2e_emu_cs_advance(h, s0, s1, st))
         _lib.check(L.v2e_emu_cs_update(h, fp, code, lrp, None, st))
 
-    def generate_events_band_batch(self, band_frames, t_frames, full_height, return_device=False):
+    def generate_events_band_batch(self, band_frames, t_frames, full_height, return_device=False, return_labels=False):
         """Pixel-sharded, batched (BASELINE config 5 without per-frame host work): band_frames [T, y1-y0, W] uint8,
         this rank's rows of T consecutive frames. The multi-frame kernels run the whole chunk with per-pixel state in
         registers; the only exchange is ONE all-reduce(MAX) of the T frame maxima (SURVEY.md 8e "batch as a [T]
         vector"). A chunk in which the refractory filter would run is replayed frame by frame (one all-reduce per
-        frame), identically on every rank. Needs rng_mode='device' when leak / shot noise is on.
-        Returns (rows [N,4] float32 with global y, offsets [T+1]) like generate_events_batch."""
+        frame), identically on every rank; so is every chunk with SCIDVS or photoreceptor noise, which the multi-frame
+        kernels do not take. Needs rng_mode='device' when leak / shot / photoreceptor noise is on.
+        Returns (rows [N,4] float32 with global y, offsets [T+1]) like generate_events_batch; return_labels=True (needs
+        label_signal_noise=True) adds the band's labels like generate_events_batch(..., return_labels=True)."""
         import torch.distributed as dist
         if self.shard is None:
             raise RuntimeError("generate_events_band_batch needs shard=(rank, world, group)")
-        if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0):
+        if return_labels and not self.label_signal_noise:
+            raise ValueError("return_labels=True needs label_signal_noise=True")
+        if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
+                                          self.photoreceptor_noise):
             raise RuntimeError("batched sharded operation with per-frame noise needs rng_mode='device'")
         rank, world, group = self.shard
         fr, code = self._to_device_frames(band_frames)
@@ -780,7 +820,7 @@ class EventEmulator(object):
         T = fr.shape[0]
         t_frames = self._frame_times(t_frames, T)
         L = self._lib
-        out, offs = [], [0]
+        out, offs, n_shot = [], [0], []
         state = {"total": 0}
         n = (y1 - y0) * fr.shape[2]
 
@@ -817,6 +857,7 @@ class EventEmulator(object):
                 for k in range(Tc):
                     self._account(info[k])
                     offs.append(state["total"] + int(info[k].ev_base) + int(info[k].n_events))
+                    n_shot.append(int(info[k].n_shot_on) + int(info[k].n_shot_off))
                 nrows = int(rows.value)
                 ev = self._ev_dev[:nrows].clone()
                 ev[:, 2] += y0
@@ -831,10 +872,12 @@ class EventEmulator(object):
             for k in range(a, b):
                 self.frame_counter += 1
                 evk = self._generate_band(fr[k], code, t_frames[k], H, return_device=True)
+                fi = self.last_frame_info
                 if evk is not None:
                     out.append(evk)
                     state["total"] += len(evk)
                 offs.append(state["total"])
+                n_shot.append(0 if evk is None else int(fi.n_shot_on) + int(fi.n_shot_off))
 
         f = 0
         if not self._initialized:
@@ -855,9 +898,15 @@ class EventEmulator(object):
             f = e
         offs = np.asarray(offs, np.int64)
         rows = torch.cat(out, 0) if out else torch.zeros((0, 4), dtype=torch.float32, device=self.device)
-        if return_device:
-            return rows, offs
-        return rows.cpu().numpy(), offs
+        labels = None
+        if return_labels:
+            from .sinks import signnoise_labels
+            labels = signnoise_labels(offs, n_shot, self.device)
+            if not return_device:
+                labels = labels.cpu().numpy().astype(bool)
+        if not return_device:
+            rows = rows.cpu().numpy()
+        return (rows, offs, labels) if return_labels else (rows, offs)
 
     def _canonical_then_shuffle(self, ev, counts, perms, shot_on, shot_off):
         """Device rows of one (iteration, polarity) group come in no particular order. The reference

@@ -45,6 +45,23 @@ def pair_range(n_pairs, rank, world):
     return p0, p0 + base + (1 if rank < extra else 0)
 
 
+def batch_pair_range(n_pairs, batch_size, rank, world):
+    """[p0, p1) of the consecutive frame pairs rank `rank` interpolates when ONE clip's SloMo is sharded over ranks
+    with a U chosen per batch (auto_upsample, slomo.py:366-385): the clip's batches of `batch_size` pairs, counted from
+    its first pair, are dealt to the ranks whole and contiguous, so that every rank's batches -- and so its U's -- are
+    those of a single-GPU run. Only the last rank gets the clip's short final batch. Raises ValueError when there are
+    fewer batches than ranks."""
+    if not (0 <= rank < world):
+        raise ValueError("rank out of range")
+    if batch_size < 1:
+        raise ValueError("batch_size must be >= 1")
+    n_batches = -(-n_pairs // batch_size)
+    if n_batches < world:
+        raise ValueError("fewer batches of frame pairs than ranks")
+    b0, b1 = pair_range(n_batches, rank, world)
+    return b0 * batch_size, min(b1 * batch_size, n_pairs)
+
+
 def band_with_halo(height, rank, world, halo=0):
     """row_band widened by `halo` rows either side, clipped to the frame (the centre-surround pixel model reads its
     neighbours' rows: emulator.py:1102-1124)."""

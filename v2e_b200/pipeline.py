@@ -27,46 +27,67 @@ class V2EPipeline:
         ev, offs = self.emulator.generate_events_batch(interp, t, return_device=return_device, copy=copy)
         return ev, offs, t, interp.shape[0]
 
-    def run_clip_sharded(self, frames_u8, src_duration_s, t_offset=0.0, group=None):
+    def run_clip_sharded(self, frames_u8, src_duration_s, t_offset=0.0, group=None, return_labels=False):
         """ONE clip over the ranks of `group` (BASELINE config 5 layout; SURVEY.md 8e). Every rank passes the
         same source frames; the emulator must have been built with shard=(rank, world, group).
-          1. SloMo over this rank's frame pairs (parallel.pair_range) -- no halo, weights replicated;
+          1. SloMo over this rank's frame pairs (parallel.pair_range) -- no halo, weights replicated. With
+             auto_upsample the pairs are whole batches (parallel.batch_pair_range), each rank picks the U of its
+             batches, and the ranks all-gather those U's to build the clip's times (slomo.clip_times);
           2. all-to-all of uint8 row bands (parallel.exchange_frame_bands);
           3. pixel model on this rank's rows of every frame (one all-reduce(MAX) of an int32 per frame).
         Returns (rows [M_r, 4] float32 host array of THIS rank's pixel rows (global y), interp_times_s,
-        n_interp_frames). Union over ranks = the events of the clip; parallel.gather_event_streams /
-        merge_by_time assemble them where one stream is wanted."""
+        n_interp_frames), and with return_labels (needs label_signal_noise=True) the labels of those rows after them.
+        Union over ranks = the events of the clip; parallel.gather_event_streams / merge_by_time assemble them where
+        one stream is wanted."""
         import torch.distributed as dist
         from . import parallel
+        from .slomo import clip_times
         world, rank = dist.get_world_size(group), dist.get_rank(group)
-        if self.emulator.shard is None:
+        em = self.emulator
+        if em.shard is None:
             raise RuntimeError("run_clip_sharded needs EventEmulator(shard=(rank, world, group))")
+        if return_labels and not em.label_signal_noise:
+            raise ValueError("return_labels=True needs label_signal_noise=True")
         if isinstance(frames_u8, np.ndarray):
             frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
         n, H, W = frames_u8.shape
         if n - 1 < world:
             raise ValueError("fewer frame pairs than ranks")
         if self.slomo.auto_upsample:
-            raise NotImplementedError("auto_upsample picks U per batch (slomo.py:366-372); a sharded clip "
-                                      "needs one U for the time axis: pass upsampling_factor")
-        p0, p1 = parallel.pair_range(n - 1, rank, world)
-        local, times_l, _ = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1])
-        U = int(self.slomo.upsampling_factor)
-        times = np.arange((n - 1) * U) * (1.0 / U)                       # slomo.py:391-395 for the whole clip
-        assert np.allclose(times_l + p0, times[p0 * U:p1 * U])
-        bands = parallel.exchange_frame_bands(local, H, group=group, halo=self.emulator.cs_halo_rows(H))
+            bs = max(1, min(int(self.slomo.batch_size), n - 1))
+            p0, p1 = parallel.batch_pair_range(n - 1, bs, rank, world)
+            local, _, _, ups_l = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1], return_ups=True)
+            # every rank's per-batch U's (a few ints; each rank knows how many batches every rank holds)
+            nb = [-(-(b - a) // bs) for a, b in (parallel.batch_pair_range(n - 1, bs, r, world) for r in range(world))]
+            send = torch.zeros(max(nb), dtype=torch.int64, device=local.device)
+            send[:len(ups_l)] = torch.tensor(ups_l, dtype=torch.int64)
+            recv = [torch.empty_like(send) for _ in range(world)]
+            dist.all_gather(recv, send, group=group)
+            ups = [u for r in range(world) for u in recv[r][:nb[r]].tolist()]
+            times, _ = clip_times(ups, n - 1, bs)
+        else:
+            p0, p1 = parallel.pair_range(n - 1, rank, world)
+            local, times_l, _ = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1])
+            U = int(self.slomo.upsampling_factor)
+            times = np.arange((n - 1) * U) * (1.0 / U)                       # slomo.py:391-395 for the whole clip
+            assert np.allclose(times_l + p0, times[p0 * U:p1 * U])
+        bands = parallel.exchange_frame_bands(local, H, group=group, halo=em.cs_halo_rows(H))
         f = src_duration_s / (np.max(times) - np.min(times))            # v2e.py:794-797
         t = t_offset + f * times
-        if self.emulator.rng_mode == "device" or not (self.emulator.leak_rate_hz > 0 or self.emulator.shot_noise_rate_hz > 0):
+        extra = dict(return_labels=True) if return_labels else {}
+        if em.rng_mode == "device" or not (em.leak_rate_hz > 0 or em.shot_noise_rate_hz > 0 or em.photoreceptor_noise):
             # chunks of frames through the multi-frame kernels: one all-reduce(MAX) of the frame maxima per chunk
-            # (frame by frame -- one all-reduce each -- for a chunk the refractory filter touches, and for the
-            # centre-surround model, whose Euler iteration exchanges halo rows)
-            rows, _ = self.emulator.generate_events_band_batch(bands, t, H)
-            return rows, t, bands.shape[0]
-        out = []
+            # (frame by frame -- one all-reduce each -- for a chunk the refractory filter touches, for the
+            # centre-surround model, whose Euler iteration exchanges halo rows, and for SCIDVS / photoreceptor noise)
+            res = em.generate_events_band_batch(bands, t, H, **extra)
+            return (res[0], t, bands.shape[0]) + tuple(res[2:])
+        out, labs = [], []
         for k in range(bands.shape[0]):
-            ev = self.emulator.generate_events_band(bands[k], t[k], H)
+            ev = em.generate_events_band(bands[k], t[k], H)
             if ev is not None:
                 out.append(ev)
+                labs.append(em.last_signnoise_label)
         rows = np.concatenate(out, 0) if out else np.zeros((0, 4), np.float32)
+        if return_labels:
+            return rows, t, bands.shape[0], (np.concatenate(labs) if labs else np.zeros((0,), bool))
         return rows, t, bands.shape[0]

@@ -47,6 +47,23 @@ def unet_layer_shapes(in_ch, out_ch):
     return s
 
 
+def batch_times(in_ctr, b, U):
+    """interpTimes of one batch of b pairs starting at pair in_ctr, up-sampled U times (slomo.py:391-395)."""
+    return in_ctr + np.array(range(U * b)) * (1 / U)
+
+
+def clip_times(ups, n_pairs, batch_size):
+    """(interpTimes, avgUpsampling) of a clip of n_pairs frame pairs interpolated in batches of batch_size consecutive
+    pairs (the last one short) with U = ups[i] for batch i: what SuperSloMo.interpolate_frames returns for the whole
+    clip, assembled from the per-batch U's alone (a pair-sharded clip gathers them from its ranks)."""
+    bs = max(1, min(int(batch_size), n_pairs))
+    starts = range(0, n_pairs, bs)
+    if len(ups) != len(starts):
+        raise ValueError("%d U's for %d batches" % (len(ups), len(starts)))
+    times = [batch_times(a, min(bs, n_pairs - a), int(U)) for a, U in zip(starts, ups)]
+    return np.concatenate(times), sum(ups) / len(ups)
+
+
 def _weights_struct(state_dict, in_ch, out_ch, keep):
     st = _lib.V2eUNetWeights()
     for i, (name, (co, ci, k)) in enumerate(zip(LAYER_NAMES, unet_layer_shapes(in_ch, out_ch))):
@@ -274,14 +291,15 @@ class SuperSloMo(object):
                 t = (k + 0.5) / U                                       # slomo.py:405
                 # frame of pair bi at step k goes to index U*bi + k of the batch (slomo.py:440): written in place
                 eng.interp(t, blk[k: U * b: U])
-            yield blk, in_ctr + np.array(range(U * b)) * (1 / U), U      # slomo.py:391-395
+            yield blk, batch_times(in_ctr, b, U), U                     # slomo.py:391-395
             in_ctr += b
 
-    def interpolate_frames(self, frames, out=None):
+    def interpolate_frames(self, frames, out=None, return_ups=False):
         """frames: [N, H, W] uint8 (ndarray or tensor, host or device), N >= 2.
-        Returns (out_u8 [M, H, W] device tensor, interpTimes [M] float64, avgUpsampling).
-        Frame order and times follow slomo.py:391-400, 440: output index = counter + U*b + k holds the
-        frame synthesised at t=(k+0.5)/U between source frames b and b+1, labelled with time b + k/U."""
+        Returns (out_u8 [M, H, W] device tensor, interpTimes [M] float64, avgUpsampling), and with return_ups the
+        list of per-batch U's after them. Frame order and times follow slomo.py:391-400, 440: output index =
+        counter + U*b + k holds the frame synthesised at t=(k+0.5)/U between source frames b and b+1, labelled with
+        time b + k/U."""
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(np.ascontiguousarray(frames))
         if frames.dtype != torch.uint8 or frames.dim() != 3:
@@ -301,6 +319,8 @@ class SuperSloMo(object):
         if fixed is None:
             out = torch.cat(chunks, 0)
         self._engine.check_finite()
+        if return_ups:
+            return out, np.concatenate(times), sum(ups) / len(ups), ups
         return out, np.concatenate(times), sum(ups) / len(ups)
 
     # -- reference file API ----------------------------------------------------------------------
