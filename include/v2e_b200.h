@@ -375,7 +375,10 @@ int v2e_slomo_interp(V2eSlomo *h, double t, uint8_t *out_u8_dev, float *out_f32_
 int v2e_slomo_check_finite(V2eSlomo *h, int *nonfinite_host, void *stream);
 /* option 0: force the per-tap convolution kernel for every layer; option 1: do not fold the up-sampling into
  * up5.conv1; option 2: do not fuse the average pools into the epilogues of conv2 / down1.conv2 (A/B measurements
- * and bit-identity tests: the fused pool must equal the separate kernel exactly), value 0/1 */
+ * and bit-identity tests: the fused pool must equal the separate kernel exactly), value 0/1;
+ * option 3: plan every later launch (per-tap tile pick, strip and up-sampling grids and their segmentation) as if
+ * the device had `value` SMs, 1 <= value <= the device's count; 0 restores the device's count (the default). A test
+ * hook: the outputs must not depend on it. Other values: V2E_E_INVALID. */
 int v2e_slomo_set_option(V2eSlomo *h, int option, int value);
 /* Measurement hooks: bracket every convolution launch with CUDA events; profile_read synchronises
  * and returns the summed device time, the number of launches and their algorithmic FLOPs

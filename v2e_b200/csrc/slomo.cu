@@ -377,6 +377,7 @@ struct V2eSlomo {
     int curB;
     std::vector<char> launch_mem, row_mem, up_mem;
     int n_sms, force_tap_kernel, no_fused_up, no_fused_pool;
+    int dev_sms;                  // the device's SM count; n_sms plans the launches (option 3 lowers it)
     int8_t ran[2][23];            // [flow, interp][layer]: V2E_SLOMO_KERNEL_* of the last launch (test hook)
     // measurement hooks: CUDA events around every conv launch
     int profile;
@@ -482,6 +483,7 @@ extern "C" int v2e_slomo_create(int H, int W, int max_batch, const V2eUNetWeight
     h->launch_mem.resize(v2e_conv_launch_size());
     h->row_mem.resize(v2e_strip_launch_size());
     { int dev = 0; cudaGetDevice(&dev); h->n_sms = 132; cudaDeviceGetAttribute(&h->n_sms, cudaDevAttrMultiProcessorCount, dev); }
+    h->dev_sms = h->n_sms;
     h->force_tap_kernel = 0;
     h->no_fused_up = getenv("V2E_NO_FUSED_UP") ? 1 : 0;        // A/B measurements
     h->no_fused_pool = getenv("V2E_NO_FUSED_POOL") ? 1 : 0;
@@ -676,6 +678,12 @@ extern "C" int v2e_slomo_set_option(V2eSlomo *h, int option, int value) {
     if (option == 0) { h->force_tap_kernel = value; return V2E_OK; }
     if (option == 1) { h->no_fused_up = value; return V2E_OK; }
     if (option == 2) { h->no_fused_pool = value; return V2E_OK; }
+    if (option == 3) {
+        // plan as if the device had `value` SMs; never more than it has, so a persistent grid cannot oversubscribe it
+        if (value < 0 || value > h->dev_sms) return v2e_set_error(V2E_E_INVALID, "SM count out of range%s", "");
+        h->n_sms = value ? value : h->dev_sms;
+        return V2E_OK;
+    }
     return v2e_set_error(V2E_E_INVALID, "unknown option%s", "");
 }
 
