@@ -133,8 +133,16 @@ int v2e_emu_first_frame(V2eEmu *h, const void *frame_dev, int frame_dtype, doubl
  * frame at a time with the phase functions below.
  * events_out_dev: [capacity][4] float32 rows [t, x, y, p] (emulator.py:1020); rows of frame f
  * start at info[f].ev_base; ev_base_start is the row at which this step starts writing.
- * Rows within one (iteration, polarity) group are in no particular order (the reference shuffles
- * them, emulator.py:866-870); groups are iteration-major, ON before OFF, shot noise last.
+ * Groups are iteration-major, ON before OFF, shot noise (ON, then OFF) last. The order of the rows inside a group
+ * is set by option 2 of v2e_emu_set_option:
+ *   0 (default): as emitted -- it can differ from run to run;
+ *   1 canonical: by pixel index y * width + x ascending, the reference's order before its randperm
+ *     (emulator.py:861-870, 1024-1059);
+ *   2 shuffled: the ON and OFF rows of one (frame, iteration) are mixed, in ascending order of a 64-bit key that is
+ *     uniform and a pure function of (seed, Philox frame index, iteration, pixel, polarity) -- what the reference's
+ *     randperm does (emulator.py:866-870), though not its permutation; shot-noise rows stay canonical and last.
+ * With 1 or 2 the rows are identical from run to run and whatever kernels, chunk sizes, replays or capacity resumes
+ * produced them; v2e_emu_collect enqueues the ordering on `stream` once every frame of the step is emitted.
  * Enqueues everything on `stream`, no host synchronisation.
  * If the buffer is too small at frame f, that frame's emission and everything after it is
  * skipped on the device (sticky abort), state is left as "frame f counted, not emitted";
@@ -155,8 +163,19 @@ int v2e_emu_step(V2eEmu *h, const void *frames_dev, int frame_dtype, int T,
  * frame before it returns. option 0 of v2e_emu_set_option: 0 = never take the fast path (A/B tests), 1 = default.
  * option 1: 1 = the photoreceptor-noise Philox counters (rng_mode 1) use rng_pixel_offset + pixel like the leak and
  * shot counters, so that a row band of a pixel-sharded clip draws what one GPU draws; 0 = the handle's own pixel index
- * (default). */
+ * (default).
+ * option 2: row order inside a group, see v2e_emu_step: 0 = as emitted (default; nothing is launched or allocated for
+ * ordering), 1 = canonical, 2 = shuffled (rng_mode 1 only). The shuffled key of a row is the first two words, high
+ * word first, of Philox4x32-7 with the seed as key and the counter (2 * pixel + (p < 0), Philox frame index, iteration,
+ * 0x726f7264 "rord"), pixel = rng_pixel_offset + y * width + x; equal keys are ordered by 2 * pixel + (p < 0). A row
+ * band of a pixel-sharded clip therefore sorts by the whole frame's keys: its rows are a subsequence of the one-GPU
+ * order. The canonical key is (p < 0) << 32 | pixel. */
 int v2e_emu_set_option(V2eEmu *h, int option, int value);
+/* Row order 1 or 2: keys_dev (nullable; uint64, one entry per row of events_out_dev, indexed like it) receives the key
+ * of every row v2e_emu_collect orders from now on. */
+int v2e_emu_set_key_buffer(V2eEmu *h, uint64_t *keys_dev);
+/* Device memory held for ordering (0 until a step has been ordered) and rows ordered so far. */
+int v2e_emu_order_stats(V2eEmu *h, uint64_t *scratch_bytes, long long *rows_ordered);
 /* The fast path in two halves for a pixel-sharded clip (SURVEY.md 8e): v2e_emu_fused_count enqueues the register-
  * resident update of the T frames and the per-frame counts; the caller all-reduces (MAX) the T int32 at
  * v2e_emu_max_vec_dev() over the ranks on the same stream; v2e_emu_fused_emit plans with the reduced maxima, emits and
@@ -184,7 +203,8 @@ int v2e_emu_time_fused(V2eEmu *h, const void *frames_dev, int frame_dtype, int T
 
 /* Copies the per-frame control blocks of the last step to the host. Synchronises `stream`.
  * info_host[T]. *frames_done = number of frames fully emitted. Returns V2E_OK,
- * V2E_E_CAPACITY or V2E_E_ITER_CAP. */
+ * V2E_E_CAPACITY or V2E_E_ITER_CAP. With a row order set (option 2) and V2E_OK, the kernels that order the step's rows
+ * in place are enqueued on `stream` after the synchronisation: work enqueued later on that stream sees ordered rows. */
 int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info_host, int T, int *frames_done,
                     uint64_t *rows_total, void *stream);
 

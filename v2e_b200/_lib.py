@@ -52,6 +52,8 @@ _SIGS = {
     "v2e_version": (_i, []),
     "v2e_abi_info": (_i, [ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     "v2e_emu_set_option": (_i, [_vp, _i, _i]),
+    "v2e_emu_set_key_buffer": (_i, [_vp, _vp]),
+    "v2e_emu_order_stats": (_i, [_vp, ctypes.POINTER(_u64), ctypes.POINTER(ctypes.c_longlong)]),
     "v2e_emu_fused_count": (_i, [_vp, _vp, _i, _i, _vp, _d, _vp]),
     "v2e_emu_max_vec_dev": (_vp, [_vp]),
     "v2e_emu_fused_emit": (_i, [_vp, _vp, _u64, _u64, _vp]),

@@ -1909,6 +1909,8 @@ __global__ void __launch_bounds__(kThreads) emu_draw_noise_kernel(EmuDev d, uint
     }
 }
 
+#include "order.cuh"        // row order: the segmented sort v2e_emu_collect runs when option 2 asks for one
+
 }  // namespace
 
 // =============================================================================================
@@ -1969,6 +1971,19 @@ struct V2eEmu {
     FrameParams cs_p;
     int cs_pending;             // v2e_emu_cs_begin ran, v2e_emu_cs_update not yet
     long long n_cs_coop, n_cs_step;   // Euler iterations (frames, or chunks when sharded) run cooperatively / per step
+    // row order (v2e_emu_set_option option 2; order.cuh): nothing here is allocated until a step is ordered
+    struct {
+        int mode;                   // 0 = none, 1 = canonical, 2 = shuffled
+        float *events;              // where the last emission wrote (the buffer v2e_emu_collect orders)
+        uint64_t *keys_out;         // v2e_emu_set_key_buffer: receives every ordered row's key, indexed like events
+        uint32_t *frame_index;      // [max_slots] host: Philox frame index of every slot of the last step
+        float4 *rows; uint64_t *keys; size_t rows_cap, keys_cap;      // scatter targets
+        uint32_t *boff; size_t nb_cap;                      // bucket counters / offsets
+        OrdSeg *segs; size_t seg_cap;
+        uint32_t *ctl;              // [max_slots] frame indices, [max_slots + 1] first segment of each frame, [2] header
+        size_t bytes;               // device memory held for ordering
+        long long rows_done;        // rows ordered so far
+    } ord;
 };
 
 thread_local char g_err[512] = "";
@@ -2083,6 +2098,7 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
     h->fused_enable = 1;
     h->ls.t_frames = new double[cfg->max_frames_per_step]();
     h->sched = new V2eEmu::Seg[(size_t)cfg->max_frames_per_step + 2]();
+    h->ord.frame_index = new uint32_t[cfg->max_frames_per_step]();
     d.px_off = cfg->rng_pixel_offset;
     d.units = (d.n + kUnitPx - 1) / kUnitPx;
     // state arrays are staged in whole 128-pixel units by the update kernel's bulk copies
@@ -2184,6 +2200,9 @@ extern "C" int v2e_emu_destroy(V2eEmu *h) {
     delete[] h->pr_vrms;
     delete[] h->ls.t_frames;
     delete[] h->sched;
+    delete[] h->ord.frame_index;
+    void *ord_ptrs[] = {h->ord.rows, h->ord.keys, h->ord.boff, h->ord.segs, h->ord.ctl};
+    for (void *p : ord_ptrs) if (p) cudaFree(p);
     void *cs_ptrs[] = {d.cs_bufs, d.cs_done, h->cs_send};
     for (void *p : cs_ptrs) if (p) cudaFree(p);
     void *fused_ptrs[] = {h->lp_alt, h->base_alt, h->rec_list, h->rec_cnt, h->blk_cnt, h->ff_dev, h->fp_dev, h->max_vec};
@@ -2491,6 +2510,7 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
 
 static int enqueue_emit(V2eEmu *h, const FrameParams &p, int slot, float *events, cudaStream_t st) {
     const EmuDev &d = h->d;
+    h->ord.events = events;
     ProfScope ps(h, slot, 2, st);
     if (d.state_f64) emu_emit_kernel<double><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
     else emu_emit_kernel<float><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
@@ -2615,6 +2635,7 @@ static int fused_upload_params(V2eEmu *h, int T, const double *t_frames, double 
         const double tp = f == 0 ? t_previous : t_frames[f - 1];
         if (t_frames[f] < tp) return fail(V2E_E_INVALID, "frame times must be non-decreasing");
         fph[f] = make_params(h, t_frames[f], tp, frame_base + (uint32_t)f, capacity);
+        h->ord.frame_index[f] = frame_base + (uint32_t)f;
         memset(&ffh[f], 0, sizeof(FusedFrame));
         ffh[f].eps_scale = fph[f].eps_scale;
         ffh[f].shot_c = fph[f].shot_c;
@@ -2660,6 +2681,7 @@ static int enqueue_fused_count(V2eEmu *h, const void *frames, int T, cudaStream_
 static int enqueue_fused_emit(V2eEmu *h, int T, float *events, uint64_t capacity, uint64_t ev_base_start,
                               const int32_t *max_vec, bool commit, cudaStream_t st, int a = 0, int chain = 0) {
     const EmuDev d = shifted_dev(h->d, a);
+    h->ord.events = events;
     {
         ProfScope ps(h, 1, 1, st);       // slot 1: v2e_emu_profile_read4 sums count + plan under "filter"
         emu_fused_plan_kernel<<<1, kThreads, (size_t)T * sizeof(uint32_t), st>>>(d, h->fp_dev + a, T, ev_base_start, capacity,
@@ -2721,6 +2743,12 @@ extern "C" int v2e_emu_set_option(V2eEmu *h, int option, int value) {
     if (!h) return fail(V2E_E_INVALID, "null handle");
     if (option == 0) { h->fused_enable = value ? 1 : 0; return V2E_OK; }
     if (option == 1) { h->d.pr_off = value ? h->d.px_off : 0u; return V2E_OK; }
+    if (option == 2) {
+        if (value < 0 || value > 2) return fail(V2E_E_INVALID, "row order must be 0, 1 or 2");
+        if (value == 2 && h->d.rng_mode != 1) return fail(V2E_E_INVALID, "the shuffled row order needs rng_mode 1");
+        h->ord.mode = value;
+        return V2E_OK;
+    }
     return fail(V2E_E_INVALID, "unknown option");
 }
 extern "C" int v2e_emu_fused_stats(V2eEmu *h, long long *chunks, long long *rejected) {
@@ -2833,6 +2861,7 @@ static int step_classic(V2eEmu *h, const void *frames, int dtype, int T, const d
         double tp = f == 0 ? t_previous : t_frames[f - 1];
         if (t_frames[f] < tp) return fail(V2E_E_INVALID, "frame times must be non-decreasing");
         FrameParams p = make_params(h, t_frames[f], tp, h->step_base + (uint32_t)f, capacity);
+        h->ord.frame_index[f] = h->step_base + (uint32_t)f;
         const char *frame = (const char *)frames + (size_t)f * fbytes;
         const float *lr = leak_randn ? leak_randn + (size_t)f * d.n : nullptr;
         const float *sr = shot_rand ? shot_rand + (size_t)f * d.n : nullptr;
@@ -2916,6 +2945,66 @@ extern "C" int v2e_emu_step(V2eEmu *h, const void *frames, int dtype, int T, con
     h->last_fused = 0;
     return step_classic(h, frames, dtype, T, t_frames, t_previous, leak_randn, shot_rand, events, capacity,
                         ev_base_start, first, resume_emit, stream);
+}
+
+// Orders the rows of the finished step (all T frames emitted, control blocks in ctrl_host) where they lie. Enqueue only.
+static int order_step(V2eEmu *h, int T, cudaStream_t st) {
+    auto &o = h->ord;
+    const EmuDev &d = h->d;
+    const uint64_t row0 = h->ctrl_host[0].ev_base;
+    const uint64_t n_rows = h->ctrl_host[T - 1].ev_base + h->ctrl_host[T - 1].n_events - row0;
+    if (n_rows == 0) return V2E_OK;
+    if (n_rows >= (1ull << 32)) return fail(V2E_E_UNSUPPORTED, "row order: more than 2^32 rows in one step");
+    if (!o.events) return fail(V2E_E_STATE, "row order: no emission precedes v2e_emu_collect");
+    size_t n_seg = 0;
+    for (int f = 0; f < T; f++) n_seg += 2 * (size_t)h->ctrl_host[f].max_n + 2;
+    const size_t n_buckets = (size_t)(n_rows / 32) + n_seg + 8;
+    auto grow = [&](void **p, size_t *cap, size_t need, size_t elem) -> bool {
+        if (*cap >= need) return true;
+        if (*p) { cudaFree(*p); o.bytes -= *cap * elem; *p = nullptr; *cap = 0; }
+        const size_t c = need + need / 2;
+        if (cudaMalloc(p, c * elem) != cudaSuccess) return false;
+        *cap = c;
+        o.bytes += c * elem;
+        return true;
+    };
+    if (!grow((void **)&o.rows, &o.rows_cap, (size_t)n_rows, sizeof(float4)) ||
+        !grow((void **)&o.keys, &o.keys_cap, (size_t)n_rows, sizeof(uint64_t)) ||
+        !grow((void **)&o.boff, &o.nb_cap, n_buckets, 4) || !grow((void **)&o.segs, &o.seg_cap, n_seg, sizeof(OrdSeg)))
+        return fail(V2E_E_CUDA, "row order: cudaMalloc: %s", cudaGetErrorString(cudaGetLastError()));
+    const size_t slots = (size_t)d.max_slots;
+    if (!o.ctl) {
+        CU(cudaMalloc((void **)&o.ctl, (2 * slots + 3) * 4));
+        o.bytes += (2 * slots + 3) * 4;
+    }
+    uint32_t *fidx = o.ctl, *seg0 = o.ctl + slots, *hdr = o.ctl + 2 * slots + 1;
+    // pageable source: staged before the call returns
+    CU(cudaMemcpyAsync(fidx, o.frame_index, (size_t)T * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(o.boff, 0, n_buckets * 4, st));
+    float4 *rows = (float4 *)o.events + row0;
+    const uint32_t n = (uint32_t)n_rows, grid = (n + 255u) / 256u;
+    order_setup_kernel<<<1, 1024, 0, st>>>(d, T, o.mode, fidx, seg0, o.segs, hdr);
+    order_count_kernel<<<grid, 256, 0, st>>>(d, rows, n, o.segs, hdr, o.boff);
+    order_scan_kernel<<<1, 1024, 0, st>>>(hdr, o.boff);
+    order_scatter_kernel<<<grid, 256, 0, st>>>(d, rows, n, o.segs, hdr, o.boff, o.rows, o.keys);
+    const size_t sort_grid = n_buckets < 132 * 16 ? n_buckets : 132 * 16;
+    order_sort_kernel<<<(unsigned)sort_grid, kOrdThreads, 0, st>>>(d, hdr, o.boff, o.rows, o.keys, rows,
+                                                                   o.keys_out ? o.keys_out + row0 : nullptr);
+    CU(cudaGetLastError());
+    o.rows_done += (long long)n_rows;
+    return V2E_OK;
+}
+
+extern "C" int v2e_emu_set_key_buffer(V2eEmu *h, uint64_t *keys_dev) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    h->ord.keys_out = keys_dev;
+    return V2E_OK;
+}
+extern "C" int v2e_emu_order_stats(V2eEmu *h, uint64_t *scratch_bytes, long long *rows_ordered) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    if (scratch_bytes) *scratch_bytes = (uint64_t)h->ord.bytes;
+    if (rows_ordered) *rows_ordered = h->ord.rows_done;
+    return V2E_OK;
 }
 
 extern "C" int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info, int T, int *frames_done,
@@ -3014,6 +3103,7 @@ extern "C" int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info, int T, int *frames
     if (rows_total) *rows_total = rows;
     if (status == V2E_E_CAPACITY) return fail(V2E_E_CAPACITY, "event buffer too small");
     if (status == V2E_E_ITER_CAP) return fail(V2E_E_ITER_CAP, "a pixel exceeded iter_cap events in one frame");
+    if (h->ord.mode) return order_step(h, T, st);
     return V2E_OK;
 }
 
@@ -3072,6 +3162,7 @@ extern "C" int v2e_emu_phase_count(V2eEmu *h, const void *frame, int dtype, doub
     if ((rc = reset_slots(h, 0, 1, st))) return rc;
     emu_begin_step_kernel<<<1, 1, 0, st>>>(h->d, 0, ev_base_start);
     FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
+    h->ord.frame_index[0] = p.frame_index;
     h->last_dt = p.dt;
     const float *prn = nullptr;
     if ((rc = take_pr_noise(h, p, &prn, "v2e_emu_phase_count"))) return rc;
@@ -3094,6 +3185,7 @@ extern "C" int v2e_emu_phase_update(V2eEmu *h, const void *frame, int dtype, dou
     if ((rc = reset_slots(h, 0, 1, st))) return rc;
     emu_begin_step_kernel<<<1, 1, 0, st>>>(h->d, 0, ev_base_start);
     FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
+    h->ord.frame_index[0] = p.frame_index;
     h->last_dt = p.dt;
     // shot_pending = 1 makes enqueue_count run the update kernel alone when there is no refractory
     // period; with one, the filter must wait for the reduced max, so launch the update kernel directly
@@ -3132,6 +3224,7 @@ extern "C" int v2e_emu_cs_begin(V2eEmu *h, const void *frame, int dtype, double 
     if ((rc = reset_slots(h, 0, 1, st))) return rc;
     emu_begin_step_kernel<<<1, 1, 0, st>>>(d, 0, ev_base_start);
     FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
+    h->ord.frame_index[0] = p.frame_index;
     h->last_dt = p.dt;
     if ((rc = cs_plan(h, p, &h->cs_num_steps, &h->cs_alpha_p, &h->cs_alpha_h))) return rc;
     if ((rc = launch_lp(d, p, frame, dtype, st))) return rc;

@@ -15,7 +15,16 @@ Two RNG modes:
       per-frame noise is enabled, statistically equivalent otherwise.
 
 Extra keywords (not in the reference): rng_mode, rng (draw source object), iter_cap,
-max_frames_per_step, exact_order, shard, fused.
+max_frames_per_step, exact_order, shard, fused, row_order.
+
+Row order in device mode. The kernels put a row inside its (frame, iteration, polarity) group wherever an atomicAdd
+placed it, so with row_order=None (default) the order inside a group can change from run to run. row_order="canonical"
+orders every frame like the reference before its randperm (iteration-major; ON rows then OFF rows by pixel index
+y*W + x; then shot ON, shot OFF by pixel); row_order="shuffled" mixes the ON and OFF rows of each (frame, iteration) in
+a pseudo-random order, uniform over permutations, as the reference's randperm leaves them (emulator.py:861-870), shot
+rows canonical and last. Both are sorted on the device by a key that is a function of the row alone (DESIGN.md 4.1):
+the bytes do not depend on fused / max_frames_per_step / replayed chunks / buffer growth, and a row band of a sharded
+clip is a subsequence of the one-GPU stream (v2e_b200.parallel.merge_by_key puts the bands back together).
 
 Sink keywords (dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text; emulator.py:325-357): the files are opened by the
 reference's own writer classes (v2ecore.output.*, h5py) when those import, and fed the way the reference feeds
@@ -219,6 +228,7 @@ class EventEmulator(object):
             exact_order: bool = True,
             shard=None,
             fused: bool = True,
+            row_order: str = None,
     ):
         if not str(device).startswith("cuda"):
             raise RuntimeError("v2e_b200.EventEmulator runs on a CUDA device only (device=%r); "
@@ -241,6 +251,10 @@ class EventEmulator(object):
                            "available by the same attribute names")
         if rng_mode not in ("replay", "device"):
             raise ValueError("rng_mode must be 'replay' or 'device'")
+        if row_order not in (None, "canonical", "shuffled"):
+            raise ValueError("row_order must be None, 'canonical' or 'shuffled'")
+        if row_order is not None and rng_mode == "replay":
+            raise ValueError("row_order needs rng_mode='device' (replay mode returns the reference's own order)")
         logger.info("ON/OFF log_e temporal contrast thresholds: {} / {} +/- {}".format(
             pos_thres, neg_thres, sigma_thres))
         self.device = torch.device(device if device != "cuda" else "cuda:0")
@@ -289,6 +303,9 @@ class EventEmulator(object):
             np.random.seed(seed)
             random.seed(seed)
         self.fused = bool(fused)
+        self.row_order = row_order
+        self._want_keys = False      # generate_events_band_batch(return_keys=True) is running
+        self._keys_dev = self._last_keys = self.last_n_shot = None
         self.cs_chunk_steps = 64     # pixel-sharded centre-surround model: Euler steps per halo exchange
         self._lib = _lib.load()
         self._hbox = [None]          # the library handle, shared with the finalizer
@@ -432,6 +449,8 @@ class EventEmulator(object):
             if self.shard is not None:
                 # a row band's photoreceptor-noise draws count whole-frame pixels, like its leak / shot draws
                 _lib.check(self._lib.v2e_emu_set_option(h, 1, 1))
+            if self.row_order is not None:
+                _lib.check(self._lib.v2e_emu_set_option(h, 2, 1 if self.row_order == "canonical" else 2))
             lut = _linlog_lut()
             _lib.check(self._lib.v2e_emu_set_linlog_lut(h, ctypes.c_void_p(lut.data_ptr()), self._stream()))
         self._H, self._W = H, W
@@ -449,6 +468,18 @@ class EventEmulator(object):
         self._ev_dev = torch.empty((max(int(rows), 16), 4), dtype=torch.float32, device=self.device)
         if keep:
             self._ev_dev[:keep].copy_(old[:keep])
+
+    def _bind_keys(self):
+        """row_order set: tells the library where to leave the sort key of every row it orders (one uint64 per row of
+        the event buffer) while generate_events_band_batch(return_keys=True) runs, nowhere otherwise."""
+        if self.row_order is None:
+            return
+        ptr = None
+        if self._want_keys:
+            if self._keys_dev is None or self._keys_dev.shape[0] < self._ev_dev.shape[0]:
+                self._keys_dev = torch.empty(self._ev_dev.shape[0], dtype=torch.int64, device=self.device)
+            ptr = ctypes.c_void_p(self._keys_dev.data_ptr())
+        _lib.check(self._lib.v2e_emu_set_key_buffer(self._h, ptr))
 
     def _rows_to_host(self, n_rows, base=0, copy=True):
         """Device rows -> host ndarray through a pinned staging buffer. copy=False returns a view of that
@@ -609,7 +640,8 @@ class EventEmulator(object):
         frame-global maximum (emulator.py:773-775) is all-reduced (MAX) between the update and the refractory filter.
         Returns the rows (y of the whole frame) in the canonical order -- unsharded with exact_order, the reference's
         own order -- on the host, or on the device with return_device, where device-RNG rows keep the kernels' order.
-        None when there are none."""
+        With row_order set the library has ordered the rows and they are returned as they are. None when there are
+        none."""
         import torch.distributed as dist
         sharded, replay = self.shard is not None, self.rng_mode == "replay"
         group = self.shard[2] if sharded else None
@@ -632,6 +664,7 @@ class EventEmulator(object):
                 _lib.check(L.v2e_emu_set_pr_noise(h, p(pr_dev), vr, 1))
             lr_dev = field(self.rng.randn) if replay and self.leak_rate_hz > 0 else None
             self._grow_event_buffer(self.event_rows_hint or max(4 * self._H * W, 1 << 16))
+            self._bind_keys()
             cap = self._ev_dev.shape[0]
             fp = ctypes.c_void_p(fr.data_ptr())
             if not sharded:
@@ -646,7 +679,7 @@ class EventEmulator(object):
                 dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=group)
                 _lib.check(L.v2e_emu_phase_filter(h, t_frame, tp, cap, 0 if shot_pending else 1, st))
             counts = perms = None
-            if replay or not return_device:
+            if replay or not (return_device or self.row_order is not None):
                 # per-(iteration, polarity) counts on the host (one synchronisation): the replayed randperm draws and
                 # the canonical row order need them
                 max_n = ctypes.c_int32(0)
@@ -673,7 +706,8 @@ class EventEmulator(object):
             fi = self._collect_one(fp, code, t_frame, tp, st)
             self.last_frame_info = fi
             n_ev = int(fi.n_events)
-            ev = self._ev_dev[:n_ev].clone() if counts is None else self._rows_to_host(n_ev)
+            ev = self._ev_dev[:n_ev].clone() if counts is None and return_device else self._rows_to_host(n_ev)
+            self._last_keys = self._keys_dev[:n_ev].clone() if self._want_keys else None
         self._account(fi)
         if n_ev == 0:
             return None
@@ -694,6 +728,7 @@ class EventEmulator(object):
         rc = L.v2e_emu_collect(h, info, 1, ctypes.byref(done), ctypes.byref(rows), st)
         if rc == _lib.V2E_E_CAPACITY:
             self._grow_event_buffer(int(info[0].n_events) + 1024)
+            self._bind_keys()
             ts = (ctypes.c_double * 1)(t_frame)
             _lib.check(L.v2e_emu_step(h, fp, code, 1, ts, tp, None, None,
                                       ctypes.c_void_p(self._ev_dev.data_ptr()), self._ev_dev.shape[0], 0,
@@ -794,7 +829,8 @@ class EventEmulator(object):
             _lib.check(L.v2e_emu_cs_advance(h, s0, s1, st))
         _lib.check(L.v2e_emu_cs_update(h, fp, code, lrp, None, st))
 
-    def generate_events_band_batch(self, band_frames, t_frames, full_height, return_device=False, return_labels=False):
+    def generate_events_band_batch(self, band_frames, t_frames, full_height, return_device=False, return_labels=False,
+                                   return_keys=False):
         """Pixel-sharded, batched (BASELINE config 5 without per-frame host work): band_frames [T, y1-y0, W] uint8,
         this rank's rows of T consecutive frames. The multi-frame kernels run the whole chunk with per-pixel state in
         registers; the only exchange is ONE all-reduce(MAX) of the T frame maxima (SURVEY.md 8e "batch as a [T]
@@ -802,15 +838,28 @@ class EventEmulator(object):
         frame), identically on every rank; so is every chunk with SCIDVS or photoreceptor noise, which the multi-frame
         kernels do not take. Needs rng_mode='device' when leak / shot / photoreceptor noise is on.
         Returns (rows [N,4] float32 with global y, offsets [T+1]) like generate_events_batch; return_labels=True (needs
-        label_signal_noise=True) adds the band's labels like generate_events_batch(..., return_labels=True)."""
-        import torch.distributed as dist
+        label_signal_noise=True) adds the band's labels like generate_events_batch(..., return_labels=True).
+        return_keys=True (needs row_order) adds, last, the uint64 sort key of every row, computed by the library while
+        it ordered the rows (a uint64 ndarray; with return_device a CUDA int64 tensor holding the same bits): what
+        v2e_b200.parallel.merge_by_key needs, with `last_n_shot` (the shot-noise rows that end each frame of this call),
+        to put the bands of all ranks into the one-GPU order."""
         if self.shard is None:
             raise RuntimeError("generate_events_band_batch needs shard=(rank, world, group)")
         if return_labels and not self.label_signal_noise:
             raise ValueError("return_labels=True needs label_signal_noise=True")
+        if return_keys and self.row_order is None:
+            raise ValueError("return_keys=True needs row_order='canonical' or 'shuffled'")
         if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
                                           self.photoreceptor_noise):
             raise RuntimeError("batched sharded operation with per-frame noise needs rng_mode='device'")
+        self._want_keys = bool(return_keys)
+        try:
+            return self._band_batch(band_frames, t_frames, full_height, return_device, return_labels, return_keys)
+        finally:
+            self._want_keys = False
+
+    def _band_batch(self, band_frames, t_frames, full_height, return_device, return_labels, return_keys):
+        import torch.distributed as dist
         rank, world, group = self.shard
         fr, code = self._to_device_frames(band_frames)
         H = int(full_height)
@@ -820,7 +869,7 @@ class EventEmulator(object):
         T = fr.shape[0]
         t_frames = self._frame_times(t_frames, T)
         L = self._lib
-        out, offs, n_shot = [], [0], []
+        out, offs, n_shot, keys = [], [0], [], []
         state = {"total": 0}
         n = (y1 - y0) * fr.shape[2]
 
@@ -833,6 +882,7 @@ class EventEmulator(object):
             with torch.cuda.device(self.device):
                 st = self._stream()
                 self._grow_event_buffer(self.event_rows_hint or max(2 * n, 1 << 16))
+                self._bind_keys()
                 rc = L.v2e_emu_fused_count(self._h, ctypes.c_void_p(chunk.data_ptr()), code, Tc, ts,
                                            float(self.t_previous), st)
                 if rc == _lib.V2E_E_UNSUPPORTED:
@@ -851,6 +901,7 @@ class EventEmulator(object):
                         break
                     need = max(int(info[k].ev_base) + int(info[k].n_events) for k in range(Tc))
                     self._grow_event_buffer(2 * need)
+                    self._bind_keys()
                 if rc == _lib.V2E_E_FALLBACK:
                     return int(done.value)
                 _lib.check(rc)
@@ -862,6 +913,8 @@ class EventEmulator(object):
                 ev = self._ev_dev[:nrows].clone()
                 ev[:, 2] += y0
                 out.append(ev)
+                if return_keys:
+                    keys.append(self._keys_dev[:nrows].clone())
                 state["total"] += nrows
                 self.last_frame_info = info[Tc - 1]
                 self.t_previous = t_frames[b - 1]
@@ -875,6 +928,8 @@ class EventEmulator(object):
                 fi = self.last_frame_info
                 if evk is not None:
                     out.append(evk)
+                    if return_keys:
+                        keys.append(self._last_keys)
                     state["total"] += len(evk)
                 offs.append(state["total"])
                 n_shot.append(0 if evk is None else int(fi.n_shot_on) + int(fi.n_shot_off))
@@ -897,6 +952,7 @@ class EventEmulator(object):
                 frame_by_frame(g, e)
             f = e
         offs = np.asarray(offs, np.int64)
+        self.last_n_shot = np.asarray(n_shot, np.int64)      # shot-noise rows that end each frame of this call
         rows = torch.cat(out, 0) if out else torch.zeros((0, 4), dtype=torch.float32, device=self.device)
         labels = None
         if return_labels:
@@ -906,7 +962,11 @@ class EventEmulator(object):
                 labels = labels.cpu().numpy().astype(bool)
         if not return_device:
             rows = rows.cpu().numpy()
-        return (rows, offs, labels) if return_labels else (rows, offs)
+        res = (rows, offs, labels) if return_labels else (rows, offs)
+        if return_keys:
+            k = torch.cat(keys, 0) if keys else torch.zeros((0,), dtype=torch.int64, device=self.device)
+            res += (k if return_device else k.cpu().numpy().view(np.uint64),)
+        return res
 
     def _canonical_then_shuffle(self, ev, counts, perms, shot_on, shot_off):
         """Device rows of one (iteration, polarity) group come in no particular order. The reference

@@ -132,3 +132,35 @@ def merge_by_time(streams):
     allr = torch.cat(streams, 0)
     order = torch.argsort(allr[:, 0], stable=True)
     return allr[order]
+
+
+def merge_by_key(streams, keys, offsets, n_shot):
+    """Merges the row bands of ONE pixel-sharded clip, generated with EventEmulator(row_order=...), into the stream
+    one GPU produces with the same row_order -- bit for bit, because every band sorted its rows by the whole frame's
+    keys. Per rank r: streams[r] [N_r, 4] rows with global y, keys[r] [N_r] uint64 and offsets[r] [T + 1] as
+    generate_events_band_batch(..., return_keys=True) returns them, n_shot[r] [T] the shot-noise rows that end each
+    frame (EventEmulator.last_n_shot). Per frame: the signal rows of all bands by (timestamp, key) -- every band stamps
+    an iteration with the same float32 time, the frame maximum being all-reduced; the iterations of a frame must have
+    distinct float32 timestamps --, equal keys by (y, x, polarity); then the shot rows by key (ON before OFF, each by
+    pixel). Host, numpy. Returns (rows [N, 4] float32, offsets [T + 1] int64)."""
+    to_np = lambda a, dt: (a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)).astype(dt, copy=False)
+    streams = [to_np(r, np.float32).reshape(-1, 4) for r in streams]
+    keys = [to_np(k, np.int64).view(np.uint64) if isinstance(k, torch.Tensor) else np.asarray(k, np.uint64) for k in keys]
+    offsets = [np.asarray(o, np.int64) for o in offsets]
+    n_shot = [np.asarray(s, np.int64) for s in n_shot]
+    if not (len(streams) == len(keys) == len(offsets) == len(n_shot)) or not streams:
+        raise ValueError("one stream, key array, offset array and shot-count array per rank")
+    T = len(offsets[0]) - 1
+    frame, shot = [], []
+    for r, k, o, s in zip(streams, keys, offsets, n_shot):
+        if len(o) != T + 1 or len(s) != T or o[-1] != len(r) or len(k) != len(r):
+            raise ValueError("streams, keys, offsets and n_shot do not fit together")
+        f = np.repeat(np.arange(T), np.diff(o))
+        frame.append(f)
+        shot.append(np.arange(len(r)) >= (o[1:] - s)[f])
+    rows, key = np.concatenate(streams, 0), np.concatenate(keys)
+    frame, shot = np.concatenate(frame), np.concatenate(shot)
+    t = np.where(shot, np.float32(0), rows[:, 0])
+    order = np.lexsort((rows[:, 3] < 0, rows[:, 1], rows[:, 2], key, t, shot, frame))
+    merged_offsets = np.concatenate([[0], np.cumsum(np.bincount(frame, minlength=T))]).astype(np.int64)
+    return np.ascontiguousarray(rows[order]), merged_offsets
