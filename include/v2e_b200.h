@@ -208,6 +208,39 @@ int v2e_emu_time_fused(V2eEmu *h, const void *frames_dev, int frame_dtype, int T
 int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info_host, int T, int *frames_done,
                     uint64_t *rows_total, void *stream);
 
+/* ---- single-pixel probes (emulator.py:985-1009, record_single_pixel_states) ----------------
+ * One sample per probe pixel and emitted frame: the pixel's model state after the frame, written by the device from
+ * the kernels that compute it (the multi-frame update kernel from its registers, the frame-by-frame path around the
+ * emission). Doubles hold the state dtype's value widened; the thresholds are the nominal doubles without per-pixel
+ * thresholds (per_pixel_thres = 0), the widened float32 per-pixel values otherwise. */
+typedef struct V2eProbeSample {
+    double new_frame;               /* the input value at the pixel (uint8 / float32 widened; float64 as given) */
+    double log_new_frame;           /* lin_log(new_frame) as float32, widened; the input itself with hdr */
+    double lp_log_frame;            /* low-passed photoreceptor after the frame */
+    double base_log_frame;          /* memorised value after the events and the shot-noise reset (emulator.py:936-942) */
+    double diff_frame;              /* change amplifier input before the events (emulator.py:748-754) */
+    double pos_thres, neg_thres;
+    int32_t final_pos_evts;         /* signal events emitted after the refractory filter (shot noise excluded) */
+    int32_t final_neg_evts;
+    int32_t frame;                  /* frame slot of the step (0 .. T-1) */
+    int32_t pixel;                  /* handle-local pixel index */
+} V2eProbeSample;
+/* sizeof(V2eProbeSample) as this library was compiled (a binding that mirrors the struct must refuse a mismatch) */
+int v2e_probe_sample_size(void);
+/* Probe pixels: n distinct handle-local indices (row * width + column within the handle's rows), 0 <= n <= 64, each in
+ * [0, width * height); n == 0 turns probing off (then nothing is launched or written for probes). The buffers are
+ * allocated on the device that was current at v2e_emu_create, whichever is current now. Frames of a step are recorded
+ * from the next step on. */
+int v2e_emu_set_probes(V2eEmu *h, const int32_t *pixels_host, int n);
+/* Synchronises `stream`, then copies the samples of the LAST step, if v2e_emu_collect returned V2E_OK for it and they
+ * have not been read yet: every frame of that step, frame-major (out_host[f * n + i] = probe i of frame slot f).
+ * *n_frames = frames copied (0 otherwise); cap = capacity of out_host in samples. A caller that wants every frame
+ * reads after each collect that returns V2E_OK: the next collect discards unread samples. A frame of a rejected
+ * multi-frame chunk or of a capacity abort is reported once, when its emission completes. */
+int v2e_emu_probe_read(V2eEmu *h, V2eProbeSample *out_host, int cap, int *n_frames, void *stream);
+/* The device the probe sample buffer lives on (-1: no probes set yet). */
+int v2e_emu_probe_device(V2eEmu *h);
+
 /* ---- single-frame phases (what v2e_emu_step enqueues per frame), exposed so that a host
  * that must replay torch's CPU generator can interleave its draws (SURVEY.md 7, RNG parity) */
 /* phase 1: low-pass, leak, event counts, global max (emulator.py:663-775) and, when the

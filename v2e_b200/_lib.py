@@ -40,9 +40,19 @@ class V2eFrameInfo(ctypes.Structure):
     ]
 
 
+class V2eProbeSample(ctypes.Structure):
+    _fields_ = [
+        ("new_frame", ctypes.c_double), ("log_new_frame", ctypes.c_double), ("lp_log_frame", ctypes.c_double),
+        ("base_log_frame", ctypes.c_double), ("diff_frame", ctypes.c_double),
+        ("pos_thres", ctypes.c_double), ("neg_thres", ctypes.c_double),
+        ("final_pos_evts", ctypes.c_int32), ("final_neg_evts", ctypes.c_int32),
+        ("frame", ctypes.c_int32), ("pixel", ctypes.c_int32),
+    ]
+
+
 V2E_OK, V2E_E_INVALID, V2E_E_CUDA, V2E_E_CAPACITY, V2E_E_ITER_CAP, V2E_E_STATE, V2E_E_UNSUPPORTED, V2E_E_FALLBACK = \
     0, -1, -2, -3, -4, -5, -6, -7
-ABI_VERSION = 201
+ABI_VERSION = 202
 U8, F32, F64 = 0, 1, 2
 
 _vp, _i, _d, _u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint64
@@ -137,6 +147,10 @@ _SIGS = {
     "v2e_emu_state_is_f64": (_i, [_vp]),
     "v2e_emu_state_ptr": (_vp, [_vp, _i]),
     "v2e_emu_draw_noise": (_i, [_vp, ctypes.c_uint32, _vp, _vp, _vp, _vp]),
+    "v2e_probe_sample_size": (_i, []),
+    "v2e_emu_set_probes": (_i, [_vp, _vp, _i]),
+    "v2e_emu_probe_read": (_i, [_vp, _vp, _i, ctypes.POINTER(_i), _vp]),
+    "v2e_emu_probe_device": (_i, [_vp]),
 }
 
 
@@ -177,6 +191,10 @@ def load(build_if_missing=True):
     if (ver.value, a.value, b.value, c.value) != want:
         raise RuntimeError("v2e_b200: %s has ABI %s, this binding expects %s -- rebuild with "
                            "`python -m v2e_b200.build --force`" % (path, (ver.value, a.value, b.value, c.value), want))
+    if lib.v2e_probe_sample_size() != ctypes.sizeof(V2eProbeSample):
+        raise RuntimeError("v2e_b200: %s has a %d-byte V2eProbeSample, this binding expects %d -- rebuild with "
+                           "`python -m v2e_b200.build --force`" % (path, lib.v2e_probe_sample_size(),
+                                                                  ctypes.sizeof(V2eProbeSample)))
     _LIB = lib
     return lib
 

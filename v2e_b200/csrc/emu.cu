@@ -1489,13 +1489,25 @@ __device__ __noinline__ uint32_t fused_load_codes_slow(const uint8_t *pf, int va
     return v;
 }
 
+// Single-pixel probes (v2e_emu_set_probes): px[n] handle-local pixels; out = the sample of frame slot f, probe i at
+// out[(f - slot0) * n + i] (slot0: the step slot the kernel's frame 0 is). A sample is staged where its frame slot
+// says; it becomes visible (v2e_emu_probe_read) only once v2e_emu_collect reports the step complete, so a rejected
+// multi-frame chunk or a capacity abort leaves nothing behind: the frames are recorded again when they are re-run.
+struct ProbeDev {
+    const int32_t *px;
+    V2eProbeSample *out;
+    int32_t n, slot0;
+};
+
 // WARPS warps per block, MINB blocks per SM: the register budget / occupancy / tail trade-off is picked on the host
-// (launch_fused_update). Units are dealt evenly to blocks and, inside a block, to warps.
-template <typename S, bool FAST, int WARPS, int MINB>
+// (launch_fused_update). Units are dealt evenly to blocks and, inside a block, to warps. PROBE: the thread that owns a
+// probe pixel writes that pixel's sample of every frame from its registers (the instantiation is launched only while
+// probes are set; PROBE = false compiles to the kernel without them).
+template <typename S, bool FAST, int WARPS, int MINB, bool PROBE>
 __global__ void __launch_bounds__(WARPS * 32, MINB)
 emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
                         S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
-                        uint32_t *__restrict__ rec_cnt) {
+                        uint32_t *__restrict__ rec_cnt, ProbeDev pr) {
     const bool f_pp = FAST || d.per_pixel_thres, f_leak = FAST || d.leak_on, f_shot = FAST || d.shot_on;
     constexpr bool f_lp = sizeof(S) == 8;        // no hdr here: float64 state <=> the low-pass is on
     extern __shared__ __align__(16) unsigned char s_dyn[];
@@ -1544,6 +1556,14 @@ emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8
                 ld4(d.noise_rate, i0, lnr);
 #pragma unroll
                 for (int k = 0; k < 4; k++) lnr[k] = d.leak_rate_f * lnr[k];      // emulator_utils.py:127, float32 product
+            }
+        }
+        int pid[4] = {-1, -1, -1, -1};                                  // PROBE: probe index of each of the 4 pixels
+        if (PROBE) {
+            for (int q = 0; q < pr.n; q++) {
+                const int o = pr.px[q] - i0;
+#pragma unroll
+                for (int k = 0; k < 4; k++) if (o == k) pid[k] = q;
             }
         }
         const uint32_t g0 = (uint32_t)i0 + d.px_off;
@@ -1602,6 +1622,20 @@ emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8
                 S bb = mag ? moved : base[k];
                 bb = flags ? lp[k] : bb;
                 base[k] = bb;
+                if (PROBE && pid[k] >= 0) {
+                    V2eProbeSample *ps = pr.out + (size_t)f * pr.n + pid[k];
+                    ps->new_frame = (double)code;
+                    ps->log_new_frame = tb.x;
+                    ps->lp_log_frame = (double)lp[k];
+                    ps->base_log_frame = (double)bb;
+                    ps->diff_frame = (double)diff;
+                    ps->pos_thres = f_pp ? (double)thp[k] : d.pos_nom;
+                    ps->neg_thres = f_pp ? (double)thn[k] : d.neg_nom;
+                    ps->final_pos_evts = neg ? 0 : mag;          // the filter is inactive in an accepted chunk
+                    ps->final_neg_evts = neg ? mag : 0;
+                    ps->frame = pr.slot0 + f;
+                    ps->pixel = i0 + k;
+                }
                 r16[k] = (mag | flags) ? make_rec16(lane * kVec + k, neg, flags, mag) : 0u;      // active => non-zero
             }
             // compaction of this frame's active pixels into the (frame, unit) list segment
@@ -1875,6 +1909,65 @@ emu_fused_commit_kernel(EmuDev d, const uint4 *__restrict__ lp_alt, const uint4 
     }
 }
 
+// Probes of the frame-by-frame path, one thread per probe, enqueued around the emit kernel of frame slot `slot` (only
+// while probes are set). Both leave when the emit kernel does (abort, frame not planned), so a frame whose emission
+// is re-run after a capacity abort is recorded by the re-run.
+// Before the emission: the update kernel's inputs are still in memory (lp, base after the leak, the surround, pr_eff,
+// the record, timestamp_mem), so diff and the counts that survive the refractory filter are recomputed with the same
+// operations as emu_update_kernel / warp_walk.
+template <typename S>
+__global__ void emu_probe_pre_kernel(EmuDev d, FrameParams p, int slot, const void *frame, int dtype, ProbeDev pr) {
+    const int i = threadIdx.x;
+    if (i >= pr.n) return;
+    if (*(volatile int32_t *)d.abort_flag) return;
+    const FrameCtrl *c = d.ctrl + slot;
+    if (!c->planned) return;
+    const int idx = pr.px[i];
+    const double xv = dtype == V2E_U8 ? (double)((const uint8_t *)frame)[idx]
+                    : dtype == V2E_F32 ? (double)((const float *)frame)[idx] : ((const double *)frame)[idx];
+    const double ln = d.hdr ? xv
+                    : (double)((xv >= 0.0 && xv <= 255.0 && xv == floor(xv)) ? d.lut[(int)xv] : lin_log_eval(xv));
+    const S lp = ((const S *)d.lp)[idx], base = ((const S *)d.base)[idx];
+    // what the change amplifier saw (emu_update_kernel: pr_eff exists iff the front kernel ran, which sets lp_done)
+    const S src = d.pr_eff ? ((const S *)d.pr_eff)[idx] : lp;
+    const S diff = d.csdvs ? (src - cs_buf<S>(d, *d.cs_cur)[idx]) - base : src - base;
+    const int cnt = d.rec[idx] >> kRecShift;
+    const int mag = cnt < 0 ? -cnt : cnt, pol = cnt < 0;
+    const TsParams ts = make_ts(p, c->max_n, d.refr_d);
+    const bool filter = ts.filter_active && d.refr_on;
+    float tm = (filter && mag) ? d.tmem[idx] : 0.f;
+    int fin = 0;
+    for (int it = 0; it < mag; it++) {
+        bool pass = true;
+        if (filter) {
+            const float t = linspace_f32(ts, it);
+            pass = (t - tm) > d.refr_f;
+            if (pass) tm = t;
+        }
+        fin += pass;
+    }
+    V2eProbeSample *ps = pr.out + i;
+    ps->new_frame = xv;
+    ps->log_new_frame = ln;
+    ps->lp_log_frame = (double)lp;
+    ps->diff_frame = (double)diff;
+    ps->pos_thres = d.per_pixel_thres ? (double)d.pos_thres[idx] : d.pos_nom;
+    ps->neg_thres = d.per_pixel_thres ? (double)d.neg_thres[idx] : d.neg_nom;
+    ps->final_pos_evts = pol ? 0 : fin;
+    ps->final_neg_evts = pol ? fin : 0;
+    ps->frame = slot;
+    ps->pixel = idx;
+}
+// After the emission: base after the events and the shot-noise reset, as the emit kernel left it
+template <typename S>
+__global__ void emu_probe_post_kernel(EmuDev d, int slot, ProbeDev pr) {
+    const int i = threadIdx.x;
+    if (i >= pr.n) return;
+    if (*(volatile int32_t *)d.abort_flag) return;
+    if (!d.ctrl[slot].planned) return;
+    pr.out[i].base_log_frame = (double)((const S *)d.base)[pr.px[i]];
+}
+
 // measurement floor: what an event bracket reports around a kernel that does nothing (v2e_emu_profile_read4)
 __global__ void emu_null_kernel() {}
 
@@ -1984,6 +2077,17 @@ struct V2eEmu {
         size_t bytes;               // device memory held for ordering
         long long rows_done;        // rows ordered so far
     } ord;
+    // single-pixel probes (v2e_emu_set_probes): nothing is allocated or launched while n == 0
+    struct {
+        int n;
+        int32_t *px;                // [64] device
+        V2eProbeSample *samples;    // [max_slots][n] device: the sample of every frame slot of the current step
+        V2eProbeSample *host;       // [max_slots][n] pinned
+        int ready;                  // frames of the last step v2e_emu_collect completed, not yet read
+        int device;                 // the handle's device (v2e_emu_create's current device): probe buffers live there
+        const void **frame;         // [max_slots] the frame each slot was counted from (the pre-emit probe reads it)
+        int *dtype;                 // [max_slots]
+    } probe;
 };
 
 thread_local char g_err[512] = "";
@@ -1999,9 +2103,9 @@ static int fail(int code, const char *fmt, const char *detail = "") {
 
 int v2e_set_error(int code, const char *fmt, const char *detail) { return fail(code, fmt, detail); }
 extern "C" const char *v2e_last_error(void) { return g_err; }
-extern "C" int v2e_version(void) { return 201; }
+extern "C" int v2e_version(void) { return 202; }
 extern "C" int v2e_abi_info(int *version, int *emu_cfg_size, int *frame_info_size, int *unet_weights_size) {
-    if (version) *version = 201;
+    if (version) *version = 202;
     if (emu_cfg_size) *emu_cfg_size = (int)sizeof(V2eEmuCfg);
     if (frame_info_size) *frame_info_size = (int)sizeof(V2eFrameInfo);
     if (unet_weights_size) *unet_weights_size = (int)sizeof(V2eUNetWeights);
@@ -2096,9 +2200,12 @@ extern "C" int v2e_emu_create(const V2eEmuCfg *cfg, V2eEmu **out) {
     h->state_elem = d.state_f64 ? 8 : 4;
     h->min_thres = 0.01;
     h->fused_enable = 1;
+    cudaGetDevice(&h->probe.device);
     h->ls.t_frames = new double[cfg->max_frames_per_step]();
     h->sched = new V2eEmu::Seg[(size_t)cfg->max_frames_per_step + 2]();
     h->ord.frame_index = new uint32_t[cfg->max_frames_per_step]();
+    h->probe.frame = new const void *[cfg->max_frames_per_step]();
+    h->probe.dtype = new int[cfg->max_frames_per_step]();
     d.px_off = cfg->rng_pixel_offset;
     d.units = (d.n + kUnitPx - 1) / kUnitPx;
     // state arrays are staged in whole 128-pixel units by the update kernel's bulk copies
@@ -2201,6 +2308,11 @@ extern "C" int v2e_emu_destroy(V2eEmu *h) {
     delete[] h->ls.t_frames;
     delete[] h->sched;
     delete[] h->ord.frame_index;
+    delete[] h->probe.frame;
+    delete[] h->probe.dtype;
+    if (h->probe.px) cudaFree(h->probe.px);
+    if (h->probe.samples) cudaFree(h->probe.samples);
+    if (h->probe.host) cudaFreeHost(h->probe.host);
     void *ord_ptrs[] = {h->ord.rows, h->ord.keys, h->ord.boff, h->ord.segs, h->ord.ctl};
     for (void *p : ord_ptrs) if (p) cudaFree(p);
     void *cs_ptrs[] = {d.cs_bufs, d.cs_done, h->cs_send};
@@ -2464,6 +2576,21 @@ static int take_pr_noise(V2eEmu *h, FrameParams &p, const float **prn, const cha
     return V2E_OK;
 }
 
+// the probes' view of frame slots [slot0, ...) of the step
+static ProbeDev probe_dev(const V2eEmu *h, int slot0) {
+    ProbeDev pr;
+    pr.px = h->probe.px;
+    pr.n = h->probe.n;
+    pr.out = h->probe.n ? h->probe.samples + (size_t)slot0 * h->probe.n : nullptr;
+    pr.slot0 = slot0;
+    return pr;
+}
+// the frame slot `slot` is counted from: the frame-by-frame probe reads the input value there at emission time
+static void probe_note_frame(V2eEmu *h, int slot, const void *frame, int dtype) {
+    h->probe.frame[slot] = frame;
+    h->probe.dtype[slot] = dtype;
+}
+
 // enqueue the counting kernels of one frame into `slot`
 static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int dtype, const float *lr,
                          const float *sr, int shot_pending, int slot, cudaStream_t st, const float *pr_randn = nullptr) {
@@ -2474,6 +2601,7 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
     if (d.shot_on && !shot_in_update && !shot_pending)
         return fail(V2E_E_INVALID, "shot_rand field required in replay mode (or shot_pending)");
     const int plan_in_update = (!d.refr_on && !shot_pending) ? 1 : 0;
+    probe_note_frame(h, slot, frame, dtype);
     int rc;
     int lp_done = 0;
     if (d.csdvs) {
@@ -2511,9 +2639,20 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
 static int enqueue_emit(V2eEmu *h, const FrameParams &p, int slot, float *events, cudaStream_t st) {
     const EmuDev &d = h->d;
     h->ord.events = events;
-    ProfScope ps(h, slot, 2, st);
-    if (d.state_f64) emu_emit_kernel<double><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
-    else emu_emit_kernel<float><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
+    const ProbeDev pr = probe_dev(h, slot);
+    if (pr.n) {
+        if (d.state_f64) emu_probe_pre_kernel<double><<<1, 64, 0, st>>>(d, p, slot, h->probe.frame[slot], h->probe.dtype[slot], pr);
+        else emu_probe_pre_kernel<float><<<1, 64, 0, st>>>(d, p, slot, h->probe.frame[slot], h->probe.dtype[slot], pr);
+    }
+    {
+        ProfScope ps(h, slot, 2, st);
+        if (d.state_f64) emu_emit_kernel<double><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
+        else emu_emit_kernel<float><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
+    }
+    if (pr.n) {
+        if (d.state_f64) emu_probe_post_kernel<double><<<1, 64, 0, st>>>(d, slot, pr);
+        else emu_probe_post_kernel<float><<<1, 64, 0, st>>>(d, slot, pr);
+    }
     return V2E_OK;
 }
 static void enqueue_null_bracket(V2eEmu *h, int slot, cudaStream_t st) {
@@ -2588,7 +2727,7 @@ static int fused_cfg() {
 }
 template <typename S, bool FAST, int WARPS, int MINB>
 static void launch_fused_update_cfg(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, size_t sm,
-                                    cudaStream_t st) {
+                                    const ProbeDev &pr, cudaStream_t st) {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -2596,26 +2735,33 @@ static void launch_fused_update_cfg(V2eEmu *h, const EmuDev &d, const FusedFrame
     const int min_units = 2 * WARPS;                       // small frames: at least two units per warp
     if (blocks > (d.units + min_units - 1) / min_units) blocks = (d.units + min_units - 1) / min_units;
     if (blocks < 1) blocks = 1;
-    emu_fused_update_kernel<S, FAST, WARPS, MINB><<<blocks, WARPS * 32, sm, st>>>(d, ff, frames, T, (S *)h->lp_alt,
-                                                                                   (S *)h->base_alt, h->rec_list, h->rec_cnt);
+    if (pr.n)
+        emu_fused_update_kernel<S, FAST, WARPS, MINB, true><<<blocks, WARPS * 32, sm, st>>>(
+            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr);
+    else
+        emu_fused_update_kernel<S, FAST, WARPS, MINB, false><<<blocks, WARPS * 32, sm, st>>>(
+            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr);
 }
 template <typename S, bool FAST>
 static void launch_fused_update_f(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, size_t sm,
-                                  cudaStream_t st) {
+                                  const ProbeDev &pr, cudaStream_t st) {
     switch (fused_cfg()) {
-        case 0: launch_fused_update_cfg<S, FAST, 8, 3>(h, d, ff, frames, T, sm, st); break;
-        case 2: launch_fused_update_cfg<S, FAST, 4, 7>(h, d, ff, frames, T, sm, st); break;
-        case 3: launch_fused_update_cfg<S, FAST, 8, 2>(h, d, ff, frames, T, sm, st); break;
-        default: launch_fused_update_cfg<S, FAST, 4, 5>(h, d, ff, frames, T, sm, st); break;
+        case 0: launch_fused_update_cfg<S, FAST, 8, 3>(h, d, ff, frames, T, sm, pr, st); break;
+        case 2: launch_fused_update_cfg<S, FAST, 4, 7>(h, d, ff, frames, T, sm, pr, st); break;
+        case 3: launch_fused_update_cfg<S, FAST, 8, 2>(h, d, ff, frames, T, sm, pr, st); break;
+        default: launch_fused_update_cfg<S, FAST, 4, 5>(h, d, ff, frames, T, sm, pr, st); break;
     }
 }
+// frames [a, a + T) of the step (d shifted to slot a)
 template <typename S>
-static int launch_fused_update(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, cudaStream_t st) {
+static int launch_fused_update(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, int a,
+                               cudaStream_t st) {
     const size_t sm = (size_t)T * sizeof(FusedFrame);
     const bool fast = sizeof(S) == 8 && d.rng_mode == 1 && d.per_pixel_thres && d.leak_on && d.shot_on;
     if (sm > 40 * 1024) return fail(V2E_E_INVALID, "fused path: too many frames per step");
-    if (fast) launch_fused_update_f<S, true>(h, d, ff, frames, T, sm, st);
-    else launch_fused_update_f<S, false>(h, d, ff, frames, T, sm, st);
+    const ProbeDev pr = probe_dev(h, a);
+    if (fast) launch_fused_update_f<S, true>(h, d, ff, frames, T, sm, pr, st);
+    else launch_fused_update_f<S, false>(h, d, ff, frames, T, sm, pr, st);
     return V2E_OK;
 }
 
@@ -2667,8 +2813,8 @@ static int enqueue_fused_count(V2eEmu *h, const void *frames, int T, cudaStream_
     int rc;
     {
         ProfScope ps(h, 0, 0, st);
-        rc = d.state_f64 ? launch_fused_update<double>(h, d, h->ff_dev + a, fr, T, st)
-                         : launch_fused_update<float>(h, d, h->ff_dev + a, fr, T, st);
+        rc = d.state_f64 ? launch_fused_update<double>(h, d, h->ff_dev + a, fr, T, a, st)
+                         : launch_fused_update<float>(h, d, h->ff_dev + a, fr, T, a, st);
     }
     if (rc) return rc;
     {
@@ -2863,6 +3009,7 @@ static int step_classic(V2eEmu *h, const void *frames, int dtype, int T, const d
         FrameParams p = make_params(h, t_frames[f], tp, h->step_base + (uint32_t)f, capacity);
         h->ord.frame_index[f] = h->step_base + (uint32_t)f;
         const char *frame = (const char *)frames + (size_t)f * fbytes;
+        probe_note_frame(h, f, frame, dtype);
         const float *lr = leak_randn ? leak_randn + (size_t)f * d.n : nullptr;
         const float *sr = shot_rand ? shot_rand + (size_t)f * d.n : nullptr;
         if (resume_emit && f == first) {
@@ -3011,6 +3158,7 @@ extern "C" int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info, int T, int *frames
                                uint64_t *rows_total, void *stream) {
     if (!h || !info || T < 1 || T > h->d.max_slots) return fail(V2E_E_INVALID, "bad argument");
     cudaStream_t st = (cudaStream_t)stream;
+    h->probe.ready = 0;             // a new step's samples replace any unread ones; set again below on V2E_OK
     CU(cudaMemcpyAsync(h->ctrl_host, h->d.ctrl, (size_t)(T + 1) * sizeof(FrameCtrl), cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h->abort_host, h->d.abort_flag, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -3101,9 +3249,64 @@ extern "C" int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info, int T, int *frames
     }
     if (frames_done) *frames_done = done;
     if (rows_total) *rows_total = rows;
+    h->probe.ready = (!status && h->probe.n) ? T : 0;      // every frame of the step emitted: its samples are final
     if (status == V2E_E_CAPACITY) return fail(V2E_E_CAPACITY, "event buffer too small");
     if (status == V2E_E_ITER_CAP) return fail(V2E_E_ITER_CAP, "a pixel exceeded iter_cap events in one frame");
     if (h->ord.mode) return order_step(h, T, st);
+    return V2E_OK;
+}
+
+extern "C" int v2e_probe_sample_size(void) { return (int)sizeof(V2eProbeSample); }
+
+extern "C" int v2e_emu_set_probes(V2eEmu *h, const int32_t *pixels_host, int n) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    if (n < 0 || n > 64 || (n > 0 && !pixels_host)) return fail(V2E_E_INVALID, "probes: 0 <= n <= 64 pixels");
+    for (int i = 0; i < n; i++) {
+        if (pixels_host[i] < 0 || pixels_host[i] >= h->d.n) return fail(V2E_E_INVALID, "probe pixel outside the handle");
+        for (int k = 0; k < i; k++)
+            if (pixels_host[k] == pixels_host[i]) return fail(V2E_E_INVALID, "probe pixels must be distinct");
+    }
+    // the buffers belong on the handle's device, whichever device is current for the caller
+    int cur = 0;
+    CU(cudaGetDevice(&cur));
+    if (cur != h->probe.device) CU(cudaSetDevice(h->probe.device));
+    const size_t per_slot = (size_t)h->d.max_slots * 64;
+    cudaError_t e = cudaSuccess;
+    if (n > 0 && !h->probe.px) {
+        e = cudaMalloc((void **)&h->probe.px, 64 * sizeof(int32_t));
+        if (e == cudaSuccess) e = cudaMalloc((void **)&h->probe.samples, per_slot * sizeof(V2eProbeSample));
+        if (e == cudaSuccess) e = cudaMallocHost((void **)&h->probe.host, per_slot * sizeof(V2eProbeSample));
+    }
+    if (e == cudaSuccess && n > 0) e = cudaMemcpy(h->probe.px, pixels_host, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (cur != h->probe.device) cudaSetDevice(cur);
+    if (e != cudaSuccess) return fail(V2E_E_CUDA, "v2e_emu_set_probes: %s", cudaGetErrorString(e));
+    h->probe.n = n;
+    h->probe.ready = 0;
+    return V2E_OK;
+}
+
+extern "C" int v2e_emu_probe_device(V2eEmu *h) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    if (!h->probe.samples) return -1;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, h->probe.samples) != cudaSuccess) return fail(V2E_E_CUDA, "cudaPointerGetAttributes failed");
+    return a.device;
+}
+
+extern "C" int v2e_emu_probe_read(V2eEmu *h, V2eProbeSample *out_host, int cap, int *n_frames, void *stream) {
+    if (!h || !n_frames) return fail(V2E_E_INVALID, "null argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    CU(cudaStreamSynchronize(st));
+    const int nf = h->probe.n ? h->probe.ready : 0;
+    const size_t cnt = (size_t)nf * h->probe.n;
+    if (cnt > 0) {
+        if (!out_host || (size_t)cap < cnt) return fail(V2E_E_INVALID, "probe samples: out_host too small");
+        CU(cudaMemcpyAsync(h->probe.host, h->probe.samples, cnt * sizeof(V2eProbeSample), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        memcpy(out_host, h->probe.host, cnt * sizeof(V2eProbeSample));
+    }
+    h->probe.ready = 0;
+    *n_frames = nf;
     return V2E_OK;
 }
 
@@ -3133,8 +3336,8 @@ extern "C" int v2e_emu_time_fused(V2eEmu *h, const void *frames, int dtype, int 
     if (!rc) rc = reset_slots(h, 0, T, st);
     cudaEventRecord(e[2], st);
     for (int k = 0; k < K && !rc; k++)
-        rc = h->d.state_f64 ? launch_fused_update<double>(h, h->d, h->ff_dev, (const uint8_t *)frames, T, st)
-                            : launch_fused_update<float>(h, h->d, h->ff_dev, (const uint8_t *)frames, T, st);
+        rc = h->d.state_f64 ? launch_fused_update<double>(h, h->d, h->ff_dev, (const uint8_t *)frames, T, 0, st)
+                            : launch_fused_update<float>(h, h->d, h->ff_dev, (const uint8_t *)frames, T, 0, st);
     cudaEventRecord(e[3], st);
     h->profile = prof;
     if (!rc) rc = reset_slots(h, 0, T, st);
@@ -3192,6 +3395,7 @@ extern "C" int v2e_emu_phase_update(V2eEmu *h, const void *frame, int dtype, dou
     const EmuDev &d = h->d;
     if (d.rng_mode == 0 && d.leak_on && !lr) return fail(V2E_E_INVALID, "leak_randn field required in replay mode");
     if (d.csdvs) return fail(V2E_E_UNSUPPORTED, "centre-surround model: a pixel-sharded handle is stepped with v2e_emu_cs_* (cs_halo_rows > 0)");
+    probe_note_frame(h, 0, frame, dtype);
     // SCIDVS / photoreceptor noise: the front end on the band's rows (the noise draws use whole-frame pixel indices)
     int lp_done = 0;
     if (d.scidvs || d.pr_noise) {
@@ -3284,6 +3488,7 @@ extern "C" int v2e_emu_cs_update(V2eEmu *h, const void *frame, int dtype, const 
     const EmuDev &d = h->d;
     if (d.rng_mode == 0 && d.leak_on && !lr) return fail(V2E_E_INVALID, "leak_randn field required in replay mode");
     cudaStream_t st = (cudaStream_t)stream;
+    probe_note_frame(h, 0, frame, dtype);
     int rc = d.state_f64 ? launch_update<double>(h, h->cs_p, frame, dtype, lr, sr, 0, 0, 1, st)
                          : launch_update<float>(h, h->cs_p, frame, dtype, lr, sr, 0, 0, 1, st);
     if (rc) return rc;

@@ -15,7 +15,7 @@ Two RNG modes:
       per-frame noise is enabled, statistically equivalent otherwise.
 
 Extra keywords (not in the reference): rng_mode, rng (draw source object), iter_cap,
-max_frames_per_step, exact_order, shard, fused, row_order.
+max_frames_per_step, exact_order, shard, fused, row_order, record_pixels.
 
 Row order in device mode. The kernels put a row inside its (frame, iteration, polarity) group wherever an atomicAdd
 placed it, so with row_order=None (default) the order inside a group can change from run to run. row_order="canonical"
@@ -33,7 +33,14 @@ formatted on the device (v2e_b200.sinks.events_to_text) and written to the write
 labels every returned row signal (1) or shot noise (0) -- `last_signnoise_label`, generate_events_batch(...,
 return_labels=True) -- and passes the labels to the text and AEDAT-2.0 sinks. A pixel-sharded emulator labels its own
 rows (generate_events_band(_batch)(..., return_labels=True)) and writes no sink: a file needs the merged stream.
-show_dvs_model_state / record_single_pixel_states (GUI / debug probes) are ignored with a warning.
+show_dvs_model_state / save_dvs_model_state (GUI probes) are ignored with a warning.
+
+record_single_pixel_states=(a, b) records, like the reference (emulator.py:278-302, 985-1009), pixel row a, column b
+(the tuple indexes frames as frame[a, b]) after every frame: single_pixel_states, single_pixel_sample_count,
+save_recorded_single_pixel_states(), saved to SINGLE_PIXEL_STATES_FILENAME in the current directory at cleanup(), at
+exit and when SINGLE_PIXEL_MAX_SAMPLES are full. record_pixels=[(a, b), ...] (extension, up to 64) records the same
+ten quantities without a limit (pixel_traces()). The device writes the samples (DESIGN.md 4.1); every path records,
+and a sharded emulator records on the rank whose own rows hold the pixel.
 """
 import ctypes
 import logging
@@ -165,9 +172,10 @@ class _Sinks:
         self.h5 = self.h5_dataset = self.aedat2 = self.aedat4 = self.text = None
 
 
-def _finalize(lib, box, sinks):
-    """weakref.finalize callback: frees the library handle and closes the writers of a collected (or
-    exiting) emulator without keeping it alive (the reference registers cleanup with atexit, emulator.py:372)."""
+def _finalize(lib, box, sinks, spx):
+    """weakref.finalize callback: frees the library handle, closes the writers and saves the single-pixel recording
+    of a collected (or exiting) emulator without keeping it alive (the reference registers cleanup with atexit,
+    emulator.py:372)."""
     h = box[0]
     box[0] = None
     if h:
@@ -177,6 +185,41 @@ def _finalize(lib, box, sinks):
             pass
     if sinks is not None:
         sinks.close()
+    if spx["pixel"] is not None and spx["owner"]:
+        _save_pixel_states(spx["states"], spx["count"], spx["file"])
+
+
+# the device's V2eProbeSample (include/v2e_b200.h) and the reference's recorded names (emulator.py:291-302)
+_PROBE_DTYPE = np.dtype([("new_frame", "<f8"), ("log_new_frame", "<f8"), ("lp_log_frame", "<f8"),
+                         ("base_log_frame", "<f8"), ("diff_frame", "<f8"), ("pos_thres", "<f8"), ("neg_thres", "<f8"),
+                         ("final_pos_evts", "<i4"), ("final_neg_evts", "<i4"), ("frame", "<i4"), ("pixel", "<i4")])
+_PIXEL_STATE_FIELDS = (("new_frame", "new_frame"), ("base_log_frame", "base_log_frame"),
+                       ("lp_log_frame", "lp_log_frame"), ("log_new_frame", "log_new_frame"),
+                       ("pos_thres", "pos_thres"), ("neg_thres", "neg_thres"), ("diff_frame", "diff_frame"),
+                       ("final_neg_evts_frame", "final_neg_evts"), ("final_pos_evts_frame", "final_pos_evts"))
+PIXEL_STATE_NAMES = ("time",) + tuple(k for k, _ in _PIXEL_STATE_FIELDS)
+
+
+def _save_pixel_states(states, count, filename):
+    """emulator.py:428-437: the dict, pickled to `filename` relative to the current directory."""
+    import pickle
+    try:
+        with open(filename, "wb") as outfile:
+            pickle.dump(states, outfile, protocol=pickle.HIGHEST_PROTOCOL)
+            logger.info(f"saved single pixel states with {count} samples to {filename}")
+    except Exception as e:
+        logger.error(f"could not save pickled pixel states, got {e}")
+
+
+def _pixel_list(arg, name):
+    if not isinstance(arg, (list, tuple)) or len(arg) > 64:
+        raise ValueError(f"{name} must be a list of at most 64 (row, column) tuples")
+    out = []
+    for p in arg:
+        if not (isinstance(p, tuple) and len(p) == 2 and all(type(i) is int for i in p)):
+            raise ValueError(f"{name}: {p!r} is not a (row, column) tuple of two ints")
+        out.append(p)
+    return out
 
 
 _STATE_IDS = {"lp_log_frame": 0, "base_log_frame": 1, "pos_thres": 2, "neg_thres": 3,
@@ -189,6 +232,8 @@ class EventEmulator(object):
                     'photoreceptor_noise_arr', 'cs_surround_frame', 'c_minus_s_frame',
                     'base_log_frame', 'diff_frame')
     MAX_CHANGE_TO_TERMINATE_EULER_SURROUND_STEPPING = 1e-5
+    SINGLE_PIXEL_STATES_FILENAME = 'pixel-states.dat'
+    SINGLE_PIXEL_MAX_SAMPLES = 10000
 
     def __init__(
             self,
@@ -229,6 +274,7 @@ class EventEmulator(object):
             shard=None,
             fused: bool = True,
             row_order: str = None,
+            record_pixels=None,
     ):
         if not str(device).startswith("cuda"):
             raise RuntimeError("v2e_b200.EventEmulator runs on a CUDA device only (device=%r); "
@@ -245,10 +291,18 @@ class EventEmulator(object):
             for i in record_single_pixel_states:
                 if not (type(i) is int):
                     raise ValueError(f'--record_single_pixel_states {record_single_pixel_states} should have two integer-value pixel addresses (x,y)')
-        if show_dvs_model_state or save_dvs_model_state or record_single_pixel_states is not None:
-            logger.warning("show_dvs_model_state / save_dvs_model_state / record_single_pixel_states are GUI / debug "
-                           "probes of the reference (out of scope, SURVEY.md 2): ignored; the state tensors are "
-                           "available by the same attribute names")
+        if show_dvs_model_state or save_dvs_model_state:
+            logger.warning("show_dvs_model_state / save_dvs_model_state are GUI probes of the reference (out of scope, "
+                           "SURVEY.md 2): ignored; the state tensors are available by the same attribute names")
+        # single-pixel recording (emulator.py:278-302, 985-1009): shared with the finalizer, which saves at exit
+        self._spx = {"pixel": record_single_pixel_states, "count": 0, "owner": True,
+                     "file": self.SINGLE_PIXEL_STATES_FILENAME, "col": None,
+                     "states": None if record_single_pixel_states is None else
+                     {k: np.empty(self.SINGLE_PIXEL_MAX_SAMPLES) * np.nan for k in PIXEL_STATE_NAMES}}
+        self._record_pixels = _pixel_list(record_pixels, "record_pixels") if record_pixels is not None else None
+        self._trace_cols = None       # record_pixels: probe index of each (-1: not on this rank's rows)
+        self._traces = []             # record_pixels: one (t, samples) per frame
+        self._n_probes = 0
         if rng_mode not in ("replay", "device"):
             raise ValueError("rng_mode must be 'replay' or 'device'")
         if row_order not in (None, "canonical", "shuffled"):
@@ -324,7 +378,7 @@ class EventEmulator(object):
         self.t_previous = 0
         # the reference registers cleanup with atexit (emulator.py:372), which would keep every instance alive
         # until exit; a finalizer frees the device memory when the object is collected AND runs at exit
-        self._finalizer = weakref.finalize(self, _finalize, self._lib, self._hbox, self._sinks)
+        self._finalizer = weakref.finalize(self, _finalize, self._lib, self._hbox, self._sinks, self._spx)
 
     @property
     def _h(self):
@@ -333,6 +387,98 @@ class EventEmulator(object):
     @_h.setter
     def _h(self, v):
         self._hbox[0] = v
+
+    # single-pixel recording, by the reference's attribute names. The pixel (a, b) indexes frames as arr[(a, b)]:
+    # row a, column b. Setting record_single_pixel_states = None stops recording (and the save at exit).
+    record_single_pixel_states = property(lambda self: self._spx["pixel"],
+                                          lambda self, v: self._spx.__setitem__("pixel", v))
+    single_pixel_states = property(lambda self: self._spx["states"],
+                                   lambda self, v: self._spx.__setitem__("states", v))
+    single_pixel_sample_count = property(lambda self: self._spx["count"],
+                                         lambda self, v: self._spx.__setitem__("count", v))
+
+    def save_recorded_single_pixel_states(self):
+        """emulator.py:428-437: pickles single_pixel_states to SINGLE_PIXEL_STATES_FILENAME in the current directory."""
+        _save_pixel_states(self._spx["states"], self._spx["count"], self.SINGLE_PIXEL_STATES_FILENAME)
+
+    def pixel_traces(self):
+        """record_pixels=[(row, column), ...]: every frame's state of those pixels since construction, without the
+        reference's sample limit: a dict of the recorder's names, 'time' as a float64 [frames] array and the others as
+        float64 [frames, pixels] arrays (NaN for a pixel outside a sharded emulator's own rows)."""
+        if self._record_pixels is None:
+            raise RuntimeError("pixel_traces needs record_pixels=[(row, column), ...]")
+        P = len(self._record_pixels)
+        out = {"time": np.array([t for t, _ in self._traces], dtype=np.float64)}
+        for key, field in _PIXEL_STATE_FIELDS:
+            a = np.full((len(self._traces), P), np.nan)
+            for f, (_, s) in enumerate(self._traces):
+                for j, col in enumerate(self._trace_cols or []):
+                    if col >= 0:
+                        a[f, j] = s[col][field]
+            out[key] = a
+        return out
+
+    def _set_probes(self, H, W, y0, y1, ye0):
+        """The probe pixels of a new handle: the recorded pixels inside this emulator's own rows [y0, y1) of frames of
+        H x W pixels, as handle-local indices (the handle's row 0 is frame row ye0)."""
+        want = []
+        if self._spx["pixel"] is not None:
+            want.append(tuple(self._spx["pixel"]))
+        want += list(self._record_pixels or [])
+        for r, c in want:
+            if not (0 <= r < H and 0 <= c < W):
+                raise ValueError("recorded pixel (row %d, column %d) is outside the %d x %d frame" % (r, c, H, W))
+        local = []
+        for r, c in want:
+            if y0 <= r < y1 and (r - ye0) * W + c not in local:
+                local.append((r - ye0) * W + c)
+        col = lambda p: local.index((p[0] - ye0) * W + p[1]) if y0 <= p[0] < y1 else -1
+        if self._spx["pixel"] is not None:
+            c = col(self._spx["pixel"])
+            self._spx["col"] = c if c >= 0 else None
+            self._spx["owner"] = c >= 0
+        if self._record_pixels is not None:
+            self._trace_cols = [col(p) for p in self._record_pixels]
+        self._n_probes = len(local)
+        if local:
+            px = np.asarray(local, dtype=np.int32)
+            _lib.check(self._lib.v2e_emu_set_probes(self._h, px.ctypes.data_as(ctypes.c_void_p), len(local)))
+
+    def _drain_probes(self, t_frames):
+        """After v2e_emu_collect returned V2E_OK (it synchronised): the probe samples of the step's frames."""
+        if not self._n_probes:
+            return
+        n = self._n_probes
+        buf = np.zeros(len(t_frames) * n, dtype=_PROBE_DTYPE)
+        nf = ctypes.c_int(0)
+        _lib.check(self._lib.v2e_emu_probe_read(self._h, buf.ctypes.data_as(ctypes.c_void_p), buf.size,
+                                                ctypes.byref(nf), self._stream()))
+        if nf.value != len(t_frames):
+            raise RuntimeError("probe samples of %d frames, expected %d" % (nf.value, len(t_frames)))
+        self._record(buf.reshape(len(t_frames), n), t_frames)
+
+    def _record(self, samples, t_frames):
+        """samples [frames, probes] (_PROBE_DTYPE) of frames at t_frames -> the recorder (emulator.py:985-1009: when
+        the counter has reached SINGLE_PIXEL_MAX_SAMPLES the next frame saves the file and stops recording) and the
+        record_pixels traces."""
+        spx = self._spx
+        for f, t in enumerate(t_frames):
+            if self._record_pixels is not None:
+                self._traces.append((float(t), samples[f].copy()))
+            if spx["pixel"] is None or not spx["owner"] or spx["col"] is None:
+                continue
+            k = spx["count"]
+            if k < self.SINGLE_PIXEL_MAX_SAMPLES:
+                if k % 250 == 0:
+                    logger.info(f"recorded {k} single pixel states")
+                s = samples[f, spx["col"]]
+                spx["states"]["time"][k] = t
+                for key, field in _PIXEL_STATE_FIELDS:
+                    spx["states"][key][k] = s[field]
+                spx["count"] = k + 1
+            else:
+                self.save_recorded_single_pixel_states()
+                spx["pixel"] = None
 
     # ------------------------------------------------------------------------------------------
     def reset(self):
@@ -349,6 +495,8 @@ class EventEmulator(object):
         self._destroy_handle()
         if self._sinks is not None:
             self._sinks.close()
+        if self._spx["pixel"] is not None and self._spx["owner"]:     # emulator.py:425-426
+            self.save_recorded_single_pixel_states()
 
     def prepare_storage(self, n_frames, frame_ts):
         return None  # HDF5 frame storage is a sink (out of scope); kept for call compatibility
@@ -521,6 +669,8 @@ class EventEmulator(object):
         self._create(ye1 - ye0, W, px_offset=ye0 * W, own=(y0 - ye0, y1 - y0) if K else None, cs_halo=K,
                      full_px=H * W)
         self._full_h, self._ye0, self._cs_K = H, ye0, K
+        with torch.cuda.device(self.device):
+            self._set_probes(H, W, y0, y1, ye0)
         rows = lambda t: t[ye0:ye1].contiguous()
         L, p = self._lib, lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
         with torch.cuda.device(self.device):
@@ -736,6 +886,7 @@ class EventEmulator(object):
             _lib.check(L.v2e_emu_collect(h, info, 1, ctypes.byref(done), ctypes.byref(rows), st))
         else:
             _lib.check(rc)
+        self._drain_probes([t_frame])
         return info[0]
 
     # pixel-sharded path (SURVEY.md 8e, BASELINE config 5): this rank owns rows [y0, y1) ---------------
@@ -905,6 +1056,7 @@ class EventEmulator(object):
                 if rc == _lib.V2E_E_FALLBACK:
                     return int(done.value)
                 _lib.check(rc)
+                self._drain_probes(t_frames[a:b])
                 for k in range(Tc):
                     self._account(info[k])
                     offs.append(state["total"] + int(info[k].ev_base) + int(info[k].n_events))
@@ -1038,6 +1190,7 @@ class EventEmulator(object):
                 # kernels only those up to the frame that did not fit
                 need = max(int(info[f].ev_base) + int(info[f].n_events) for f in range(first, T))
                 self._grow_event_buffer(max(2 * need, 2 * self._ev_dev.shape[0]), keep=base)
+            self._drain_probes(t_frames)
             total = int(rows.value)
             offsets = np.array([int(info[f].ev_base) for f in range(T)] + [total], np.int64)
             n_shot = np.array([int(info[f].n_shot_on) + int(info[f].n_shot_off) for f in range(T)], np.int64)
