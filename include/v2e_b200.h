@@ -241,6 +241,28 @@ int v2e_emu_probe_read(V2eEmu *h, V2eProbeSample *out_host, int cap, int *n_fram
 /* The device the probe sample buffer lives on (-1: no probes set yet). */
 int v2e_emu_probe_device(V2eEmu *h);
 
+/* ---- model-state planes (emulator.py:41-50, 580-617, 756-767, show_dvs_model_state) -----------------------------
+ * One uint8 plane per shown state and emitted frame, taken after the low-pass, noise, SCIDVS, surround and leak
+ * updates and before the events: byte = u8(((x - lo) / span) * 255) in float64, x the state's value widened, u8 the
+ * cast numpy's astype(uint8) makes (truncation toward zero, low 8 bits; NaN, +-inf and values outside int32 range
+ * give 0). The planes cover the handle's own rows only (never a sharded handle's halo rows). */
+#define V2E_MODEL_STATES 9      /* state bits, EventEmulator.MODEL_STATES order: */
+/* 0 new_frame, 1 log_new_frame, 2 lp_log_frame, 3 scidvs_highpass, 4 photoreceptor_noise_arr, 5 cs_surround_frame,
+ * 6 c_minus_s_frame, 7 base_log_frame, 8 diff_frame */
+/* mask: the shown states (bit i = state i; 0 turns capture off, then nothing is launched or written for it).
+ * lo_span_host[2 * i], [2 * i + 1]: lo and hi - lo of state i (read for the shown states only). Bit 3 needs SCIDVS,
+ * bits 5 and 6 the centre-surround model. The staging buffer [max_slots][shown states][own pixels] is allocated on the
+ * handle's device (v2e_emu_create's current device) whichever is current now. Frames are captured from the next step
+ * on. */
+int v2e_emu_set_model_states(V2eEmu *h, uint32_t mask, const double *lo_span_host);
+/* Copies (device to device, enqueued on `stream`) the planes of the LAST step, if v2e_emu_collect returned V2E_OK for
+ * it and they have not been read yet: dst_dev[f][s][p] = frame slot f, s-th shown state in bit order, own pixel p.
+ * *n_frames = frames copied (0 otherwise); cap = capacity of dst_dev in bytes. Like v2e_emu_probe_read, the next
+ * collect discards unread planes; a frame of a rejected multi-frame chunk or of a capacity abort is reported once. */
+int v2e_emu_model_state_read(V2eEmu *h, void *dst_dev, uint64_t cap, int *n_frames, void *stream);
+/* The device the model-state staging buffer lives on (-1: none allocated yet). */
+int v2e_emu_model_state_device(V2eEmu *h);
+
 /* ---- single-frame phases (what v2e_emu_step enqueues per frame), exposed so that a host
  * that must replay torch's CPU generator can interleave its draws (SURVEY.md 7, RNG parity) */
 /* phase 1: low-pass, leak, event counts, global max (emulator.py:663-775) and, when the

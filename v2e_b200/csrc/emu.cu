@@ -1499,15 +1499,35 @@ struct ProbeDev {
     int32_t n, slot0;
 };
 
-// WARPS warps per block, MINB blocks per SM: the register budget / occupancy / tail trade-off is picked on the host
-// (launch_fused_update). Units are dealt evenly to blocks and, inside a block, to warps. PROBE: the thread that owns a
-// probe pixel writes that pixel's sample of every frame from its registers (the instantiation is launched only while
-// probes are set; PROBE = false compiles to the kernel without them).
-template <typename S, bool FAST, int WARPS, int MINB, bool PROBE>
-__global__ void __launch_bounds__(WARPS * 32, MINB)
-emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
-                        S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
-                        uint32_t *__restrict__ rec_cnt, ProbeDev pr) {
+// Model-state planes (v2e_emu_set_model_states): out = plane s (the s-th shown state in bit order) of the kernel's
+// frame f at out + (f * nst + s) * npx, pixel p of the plane = handle pixel p0 + p. Staged by frame slot and made
+// visible by v2e_emu_collect, like the probe samples.
+struct PlaneDev {
+    uint8_t *out;
+    uint32_t mask;
+    int32_t nst, npx, p0;
+    double lo[V2E_MODEL_STATES], span[V2E_MODEL_STATES];
+};
+// ndarray.astype(np.uint8) of a float64 on x86-64: a truncating conversion to int32 (cvttsd2si) whose low 8 bits are
+// kept; NaN and values outside int32 range convert to 0x80000000, whose low byte is 0
+__device__ __forceinline__ uint32_t np_u8(double v) {
+    return (v > -2147483649.0 && v < 2147483648.0) ? ((uint32_t)(int32_t)v & 0xffu) : 0u;
+}
+// emulator.py:594-617: (x - lo) / (hi - lo), * 255, astype(uint8), all in float64 (the ranges are float64 scalars)
+__device__ __forceinline__ uint32_t state_byte(const PlaneDev &pl, int s, double x) {
+    return np_u8(((x - pl.lo[s]) / pl.span[s]) * 255.0);
+}
+
+// The multi-frame update (pass 1), shared by the kernel without planes (emu_fused_update_kernel) and the one that
+// writes them (emu_fused_update_planes_kernel). PROBE: the thread that owns a probe pixel writes that pixel's sample of
+// every frame from its registers. PLANES: every thread writes its quad's bytes of the shown states of every frame
+// from its registers (new_frame, log_new_frame, lp_log_frame, the zero photoreceptor_noise_arr, base_log_frame after
+// the leak and before the events, diff_frame: the states that exist where the multi-frame kernels run).
+template <typename S, bool FAST, int WARPS, bool PROBE, bool PLANES>
+__device__ __forceinline__ void
+fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
+                  S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
+                  uint32_t *__restrict__ rec_cnt, const ProbeDev &pr, const PlaneDev &pl) {
     const bool f_pp = FAST || d.per_pixel_thres, f_leak = FAST || d.leak_on, f_shot = FAST || d.shot_on;
     constexpr bool f_lp = sizeof(S) == 8;        // no hdr here: float64 state <=> the low-pass is on
     extern __shared__ __align__(16) unsigned char s_dyn[];
@@ -1566,6 +1586,9 @@ emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8
                 for (int k = 0; k < 4; k++) if (o == k) pid[k] = q;
             }
         }
+        // PLANES: each plane's rows of bytes are 4-byte aligned at a quad iff the plane size is a multiple of 4
+        const bool pal = (pl.npx & 3) == 0;
+        const uint32_t nz_byte = PLANES ? state_byte(pl, 4, 0.0) * 0x01010101u : 0u;
         const uint32_t g0 = (uint32_t)i0 + d.px_off;
         uint16_t *seg = rec_list + (size_t)unit * kUnitPx;               // + f * units * kUnitPx per frame
         uint32_t *cntp = rec_cnt + unit;
@@ -1581,6 +1604,7 @@ emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8
             float lr[4] = {0.f, 0.f, 0.f, 0.f};
             uint32_t pref[4] = {0u, 0u, 0u, 0u};
             if (use_rng) noise_px4(d.seed, g0, frame_index, lr, pref);
+            uint32_t pb[5] = {0u, 0u, 0u, 0u, 0u};     // PLANES: new_frame, log_new_frame, lp, base, diff bytes
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int code = (int)((codes >> (8 * k)) & 0xffu);
@@ -1600,6 +1624,13 @@ emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8
                 }
                 // difference and event count (emulator.py:748-772, emulator_utils.py:137-173)
                 const S diff = lp[k] - base[k];
+                if (PLANES) {
+                    if (pl.mask & 1u) pb[0] |= state_byte(pl, 0, (double)code) << (8 * k);
+                    if (pl.mask & 2u) pb[1] |= state_byte(pl, 1, tb.x) << (8 * k);
+                    if (pl.mask & 4u) pb[2] |= state_byte(pl, 2, (double)lp[k]) << (8 * k);
+                    if (pl.mask & 128u) pb[3] |= state_byte(pl, 7, (double)base[k]) << (8 * k);
+                    if (pl.mask & 256u) pb[4] |= state_byte(pl, 8, (double)diff) << (8 * k);
+                }
                 const bool neg = diff < (S)0;
                 const float thf = neg ? thn[k] : thp[k];
                 S b;
@@ -1638,6 +1669,20 @@ emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8
                 }
                 r16[k] = (mag | flags) ? make_rec16(lane * kVec + k, neg, flags, mag) : 0u;      // active => non-zero
             }
+            if (PLANES && valid) {
+                uint8_t *o = pl.out + (size_t)f * pl.nst * pl.npx + i0;
+                const uint32_t v[V2E_MODEL_STATES] = {pb[0], pb[1], pb[2], 0u, nz_byte, 0u, 0u, pb[3], pb[4]};
+#pragma unroll
+                for (int j = 0; j < V2E_MODEL_STATES; j++) {
+                    if (!((pl.mask >> j) & 1u)) continue;
+                    if (pal && valid == 4) {
+                        *(uint32_t *)o = v[j];
+                    } else {
+                        for (int k = 0; k < valid; k++) o[k] = (uint8_t)(v[j] >> (8 * k));
+                    }
+                    o += pl.npx;
+                }
+            }
             // compaction of this frame's active pixels into the (frame, unit) list segment
             uint32_t cnt = 0;
             if (__any_sync(0xffffffffu, (r16[0] | r16[1] | r16[2] | r16[3]) != 0u)) {
@@ -1657,6 +1702,26 @@ emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8
             st4(base_out, i0, base);
         }
     }
+}
+
+// WARPS warps per block, MINB blocks per SM: the register budget / occupancy / tail trade-off is picked on the host
+// (launch_fused_update). Units are dealt evenly to blocks and, inside a block, to warps. PROBE = false compiles to the
+// kernel without probes; the instantiation with them is launched only while probes are set.
+template <typename S, bool FAST, int WARPS, int MINB, bool PROBE>
+__global__ void __launch_bounds__(WARPS * 32, MINB)
+emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
+                        S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
+                        uint32_t *__restrict__ rec_cnt, ProbeDev pr) {
+    const PlaneDev pl{};
+    fused_update_body<S, FAST, WARPS, PROBE, false>(d, ff, frames, T, lp_out, base_out, rec_list, rec_cnt, pr, pl);
+}
+// The same update writing the model-state planes (launched only while states are shown; probes may be set too).
+template <typename S, bool FAST, int WARPS, int MINB>
+__global__ void __launch_bounds__(WARPS * 32, MINB)
+emu_fused_update_planes_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
+                               S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
+                               uint32_t *__restrict__ rec_cnt, ProbeDev pr, PlaneDev pl) {
+    fused_update_body<S, FAST, WARPS, true, true>(d, ff, frames, T, lp_out, base_out, rec_list, rec_cnt, pr, pl);
 }
 
 // the records of up to 8 consecutive units of one frame as one list: off[k] = first list position of unit k
@@ -1915,6 +1980,27 @@ emu_fused_commit_kernel(EmuDev d, const uint4 *__restrict__ lp_alt, const uint4 
 // Before the emission: the update kernel's inputs are still in memory (lp, base after the leak, the surround, pr_eff,
 // the record, timestamp_mem), so diff and the counts that survive the refractory filter are recomputed with the same
 // operations as emu_update_kernel / warp_walk.
+template <typename S> struct PreEmit {
+    double xv, ln;                      // new_frame, log_new_frame
+    S lp, sur, cms, base, diff;         // lp_log_frame, cs_surround_frame, c_minus_s_frame, base after the leak, diff
+};
+template <typename S>
+__device__ __forceinline__ PreEmit<S> pre_emit_state(const EmuDev &d, int idx, const void *frame, int dtype) {
+    PreEmit<S> e;
+    e.xv = dtype == V2E_U8 ? (double)((const uint8_t *)frame)[idx]
+         : dtype == V2E_F32 ? (double)((const float *)frame)[idx] : ((const double *)frame)[idx];
+    e.ln = d.hdr ? e.xv
+         : (double)((e.xv >= 0.0 && e.xv <= 255.0 && e.xv == floor(e.xv)) ? d.lut[(int)e.xv] : lin_log_eval(e.xv));
+    e.lp = ((const S *)d.lp)[idx];
+    e.base = ((const S *)d.base)[idx];
+    // what the change amplifier saw (emu_update_kernel: pr_eff exists iff the front kernel ran, which sets lp_done)
+    const S src = d.pr_eff ? ((const S *)d.pr_eff)[idx] : e.lp;
+    e.sur = d.csdvs ? cs_buf<S>(d, *d.cs_cur)[idx] : (S)0;
+    e.cms = src - e.sur;
+    e.diff = d.csdvs ? e.cms - e.base : src - e.base;
+    return e;
+}
+
 template <typename S>
 __global__ void emu_probe_pre_kernel(EmuDev d, FrameParams p, int slot, const void *frame, int dtype, ProbeDev pr) {
     const int i = threadIdx.x;
@@ -1923,14 +2009,9 @@ __global__ void emu_probe_pre_kernel(EmuDev d, FrameParams p, int slot, const vo
     const FrameCtrl *c = d.ctrl + slot;
     if (!c->planned) return;
     const int idx = pr.px[i];
-    const double xv = dtype == V2E_U8 ? (double)((const uint8_t *)frame)[idx]
-                    : dtype == V2E_F32 ? (double)((const float *)frame)[idx] : ((const double *)frame)[idx];
-    const double ln = d.hdr ? xv
-                    : (double)((xv >= 0.0 && xv <= 255.0 && xv == floor(xv)) ? d.lut[(int)xv] : lin_log_eval(xv));
-    const S lp = ((const S *)d.lp)[idx], base = ((const S *)d.base)[idx];
-    // what the change amplifier saw (emu_update_kernel: pr_eff exists iff the front kernel ran, which sets lp_done)
-    const S src = d.pr_eff ? ((const S *)d.pr_eff)[idx] : lp;
-    const S diff = d.csdvs ? (src - cs_buf<S>(d, *d.cs_cur)[idx]) - base : src - base;
+    const PreEmit<S> e = pre_emit_state<S>(d, idx, frame, dtype);
+    const double xv = e.xv, ln = e.ln;
+    const S lp = e.lp, diff = e.diff;
     const int cnt = d.rec[idx] >> kRecShift;
     const int mag = cnt < 0 ? -cnt : cnt, pol = cnt < 0;
     const TsParams ts = make_ts(p, c->max_n, d.refr_d);
@@ -1966,6 +2047,38 @@ __global__ void emu_probe_post_kernel(EmuDev d, int slot, ProbeDev pr) {
     if (*(volatile int32_t *)d.abort_flag) return;
     if (!d.ctrl[slot].planned) return;
     pr.out[i].base_log_frame = (double)((const S *)d.base)[pr.px[i]];
+}
+
+// Model-state planes of the frame-by-frame path, one thread per own pixel, enqueued before the emit kernel of frame
+// slot `slot` (only while states are shown), where the pre-emit probe reads the same state; it leaves when the emit
+// kernel does (abort, frame not planned), so a re-run emission writes the frame's planes again.
+template <typename S>
+__global__ void __launch_bounds__(kThreads) emu_model_state_kernel(EmuDev d, int slot, const void *frame, int dtype,
+                                                                   PlaneDev pl) {
+    if (*(volatile int32_t *)d.abort_flag) return;
+    if (!d.ctrl[slot].planned) return;
+    const int p = blockIdx.x * kThreads + threadIdx.x;
+    if (p >= pl.npx) return;
+    const int idx = pl.p0 + p;
+    const PreEmit<S> e = pre_emit_state<S>(d, idx, frame, dtype);
+    uint8_t *o = pl.out + p;
+    for (int j = 0; j < V2E_MODEL_STATES; j++) {
+        if (!((pl.mask >> j) & 1u)) continue;
+        double x;
+        switch (j) {
+            case 0: x = e.xv; break;
+            case 1: x = e.ln; break;
+            case 2: x = (double)e.lp; break;
+            case 3: x = (double)((const S *)d.hp)[idx]; break;
+            case 4: x = d.pr_noise ? (double)d.noise_arr[idx] : 0.0; break;
+            case 5: x = (double)e.sur; break;
+            case 6: x = (double)e.cms; break;
+            case 7: x = (double)e.base; break;
+            default: x = (double)e.diff; break;
+        }
+        *o = (uint8_t)state_byte(pl, j, x);
+        o += pl.npx;
+    }
 }
 
 // measurement floor: what an event bracket reports around a kernel that does nothing (v2e_emu_profile_read4)
@@ -2088,6 +2201,15 @@ struct V2eEmu {
         const void **frame;         // [max_slots] the frame each slot was counted from (the pre-emit probe reads it)
         int *dtype;                 // [max_slots]
     } probe;
+    // model-state planes (v2e_emu_set_model_states): nothing is allocated or launched while mask == 0
+    struct {
+        uint32_t mask;
+        int nst;                    // shown states
+        double lo[V2E_MODEL_STATES], span[V2E_MODEL_STATES];
+        uint8_t *planes;            // [max_slots][nst][own pixels] device
+        size_t cap;                 // bytes of planes
+        int ready;                  // frames of the last step v2e_emu_collect completed, not yet read
+    } ms;
 };
 
 thread_local char g_err[512] = "";
@@ -2103,9 +2225,9 @@ static int fail(int code, const char *fmt, const char *detail = "") {
 
 int v2e_set_error(int code, const char *fmt, const char *detail) { return fail(code, fmt, detail); }
 extern "C" const char *v2e_last_error(void) { return g_err; }
-extern "C" int v2e_version(void) { return 202; }
+extern "C" int v2e_version(void) { return 203; }
 extern "C" int v2e_abi_info(int *version, int *emu_cfg_size, int *frame_info_size, int *unet_weights_size) {
-    if (version) *version = 202;
+    if (version) *version = 203;
     if (emu_cfg_size) *emu_cfg_size = (int)sizeof(V2eEmuCfg);
     if (frame_info_size) *frame_info_size = (int)sizeof(V2eFrameInfo);
     if (unet_weights_size) *unet_weights_size = (int)sizeof(V2eUNetWeights);
@@ -2313,6 +2435,7 @@ extern "C" int v2e_emu_destroy(V2eEmu *h) {
     if (h->probe.px) cudaFree(h->probe.px);
     if (h->probe.samples) cudaFree(h->probe.samples);
     if (h->probe.host) cudaFreeHost(h->probe.host);
+    if (h->ms.planes) cudaFree(h->ms.planes);
     void *ord_ptrs[] = {h->ord.rows, h->ord.keys, h->ord.boff, h->ord.segs, h->ord.ctl};
     for (void *p : ord_ptrs) if (p) cudaFree(p);
     void *cs_ptrs[] = {d.cs_bufs, d.cs_done, h->cs_send};
@@ -2585,6 +2708,17 @@ static ProbeDev probe_dev(const V2eEmu *h, int slot0) {
     pr.slot0 = slot0;
     return pr;
 }
+// the planes' view of frame slots [slot0, ...) of the step
+static PlaneDev plane_dev(const V2eEmu *h, int slot0) {
+    PlaneDev pl;
+    pl.mask = h->ms.mask;
+    pl.nst = h->ms.nst;
+    pl.p0 = h->d.own_lo;
+    pl.npx = h->d.own_hi - h->d.own_lo;
+    pl.out = h->ms.mask ? h->ms.planes + (size_t)slot0 * pl.nst * pl.npx : nullptr;
+    for (int j = 0; j < V2E_MODEL_STATES; j++) { pl.lo[j] = h->ms.lo[j]; pl.span[j] = h->ms.span[j]; }
+    return pl;
+}
 // the frame slot `slot` is counted from: the frame-by-frame probe reads the input value there at emission time
 static void probe_note_frame(V2eEmu *h, int slot, const void *frame, int dtype) {
     h->probe.frame[slot] = frame;
@@ -2643,6 +2777,12 @@ static int enqueue_emit(V2eEmu *h, const FrameParams &p, int slot, float *events
     if (pr.n) {
         if (d.state_f64) emu_probe_pre_kernel<double><<<1, 64, 0, st>>>(d, p, slot, h->probe.frame[slot], h->probe.dtype[slot], pr);
         else emu_probe_pre_kernel<float><<<1, 64, 0, st>>>(d, p, slot, h->probe.frame[slot], h->probe.dtype[slot], pr);
+    }
+    if (h->ms.mask) {
+        const PlaneDev pl = plane_dev(h, slot);
+        const int g = (pl.npx + kThreads - 1) / kThreads;
+        if (d.state_f64) emu_model_state_kernel<double><<<g, kThreads, 0, st>>>(d, slot, h->probe.frame[slot], h->probe.dtype[slot], pl);
+        else emu_model_state_kernel<float><<<g, kThreads, 0, st>>>(d, slot, h->probe.frame[slot], h->probe.dtype[slot], pl);
     }
     {
         ProfScope ps(h, slot, 2, st);
@@ -2727,7 +2867,7 @@ static int fused_cfg() {
 }
 template <typename S, bool FAST, int WARPS, int MINB>
 static void launch_fused_update_cfg(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, size_t sm,
-                                    const ProbeDev &pr, cudaStream_t st) {
+                                    const ProbeDev &pr, const PlaneDev &pl, cudaStream_t st) {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -2735,7 +2875,10 @@ static void launch_fused_update_cfg(V2eEmu *h, const EmuDev &d, const FusedFrame
     const int min_units = 2 * WARPS;                       // small frames: at least two units per warp
     if (blocks > (d.units + min_units - 1) / min_units) blocks = (d.units + min_units - 1) / min_units;
     if (blocks < 1) blocks = 1;
-    if (pr.n)
+    if (pl.mask)
+        emu_fused_update_planes_kernel<S, FAST, WARPS, MINB><<<blocks, WARPS * 32, sm, st>>>(
+            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr, pl);
+    else if (pr.n)
         emu_fused_update_kernel<S, FAST, WARPS, MINB, true><<<blocks, WARPS * 32, sm, st>>>(
             d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr);
     else
@@ -2744,12 +2887,12 @@ static void launch_fused_update_cfg(V2eEmu *h, const EmuDev &d, const FusedFrame
 }
 template <typename S, bool FAST>
 static void launch_fused_update_f(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, size_t sm,
-                                  const ProbeDev &pr, cudaStream_t st) {
+                                  const ProbeDev &pr, const PlaneDev &pl, cudaStream_t st) {
     switch (fused_cfg()) {
-        case 0: launch_fused_update_cfg<S, FAST, 8, 3>(h, d, ff, frames, T, sm, pr, st); break;
-        case 2: launch_fused_update_cfg<S, FAST, 4, 7>(h, d, ff, frames, T, sm, pr, st); break;
-        case 3: launch_fused_update_cfg<S, FAST, 8, 2>(h, d, ff, frames, T, sm, pr, st); break;
-        default: launch_fused_update_cfg<S, FAST, 4, 5>(h, d, ff, frames, T, sm, pr, st); break;
+        case 0: launch_fused_update_cfg<S, FAST, 8, 3>(h, d, ff, frames, T, sm, pr, pl, st); break;
+        case 2: launch_fused_update_cfg<S, FAST, 4, 7>(h, d, ff, frames, T, sm, pr, pl, st); break;
+        case 3: launch_fused_update_cfg<S, FAST, 8, 2>(h, d, ff, frames, T, sm, pr, pl, st); break;
+        default: launch_fused_update_cfg<S, FAST, 4, 5>(h, d, ff, frames, T, sm, pr, pl, st); break;
     }
 }
 // frames [a, a + T) of the step (d shifted to slot a)
@@ -2760,8 +2903,9 @@ static int launch_fused_update(V2eEmu *h, const EmuDev &d, const FusedFrame *ff,
     const bool fast = sizeof(S) == 8 && d.rng_mode == 1 && d.per_pixel_thres && d.leak_on && d.shot_on;
     if (sm > 40 * 1024) return fail(V2E_E_INVALID, "fused path: too many frames per step");
     const ProbeDev pr = probe_dev(h, a);
-    if (fast) launch_fused_update_f<S, true>(h, d, ff, frames, T, sm, pr, st);
-    else launch_fused_update_f<S, false>(h, d, ff, frames, T, sm, pr, st);
+    const PlaneDev pl = plane_dev(h, a);
+    if (fast) launch_fused_update_f<S, true>(h, d, ff, frames, T, sm, pr, pl, st);
+    else launch_fused_update_f<S, false>(h, d, ff, frames, T, sm, pr, pl, st);
     return V2E_OK;
 }
 
@@ -3159,6 +3303,7 @@ extern "C" int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info, int T, int *frames
     if (!h || !info || T < 1 || T > h->d.max_slots) return fail(V2E_E_INVALID, "bad argument");
     cudaStream_t st = (cudaStream_t)stream;
     h->probe.ready = 0;             // a new step's samples replace any unread ones; set again below on V2E_OK
+    h->ms.ready = 0;
     CU(cudaMemcpyAsync(h->ctrl_host, h->d.ctrl, (size_t)(T + 1) * sizeof(FrameCtrl), cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h->abort_host, h->d.abort_flag, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -3250,6 +3395,7 @@ extern "C" int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info, int T, int *frames
     if (frames_done) *frames_done = done;
     if (rows_total) *rows_total = rows;
     h->probe.ready = (!status && h->probe.n) ? T : 0;      // every frame of the step emitted: its samples are final
+    h->ms.ready = (!status && h->ms.mask) ? T : 0;
     if (status == V2E_E_CAPACITY) return fail(V2E_E_CAPACITY, "event buffer too small");
     if (status == V2E_E_ITER_CAP) return fail(V2E_E_ITER_CAP, "a pixel exceeded iter_cap events in one frame");
     if (h->ord.mode) return order_step(h, T, st);
@@ -3290,6 +3436,63 @@ extern "C" int v2e_emu_probe_device(V2eEmu *h) {
     if (!h->probe.samples) return -1;
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, h->probe.samples) != cudaSuccess) return fail(V2E_E_CUDA, "cudaPointerGetAttributes failed");
+    return a.device;
+}
+
+extern "C" int v2e_emu_set_model_states(V2eEmu *h, uint32_t mask, const double *lo_span_host) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    if (mask >> V2E_MODEL_STATES) return fail(V2E_E_INVALID, "model states: unknown state bit");
+    if (mask && !lo_span_host) return fail(V2E_E_INVALID, "model states: lo_span_host is null");
+    if ((mask & (1u << 3)) && !h->d.scidvs) return fail(V2E_E_INVALID, "model states: scidvs_highpass needs SCIDVS");
+    if ((mask & (3u << 5)) && !h->d.csdvs)
+        return fail(V2E_E_INVALID, "model states: cs_surround_frame / c_minus_s_frame need the centre-surround model");
+    const int nst = __builtin_popcount(mask);
+    for (int j = 0; j < V2E_MODEL_STATES; j++) {
+        h->ms.lo[j] = (mask >> j & 1u) ? lo_span_host[2 * j] : 0.0;
+        h->ms.span[j] = (mask >> j & 1u) ? lo_span_host[2 * j + 1] : 1.0;
+    }
+    const size_t need = (size_t)h->d.max_slots * nst * (size_t)(h->d.own_hi - h->d.own_lo);
+    if (need > h->ms.cap) {
+        // the buffer belongs on the handle's device, whichever device is current for the caller
+        int cur = 0;
+        CU(cudaGetDevice(&cur));
+        if (cur != h->probe.device) CU(cudaSetDevice(h->probe.device));
+        if (h->ms.planes) cudaFree(h->ms.planes);
+        h->ms.cap = 0;
+        cudaError_t e = cudaMalloc((void **)&h->ms.planes, need);
+        if (e != cudaSuccess) h->ms.planes = nullptr;
+        if (cur != h->probe.device) cudaSetDevice(cur);
+        if (e != cudaSuccess) {
+            h->ms.mask = 0;
+            h->ms.nst = 0;
+            return fail(V2E_E_CUDA, "v2e_emu_set_model_states: %s", cudaGetErrorString(e));
+        }
+        h->ms.cap = need;
+    }
+    h->ms.mask = mask;
+    h->ms.nst = nst;
+    h->ms.ready = 0;
+    return V2E_OK;
+}
+
+extern "C" int v2e_emu_model_state_read(V2eEmu *h, void *dst_dev, uint64_t cap, int *n_frames, void *stream) {
+    if (!h || !n_frames) return fail(V2E_E_INVALID, "null argument");
+    const int nf = h->ms.mask ? h->ms.ready : 0;
+    const size_t bytes = (size_t)nf * h->ms.nst * (size_t)(h->d.own_hi - h->d.own_lo);
+    if (bytes > 0) {
+        if (!dst_dev || cap < bytes) return fail(V2E_E_INVALID, "model states: dst_dev too small");
+        CU(cudaMemcpyAsync(dst_dev, h->ms.planes, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    }
+    h->ms.ready = 0;
+    *n_frames = nf;
+    return V2E_OK;
+}
+
+extern "C" int v2e_emu_model_state_device(V2eEmu *h) {
+    if (!h) return fail(V2E_E_INVALID, "null handle");
+    if (!h->ms.planes) return -1;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, h->ms.planes) != cudaSuccess) return fail(V2E_E_CUDA, "cudaPointerGetAttributes failed");
     return a.device;
 }
 

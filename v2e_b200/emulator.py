@@ -33,7 +33,15 @@ formatted on the device (v2e_b200.sinks.events_to_text) and written to the write
 labels every returned row signal (1) or shot noise (0) -- `last_signnoise_label`, generate_events_batch(...,
 return_labels=True) -- and passes the labels to the text and AEDAT-2.0 sinks. A pixel-sharded emulator labels its own
 rows (generate_events_band(_batch)(..., return_labels=True)) and writes no sink: a file needs the merged stream.
-show_dvs_model_state / save_dvs_model_state (GUI probes) are ignored with a warning.
+
+show_dvs_model_state=[names] (or ['all']) captures, like the reference (emulator.py:41-50, 580-617, 756-767), every
+frame but the first: each shown state after the low-pass, noise, SCIDVS, surround and leak updates and before the
+events, scaled to its MODEL_STATE_RANGES range and cast to uint8 -- on the device, on every path (DESIGN.md 4.1).
+model_state_frames() returns the frames of the last call. No window is opened. save_dvs_model_state=True writes
+<output_folder>/<name>.avi through the reference's v2ecore.v2e_utils.video_writer with the reference's text overlay
+when that imports (a warning and no files otherwise); a sharded emulator captures its own rows and writes no file.
+Two cases where the reference fails mid-run raise ValueError here at construction: save_dvs_model_state with
+output_folder=None, and a shown name that is a state tensor without a display range (e.g. 'pos_thres').
 
 record_single_pixel_states=(a, b) records, like the reference (emulator.py:278-302, 985-1009), pixel row a, column b
 (the tuple indexes frames as frame[a, b]) after every frame: single_pixel_states, single_pixel_sample_count,
@@ -172,10 +180,11 @@ class _Sinks:
         self.h5 = self.h5_dataset = self.aedat2 = self.aedat4 = self.text = None
 
 
-def _finalize(lib, box, sinks, spx):
+def _finalize(lib, box, sinks, spx, ms_writers=None):
     """weakref.finalize callback: frees the library handle, closes the writers and saves the single-pixel recording
     of a collected (or exiting) emulator without keeping it alive (the reference registers cleanup with atexit,
     emulator.py:372)."""
+    _release_writers(ms_writers)
     h = box[0]
     box[0] = None
     if h:
@@ -187,6 +196,29 @@ def _finalize(lib, box, sinks, spx):
         sinks.close()
     if spx["pixel"] is not None and spx["owner"]:
         _save_pixel_states(spx["states"], spx["count"], spx["file"])
+
+
+def _release_writers(writers):
+    """emulator.py:424-426: the model-state video writers are released at cleanup."""
+    for w in list((writers or {}).values()):
+        try:
+            w.release()
+        except Exception:
+            pass
+    if writers:
+        writers.clear()
+
+
+# Display ranges of the model states (emulator.py:41-50): (lo, hi) built as the reference builds them, from the
+# float64 scalar np.log(255), so that lo and hi - lo are the same doubles. Keys in EventEmulator.MODEL_STATES order.
+_L255 = np.log(255)
+_GR, _LG, _SLG = (0, 255), (0, _L255), (-_L255 / 8, _L255 / 8)
+MODEL_STATE_RANGES = {'new_frame': _GR, 'log_new_frame': _LG, 'lp_log_frame': _LG, 'scidvs_highpass': _SLG,
+                      'photoreceptor_noise_arr': _SLG, 'cs_surround_frame': _LG, 'c_minus_s_frame': _SLG,
+                      'base_log_frame': _SLG, 'diff_frame': _SLG}
+# state tensors without a display range: the reference raises KeyError when asked to show one
+_NO_RANGE_TENSORS = ('pos_thres', 'neg_thres', 'noise_rate_array', 'timestamp_mem', 'scidvs_tau_arr',
+                     'scidvs_previous_photo')
 
 
 # the device's V2eProbeSample (include/v2e_b200.h) and the reference's recorded names (emulator.py:291-302)
@@ -291,9 +323,44 @@ class EventEmulator(object):
             for i in record_single_pixel_states:
                 if not (type(i) is int):
                     raise ValueError(f'--record_single_pixel_states {record_single_pixel_states} should have two integer-value pixel addresses (x,y)')
-        if show_dvs_model_state or save_dvs_model_state:
-            logger.warning("show_dvs_model_state / save_dvs_model_state are GUI probes of the reference (out of scope, "
-                           "SURVEY.md 2): ignored; the state tensors are available by the same attribute names")
+        # model-state planes (emulator.py:365-368, 580-617, 756-767): the shown states that exist in this
+        # configuration; a name that does not is logged once and skipped, as the reference does
+        self.show_dvs_model_state = None
+        self.save_dvs_model_state = save_dvs_model_state
+        self._ms_names = []
+        self._ms_chunks = []          # (frame counters, t_previous, planes [k, states, rows, W]) of the last call
+        self._ms_writers = {}         # name -> the reference's video writer
+        self._ms_video_writer = None
+        if show_dvs_model_state is not None:
+            names = list(show_dvs_model_state)
+            if len(names) == 1 and names[0] == 'all':
+                names = list(MODEL_STATE_RANGES)
+            self.show_dvs_model_state = names
+            absent = set()
+            if not scidvs:
+                absent.add('scidvs_highpass')
+            if cs_lambda_pixels is None:
+                absent.update(('cs_surround_frame', 'c_minus_s_frame'))
+            for s in names:
+                if s in self._ms_names:
+                    continue
+                if s in MODEL_STATE_RANGES and s not in absent:
+                    self._ms_names.append(s)
+                elif s in _NO_RANGE_TENSORS:
+                    raise ValueError(f"show_dvs_model_state: {s} has no display range (MODEL_STATE_RANGES)")
+                else:
+                    logger.error(f'{s} does not exist so we cannot show it')
+            if self._ms_names:
+                logger.info("show_dvs_model_state: the frames are captured on the device (model_state_frames()); "
+                            "no window is opened")
+                if save_dvs_model_state and output_folder is None:
+                    raise ValueError("save_dvs_model_state needs an output_folder for <output_folder>/<name>.avi")
+                if save_dvs_model_state and shard is None:
+                    try:
+                        from v2ecore.v2e_utils import video_writer
+                        self._ms_video_writer = video_writer
+                    except ImportError as e:
+                        logger.warning("save_dvs_model_state ignored: v2ecore.v2e_utils is not importable (%s)", e)
         # single-pixel recording (emulator.py:278-302, 985-1009): shared with the finalizer, which saves at exit
         self._spx = {"pixel": record_single_pixel_states, "count": 0, "owner": True,
                      "file": self.SINGLE_PIXEL_STATES_FILENAME, "col": None,
@@ -378,7 +445,8 @@ class EventEmulator(object):
         self.t_previous = 0
         # the reference registers cleanup with atexit (emulator.py:372), which would keep every instance alive
         # until exit; a finalizer frees the device memory when the object is collected AND runs at exit
-        self._finalizer = weakref.finalize(self, _finalize, self._lib, self._hbox, self._sinks, self._spx)
+        self._finalizer = weakref.finalize(self, _finalize, self._lib, self._hbox, self._sinks, self._spx,
+                                           self._ms_writers)
 
     @property
     def _h(self):
@@ -480,6 +548,77 @@ class EventEmulator(object):
                 self.save_recorded_single_pixel_states()
                 spx["pixel"] = None
 
+    def model_state_frames(self):
+        """show_dvs_model_state: the frames the last generate_events / generate_events_batch /
+        generate_events_band(_batch) call captured, a dict: 'frame' (the reference's frame_counter of each frame,
+        int64 [k]), 't_previous' (the previous frame's time, float64 [k]; the overlay text shows both) and, for each
+        shown state, a uint8 CUDA tensor [k, rows, W] of the bytes before the text overlay (a sharded emulator's own
+        rows)."""
+        if not self._ms_names:
+            raise RuntimeError("model_state_frames needs show_dvs_model_state with a state that exists here")
+        out = {"frame": np.array([f for c in self._ms_chunks for f in c[0]], np.int64),
+               "t_previous": np.array([t for c in self._ms_chunks for t in c[1]], np.float64)}
+        order = self._ms_order()
+        if self._ms_chunks:
+            planes = torch.cat([c[2] for c in self._ms_chunks], 0)
+        else:
+            planes = torch.zeros((0, len(order), 0, 0), dtype=torch.uint8, device=self.device)
+        for name in self._ms_names:
+            out[name] = planes[:, order.index(name)].contiguous()
+        return out
+
+    def _ms_order(self):
+        """The shown states in the device's plane order (MODEL_STATES order)."""
+        return [s for s in self.MODEL_STATES if s in self._ms_names]
+
+    def _set_model_states(self):
+        order = self._ms_order()
+        mask, ls = 0, np.zeros(2 * len(self.MODEL_STATES), np.float64)
+        for s in order:
+            i = self.MODEL_STATES.index(s)
+            lo, hi = MODEL_STATE_RANGES[s]
+            mask |= 1 << i
+            ls[2 * i], ls[2 * i + 1] = lo, hi - lo          # Python's own lo and hi - lo
+        _lib.check(self._lib.v2e_emu_set_model_states(self._h, mask, ls.ctypes.data_as(ctypes.c_void_p)))
+
+    def _drain_states(self, t_frames, fc0):
+        """After v2e_emu_collect returned V2E_OK: the planes of the step's frames (frame counters fc0, fc0 + 1, ...;
+        self.t_previous is still the time before the step's first frame)."""
+        if not self._ms_names:
+            return
+        k = len(t_frames)
+        buf = torch.empty((k, len(self._ms_names), self._own_rows, self._W), dtype=torch.uint8, device=self.device)
+        nf = ctypes.c_int(0)
+        _lib.check(self._lib.v2e_emu_model_state_read(self._h, ctypes.c_void_p(buf.data_ptr()), buf.numel(),
+                                                      ctypes.byref(nf), self._stream()))
+        if nf.value != k:
+            raise RuntimeError("model-state planes of %d frames, expected %d" % (nf.value, k))
+        fcs = list(range(fc0, fc0 + k))
+        tps = [float(self.t_previous)] + [float(t) for t in t_frames[:-1]]
+        self._ms_chunks.append((fcs, tps, buf))
+        if self._ms_video_writer is not None:
+            self._write_states(buf, fcs, tps)
+
+    def _write_states(self, buf, fcs, tps):
+        """emulator.py:598-617 for the captured bytes: the two putText calls draw 0.0 and 255.0 into the float image,
+        which the x255 uint8 cast turns into 0 and 1; drawing 0 and 1 into the bytes gives the same frame."""
+        import cv2
+        host = buf.cpu().numpy()
+        order = self._ms_order()
+        for j, (fc, tp) in enumerate(zip(fcs, tps)):
+            text = f'fr:{fc} t:{tp:.4f}s'
+            for name in self._ms_names:
+                img = np.ascontiguousarray(host[j, order.index(name)])
+                cv2.putText(img, text, org=(0, self.output_height), fontScale=1.3, color=(0, 0, 0),
+                            fontFace=cv2.FONT_HERSHEY_PLAIN, thickness=1)
+                cv2.putText(img, text, org=(1, self.output_height - 1), fontScale=1.3, color=(1, 1, 1),
+                            fontFace=cv2.FONT_HERSHEY_PLAIN, thickness=1)
+                w = self._ms_writers.get(name)
+                if w is None:
+                    w = self._ms_writers[name] = self._ms_video_writer(
+                        os.path.join(self.output_folder, name + '.avi'), self.output_height, self.output_width)
+                w.write(cv2.cvtColor(img, cv2.COLOR_GRAY2BGR))
+
     # ------------------------------------------------------------------------------------------
     def reset(self):
         """emulator.py:558-578: next frame re-initialises the per-pixel state."""
@@ -493,6 +632,7 @@ class EventEmulator(object):
 
     def cleanup(self):
         self._destroy_handle()
+        _release_writers(self._ms_writers)
         if self._sinks is not None:
             self._sinks.close()
         if self._spx["pixel"] is not None and self._spx["owner"]:     # emulator.py:425-426
@@ -601,7 +741,10 @@ class EventEmulator(object):
                 _lib.check(self._lib.v2e_emu_set_option(h, 2, 1 if self.row_order == "canonical" else 2))
             lut = _linlog_lut()
             _lib.check(self._lib.v2e_emu_set_linlog_lut(h, ctypes.c_void_p(lut.data_ptr()), self._stream()))
+            if self._ms_names:
+                self._set_model_states()
         self._H, self._W = H, W
+        self._own_rows = H if own is None else int(own[1])
         self.output_width = W if self.output_width is None else self.output_width
         self.output_height = H if self.output_height is None else self.output_height
         self._state_f64 = bool(self._lib.v2e_emu_state_is_f64(h))
@@ -695,6 +838,7 @@ class EventEmulator(object):
         t_frame = float(t_frame)
         self.frame_counter += 1
         self._frame_times([t_frame], 1)
+        self._ms_chunks = []
         fr, code = self._to_device_frames(new_frame)
         if fr.dim() != 2:
             raise ValueError("new_frame must be [height, width]")
@@ -711,7 +855,7 @@ class EventEmulator(object):
         if self.rng_mode == "replay" and (per_frame_rng or self.exact_order):
             ev = self._phase_frame(fr, code, t_frame)
         else:
-            total, _, _ = self._run_step(fr.unsqueeze(0), code, [t_frame])
+            total, _, _ = self._run_step(fr.unsqueeze(0), code, [t_frame], self.frame_counter)
             ev = self._rows_to_host(total)
         self.t_previous = t_frame
         if ev is not None and len(ev) > 0:
@@ -887,6 +1031,7 @@ class EventEmulator(object):
         else:
             _lib.check(rc)
         self._drain_probes([t_frame])
+        self._drain_states([t_frame], self.frame_counter)
         return info[0]
 
     # pixel-sharded path (SURVEY.md 8e, BASELINE config 5): this rank owns rows [y0, y1) ---------------
@@ -918,6 +1063,7 @@ class EventEmulator(object):
         t_frame = float(t_frame)
         self.frame_counter += 1
         self._frame_times([t_frame], 1)
+        self._ms_chunks = []
         fr, code = self._to_device_frames(band_frame)
         y0, y1 = self.ext_band(int(full_height))       # the band (+ halo rows for the centre-surround model)
         if fr.dim() != 2 or fr.shape[0] != y1 - y0:
@@ -1004,6 +1150,7 @@ class EventEmulator(object):
                                           self.photoreceptor_noise):
             raise RuntimeError("batched sharded operation with per-frame noise needs rng_mode='device'")
         self._want_keys = bool(return_keys)
+        self._ms_chunks = []
         try:
             return self._band_batch(band_frames, t_frames, full_height, return_device, return_labels, return_keys)
         finally:
@@ -1057,6 +1204,7 @@ class EventEmulator(object):
                     return int(done.value)
                 _lib.check(rc)
                 self._drain_probes(t_frames[a:b])
+                self._drain_states(t_frames[a:b], self.frame_counter + 1)
                 for k in range(Tc):
                     self._account(info[k])
                     offs.append(state["total"] + int(info[k].ev_base) + int(info[k].n_events))
@@ -1156,9 +1304,10 @@ class EventEmulator(object):
         self.num_events_total += int(fi.n_events)
 
     # batched path ------------------------------------------------------------------------------
-    def _run_step(self, frames_dev, code, t_frames, base_row=0):
-        """frames_dev: [T,H,W] device tensor, T <= max_frames_per_step. Appends this chunk's rows to the
-        device event buffer starting at base_row; returns (end_row, absolute offsets[T+1], shot-noise rows [T])."""
+    def _run_step(self, frames_dev, code, t_frames, fc0, base_row=0):
+        """frames_dev: [T,H,W] device tensor, T <= max_frames_per_step, of frame counters fc0, fc0 + 1, ... Appends
+        this chunk's rows to the device event buffer starting at base_row; returns (end_row, absolute offsets[T+1],
+        shot-noise rows [T])."""
         T = frames_dev.shape[0]
         L, h = self._lib, self._h
         n = self._H * self._W
@@ -1191,6 +1340,7 @@ class EventEmulator(object):
                 need = max(int(info[f].ev_base) + int(info[f].n_events) for f in range(first, T))
                 self._grow_event_buffer(max(2 * need, 2 * self._ev_dev.shape[0]), keep=base)
             self._drain_probes(t_frames)
+            self._drain_states(t_frames, fc0)
             total = int(rows.value)
             offsets = np.array([int(info[f].ev_base) for f in range(T)] + [total], np.int64)
             n_shot = np.array([int(info[f].n_shot_on) + int(info[f].n_shot_off) for f in range(T)], np.int64)
@@ -1222,6 +1372,7 @@ class EventEmulator(object):
             raise ValueError("frames must be [T, height, width]")
         T = fr.shape[0]
         t_frames = self._frame_times(t_frames, T)
+        self._ms_chunks = []
         offs, n_shot = [0], []
         start = 0
         if not self._initialized:
@@ -1233,7 +1384,7 @@ class EventEmulator(object):
         f, row = start, 0
         while f < T:
             e = min(T, f + self.max_frames_per_step)
-            row, o, s = self._run_step(fr[f:e], code, t_frames[f:e], base_row=row)
+            row, o, s = self._run_step(fr[f:e], code, t_frames[f:e], self.frame_counter + 1, base_row=row)
             offs.extend(o[1:].tolist())
             n_shot.extend(s.tolist())
             self.t_previous = t_frames[e - 1]
