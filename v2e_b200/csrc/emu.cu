@@ -27,6 +27,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/v2e_b200.h"
@@ -174,6 +175,104 @@ __device__ __forceinline__ float lin_log_eval(double x) {
     double y = (x <= 20.0) ? x * f : log(x);
     y = rint(y * 1e8) / 1e8;
     return (float)y;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Per-pixel steps of the model. Every kernel that advances a pixel, and every kernel that recomputes a pixel's state
+// for a probe or a model-state plane, calls these, so the operations and their order are written down once.
+// ---------------------------------------------------------------------------------------------
+// lin_log of an input value (emulator_utils.py:18-45): the table entry for an integer code 0..255 (every value of a
+// uint8 frame), else lin_log_eval. tab holds the float32 lin_log values, as float or widened to double.
+template <int FT, typename T> __device__ __forceinline__ T lin_log_of(const T *tab, double x) {
+    return (FT == V2E_U8 || (x >= 0.0 && x <= 255.0 && x == floor(x))) ? tab[(int)x] : (T)lin_log_eval(x);
+}
+// the intensity in [0, 1] the low-pass filter and the shot noise scale with (emulator_utils.py:48-54)
+__device__ __forceinline__ double inten01_of(double x) { return (x + 20.0) / 275.0; }
+// low-pass factor eps = inten01 * delta_time / tau, clamped at 1 (emulator_utils.py:84, 96); a NaN stays NaN, as
+// torch.clamp(max=1) leaves it
+__device__ __forceinline__ double lp_eps(double inten01, double eps_scale) {
+    const double eps = inten01 * eps_scale;
+    return eps > 1.0 ? 1.0 : eps;
+}
+// The multi-frame body's form of the same clamp, one fmin: there inten01 is that of a uint8 code (finite, > 0), so
+// eps is a number for every finite frame time and the two forms agree.
+__device__ __forceinline__ double lp_eps_code(double inten01, double eps_scale) {
+    return fmin(inten01 * eps_scale, 1.0);
+}
+// photoreceptor low-pass step (emulator_utils.py:57-109): lp' = (1-eps)*lp + eps*ln in float64. Without a low-pass
+// (or in a float32 state, which has none: cutoff_hz == 0) lp' = ln, exact: ln is a widened float32 or a raw hdr value
+// in a float64 state. EPS: the clamp (lp_eps, or lp_eps_code where inten01 is a code's).
+template <typename S, double (*EPS)(double, double) = lp_eps>
+__device__ __forceinline__ S lp_step(bool lowpass, S lp, double ln, double inten01, double eps_scale) {
+    if (sizeof(S) == 8 && lowpass) {
+        const double eps = EPS(inten01, eps_scale);
+        return (S)((1.0 - eps) * (double)lp + eps * ln);
+    }
+    return (S)ln;
+}
+// leak (emulator_utils.py:114-134): rate_nr = leak_rate_hz * noise_rate (float32, the same every frame), jittered by
+// the normal draw lr; float32 products, subtracted in the state dtype
+template <typename S>
+__device__ __forceinline__ S leak_step(S base, float rate_nr, float jit_f, float lr, float dt_f, float thp) {
+    const float rate = rate_nr * (1.0f - jit_f * lr);
+    const float delta = (dt_f * rate) * thp;
+    return base - (S)delta;
+}
+// difference (emulator.py:748-752): what the change amplifier sees minus base; with the centre-surround model the
+// photoreceptor minus the surround (c_minus_s) first
+template <typename S> __device__ __forceinline__ S diff_of(bool csdvs, S photo, S surround, S base) {
+    return csdvs ? (photo - surround) - base : photo - base;
+}
+// event count (emulator.py:757-772, emulator_utils.py:137-173): ON iff diff >= pos threshold, OFF iff -diff >= neg
+// threshold (thresholds > 0), so one magnitude a and one threshold b: the float32 threshold of the side (thp / thn),
+// or, in a float64 state with scalar thresholds, the float64 nominal one (pos_nom / neg_nom). mag is ATen's floor
+// division a // b where it is 0 / 1 / 2, computed without a branch (see div_floor_count); `deep` says it is >= 3 and
+// needs div_floor_count(a, b) itself (rare).
+template <typename S> struct EventCount {
+    S a, b;
+    int32_t mag;
+    bool neg, deep;
+};
+template <typename S>
+__device__ __forceinline__ EventCount<S> event_count(S diff, float thp, float thn, bool scalar_thres, double pos_nom,
+                                                     double neg_nom) {
+    EventCount<S> c;
+    c.neg = diff < (S)0;
+    c.a = c.neg ? -diff : diff;
+    const float thf = c.neg ? thn : thp;
+    if (sizeof(S) == 8 && scalar_thres) c.b = (S)(c.neg ? neg_nom : pos_nom);
+    else c.b = (S)thf;
+    const S b2 = c.b + c.b;
+    const int ge2 = c.a >= b2;
+    c.mag = (int)(c.a >= c.b) + ge2;
+    c.deep = ge2 && !(c.a - b2 < c.b);
+    return c;
+}
+// shot-noise flags of one pixel (emulator_utils.py:323-349): bit0 ON, bit1 OFF
+__device__ __forceinline__ int shot_flags(double shot_inten_m1, int per_pixel_thres, double pos_nom, double neg_nom,
+                                          double shot_c, double x, float rnd, float thp, float thn) {
+    double factor = shot_c * (shot_inten_m1 * inten01_of(x) + 1.0);
+    double pre_on, pre_off;
+    if (per_pixel_thres) {
+        pre_on = (double)((float)pos_nom / thp);         // emulator.py:475-478, float32 tensor
+        pre_off = (double)((float)neg_nom / thn);
+    } else {
+        pre_on = (double)(float)(pos_nom / pos_nom);     // torch.div of two Python floats
+        pre_off = (double)(float)(neg_nom / neg_nom);
+    }
+    double r = (double)rnd;
+    int on = r > 1.0 - factor * pre_on;
+    int off = r < factor * pre_off;
+    return on | (off << 1);
+}
+// base after the emission (emulator.py:936-942): count events of threshold th move it (int32 * float32 -> float32,
+// then the state dtype), a shot-noise event resets it to lp. Selects, not branches: x + 0.0 would turn a -0.0 into
+// +0.0, and x - p == x + (-p) exactly.
+template <typename S> __device__ __forceinline__ S base_after(S base, int count, float th, bool neg, int flags, S lp) {
+    const S prod = (S)((float)count * th);
+    const S moved = base + (neg ? -prod : prod);
+    const S b = count ? moved : base;
+    return flags ? lp : b;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -328,28 +427,59 @@ __device__ __forceinline__ void st4(double *p, int i, const double v[4]) {
     *(double2 *)(p + i + 2) = make_double2(v[2], v[3]);
 }
 
-// shot-noise flags of one pixel (emulator_utils.py:323-349): bit0 ON, bit1 OFF
-__device__ __forceinline__ int shot_flags(const EmuDev &d, double shot_c, double x, float rnd,
-                                          float thp, float thn) {
-    double inten01 = (x + 20.0) / 275.0;
-    double factor = shot_c * (d.shot_inten_m1 * inten01 + 1.0);
-    double pre_on, pre_off;
-    if (d.per_pixel_thres) {
-        pre_on = (double)((float)d.pos_nom / thp);       // emulator.py:475-478, float32 tensor
-        pre_off = (double)((float)d.neg_nom / thn);
-    } else {
-        pre_on = (double)(float)(d.pos_nom / d.pos_nom); // torch.div of two Python floats
-        pre_off = (double)(float)(d.neg_nom / d.neg_nom);
-    }
-    double r = (double)rnd;
-    int on = r > 1.0 - factor * pre_on;
-    int off = r < factor * pre_off;
-    return on | (off << 1);
-}
-
 // ---------------------------------------------------------------------------------------------
 // emission plan: run by the last block of the last counting kernel of a frame
 // ---------------------------------------------------------------------------------------------
+// Exclusive row offsets of up to 64 (iteration, polarity) segments h[0, nseg) by one warp, two segments per lane
+// (iteration `lane`, ON and OFF), shuffle scan. Every lane gets the signal rows of the frame (sig) and the ON ones.
+__device__ __forceinline__ void warp_seg_scan(const uint32_t *h, uint32_t *off, int nseg, int lane, uint32_t &sig,
+                                              uint32_t &sig_on) {
+    const int s0 = 2 * lane, s1 = 2 * lane + 1;
+    const uint32_t v0 = s0 < nseg ? h[s0] : 0u, v1 = s1 < nseg ? h[s1] : 0u;
+    uint32_t incl = v0 + v1;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    const uint32_t excl = incl - (v0 + v1);
+    if (s0 < nseg) off[s0] = excl;
+    if (s1 < nseg) off[s1] = excl + v0;
+    sig = __shfl_sync(0xffffffffu, incl, 31);
+    sig_on = __reduce_add_sync(0xffffffffu, v0);
+}
+// A frame's counters once its signal segments are laid out (sig rows, sig_on of them ON): the shot rows follow them,
+// ON then OFF (their counts sit at the end of the histogram hs). Returns the frame's rows.
+__device__ __forceinline__ uint32_t write_frame_counts(const EmuDev &d, FrameCtrl *c, const uint32_t *hs, uint32_t *off,
+                                                       uint32_t sig, uint32_t sig_on, int filter_active) {
+    const uint32_t shot_on = hs[2 * d.iter_cap], shot_off = hs[2 * d.iter_cap + 1];
+    off[2 * d.iter_cap] = sig;
+    off[2 * d.iter_cap + 1] = sig + shot_on;
+    const uint32_t total = sig + shot_on + shot_off;
+    c->filter_active = filter_active;
+    c->n_on = sig_on + shot_on;
+    c->n_off = (sig - sig_on) + shot_off;
+    c->n_shot_on = shot_on;
+    c->n_shot_off = shot_off;
+    c->n_events = total;
+    return total;
+}
+// plan_frame's end (one thread): counters, then the capacity check; the next frame continues after this one's rows
+__device__ __forceinline__ void plan_frame_tail(const EmuDev &d, const FrameParams &p, int slot, const uint32_t *hs,
+                                                uint32_t *off, uint32_t sig, uint32_t sig_on, int filter_active) {
+    FrameCtrl *c = d.ctrl + slot;
+    const uint32_t total = write_frame_counts(d, c, hs, off, sig, sig_on, filter_active);
+    const uint64_t base = c->ev_base;
+    if (base + total > p.capacity) {
+        if (atomicCAS(d.abort_flag, 0, V2E_E_CAPACITY) == 0) d.abort_flag[1] = slot;
+    } else {
+        d.ctrl[slot + 1].ev_base = base + total;
+        *d.chain_base = base + total;
+        c->planned = 1;
+    }
+    __threadfence();
+}
+
 __device__ void plan_frame(const EmuDev &d, const FrameParams &p, int slot) {
     __shared__ uint32_t s_part[kThreads];
     __shared__ uint32_t s_tot[2];
@@ -366,43 +496,13 @@ __device__ void plan_frame(const EmuDev &d, const FrameParams &p, int slot) {
     const uint32_t *hs = d.hist_pre + (size_t)slot * d.seg_stride;     // shot counters live at the end
     uint32_t *off = d.segoff + (size_t)slot * d.seg_stride;
     const int nseg = 2 * max_n;
+    const int filter_active = ts.filter_active && d.refr_on;
     if (nseg <= 64) {
-        // the usual case (a handful of iterations): one warp, two segments per lane, shuffle scan
+        // the usual case (a handful of iterations): one warp
         if (tid >= 32) return;
-        const int s0 = 2 * tid, s1 = 2 * tid + 1;           // (iteration tid, ON) and (iteration tid, OFF)
-        const uint32_t v0 = s0 < nseg ? h[s0] : 0u, v1 = s1 < nseg ? h[s1] : 0u;
-        uint32_t incl = v0 + v1;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (tid >= o) incl += t;
-        }
-        const uint32_t excl = incl - (v0 + v1);
-        if (s0 < nseg) off[s0] = excl;
-        if (s1 < nseg) off[s1] = excl + v0;
-        const uint32_t sig = __shfl_sync(0xffffffffu, incl, 31);
-        const uint32_t sig_on = __reduce_add_sync(0xffffffffu, v0);
-        if (tid == 0) {
-            const uint32_t shot_on = hs[2 * d.iter_cap], shot_off = hs[2 * d.iter_cap + 1];
-            off[2 * d.iter_cap] = sig;
-            off[2 * d.iter_cap + 1] = sig + shot_on;
-            const uint32_t total = sig + shot_on + shot_off;
-            c->filter_active = ts.filter_active && d.refr_on;
-            c->n_on = sig_on + shot_on;
-            c->n_off = (sig - sig_on) + shot_off;
-            c->n_shot_on = shot_on;
-            c->n_shot_off = shot_off;
-            c->n_events = total;
-            const uint64_t base = c->ev_base;
-            if (base + total > p.capacity) {
-                if (atomicCAS(d.abort_flag, 0, V2E_E_CAPACITY) == 0) d.abort_flag[1] = slot;
-            } else {
-                d.ctrl[slot + 1].ev_base = base + total;
-                *d.chain_base = base + total;
-                c->planned = 1;
-            }
-            __threadfence();
-        }
+        uint32_t sig, sig_on;
+        warp_seg_scan(h, off, nseg, tid, sig, sig_on);
+        if (tid == 0) plan_frame_tail(d, p, slot, hs, off, sig, sig_on, filter_active);
         return;
     }
     const int per = (nseg + kThreads - 1) / kThreads;
@@ -436,30 +536,19 @@ __device__ void plan_frame(const EmuDev &d, const FrameParams &p, int slot) {
         }
     }
     __syncthreads();
-    if (tid == 0) {
-        uint32_t sig = s_part[kThreads - 1];
-        uint32_t sig_on = s_tot[0];
-        uint32_t shot_on = hs[2 * d.iter_cap], shot_off = hs[2 * d.iter_cap + 1];
-        off[2 * d.iter_cap] = sig;
-        off[2 * d.iter_cap + 1] = sig + shot_on;
-        uint32_t total = sig + shot_on + shot_off;
-        c->filter_active = ts.filter_active && d.refr_on;
-        c->n_on = sig_on + shot_on;
-        c->n_off = (sig - sig_on) + shot_off;
-        c->n_shot_on = shot_on;
-        c->n_shot_off = shot_off;
-        c->n_events = total;
-        uint64_t base = c->ev_base;
-        if (base + total > p.capacity) {
-            if (atomicCAS(d.abort_flag, 0, V2E_E_CAPACITY) == 0) d.abort_flag[1] = slot;
-        } else {
-            d.ctrl[slot + 1].ev_base = base + total;
-            *d.chain_base = base + total;
-            c->planned = 1;
-        }
-        __threadfence();
-    }
+    if (tid == 0) plan_frame_tail(d, p, slot, hs, off, s_part[kThreads - 1], s_tot[0], filter_active);
 }
+
+// Histogram of a frame's rows by (iteration, polarity) segment, 2 * it + (OFF). A block adds into its shared-memory
+// bins for the first kSegSmem segments and straight into the frame's histogram beyond; bins kSegSmem and kSegSmem + 1
+// of a block count its ON / OFF shot rows.
+// lane 0: the lanes of the warp whose event of iteration `it` counts (ON / OFF ballots)
+__device__ __forceinline__ void seg_add(uint32_t *s_hist, uint32_t *hist, int it, unsigned on, unsigned off) {
+    if (on) { if (2 * it < kSegSmem) atomicAdd(&s_hist[2 * it], __popc(on)); else atomicAdd(&hist[2 * it], __popc(on)); }
+    if (off) { if (2 * it + 1 < kSegSmem) atomicAdd(&s_hist[2 * it + 1], __popc(off)); else atomicAdd(&hist[2 * it + 1], __popc(off)); }
+}
+// the frame's segment of block bin i
+__device__ __forceinline__ int bin_seg(const EmuDev &d, int i) { return i < kSegSmem ? i : 2 * d.iter_cap + (i - kSegSmem); }
 
 __device__ __forceinline__ bool last_block(uint32_t *ticket) {
     __shared__ int s_last;
@@ -488,25 +577,14 @@ __global__ void __launch_bounds__(kThreads) emu_first_frame_kernel(EmuDev d, Fra
     S su[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) {
-        double xv = x[k];
-        float lnf = 0.f;
-        if (!d.hdr) lnf = (FT == V2E_U8 || (xv >= 0.0 && xv <= 255.0 && xv == floor(xv))) ? s_lut[(int)xv] : lin_log_eval(xv);
-        if (sizeof(S) == 8) {
-            double ln = d.hdr ? xv : (double)lnf;
-            double v = ln;
-            if (d.lowpass_on) {
-                double eps = ((xv + 20.0) / 275.0) * p.eps_scale;
-                if (eps > 1.0) eps = 1.0;
-                v = (1.0 - eps) * ln + eps * ln;      // lp seeded with log_new, still filtered once
-            }
-            lp[k] = (S)v;
-            su[k] = (S)v;
-            base[k] = (S)(d.csdvs ? v - v : v);      // emulator.py:714
-        } else {
-            lp[k] = (S)lnf;
-            su[k] = (S)lnf;
-            base[k] = (S)(d.csdvs ? lnf - lnf : lnf);
-        }
+        const double xv = x[k];
+        // (hdr implies a float64 state)
+        const double ln = (sizeof(S) == 8 && d.hdr) ? xv : (double)lin_log_of<FT>(s_lut, xv);
+        // lp seeded with log_new, still filtered once
+        const S v = lp_step<S>(d.lowpass_on, (S)ln, ln, inten01_of(xv), p.eps_scale);
+        lp[k] = v;
+        su[k] = v;
+        base[k] = d.csdvs ? v - v : v;               // emulator.py:714
         tm[k] = 0.0f - d.refr_f;                     // emulator.py:508-511
     }
     st4((S *)d.lp, i0, lp);
@@ -540,16 +618,8 @@ __global__ void __launch_bounds__(kThreads) emu_lp_kernel(EmuDev d, FrameParams 
 #pragma unroll
     for (int k = 0; k < 4; k++) {
         const double xv = x[k];
-        double ln;
-        if (d.hdr) ln = xv;
-        else ln = (double)((FT == V2E_U8 || (xv >= 0.0 && xv <= 255.0 && xv == floor(xv))) ? s_lut[(int)xv] : lin_log_eval(xv));
-        if (sizeof(S) == 8 && d.lowpass_on) {
-            double eps = ((xv + 20.0) / 275.0) * p.eps_scale;
-            if (eps > 1.0) eps = 1.0;
-            lp[k] = (S)((1.0 - eps) * (double)lp[k] + eps * ln);
-        } else {
-            lp[k] = (S)ln;                          // float32 state: exact, ln is a widened float32
-        }
+        const double ln = d.hdr ? xv : (double)lin_log_of<FT>(s_lut, xv);
+        lp[k] = lp_step<S>(d.lowpass_on, lp[k], ln, inten01_of(xv), p.eps_scale);
     }
     st4((S *)d.lp, i0, lp);
 }
@@ -757,20 +827,8 @@ __global__ void __launch_bounds__(kThreads) emu_front_kernel(EmuDev d, FramePara
     for (int k = 0; k < 4; k++) {
         const double xv = x[k];
         if (!lp_done) {
-            float lnf = 0.f;
-            if (!d.hdr) lnf = (FT == V2E_U8 || (xv >= 0.0 && xv <= 255.0 && xv == floor(xv))) ? s_lut[(int)xv] : lin_log_eval(xv);
-            if (sizeof(S) == 8) {
-                const double ln = d.hdr ? xv : (double)lnf;
-                if (d.lowpass_on) {
-                    double eps = ((xv + 20.0) / 275.0) * p.eps_scale;
-                    if (eps > 1.0) eps = 1.0;
-                    lp[k] = (S)((1.0 - eps) * (double)lp[k] + eps * ln);
-                } else {
-                    lp[k] = (S)ln;
-                }
-            } else {
-                lp[k] = (S)lnf;
-            }
+            const double ln = d.hdr ? xv : (double)lin_log_of<FT>(s_lut, xv);
+            lp[k] = lp_step<S>(d.lowpass_on, lp[k], ln, inten01_of(xv), p.eps_scale);
         }
         // photoreceptor noise (emulator.py:694-701; emulator_utils.py:96-99 with a scalar eps, no clamp)
         if (d.pr_noise) {
@@ -855,15 +913,6 @@ __device__ __forceinline__ void mbar_expect_tx_pred(uint32_t bar, uint32_t bytes
                  "@q mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes), "r"(leader) : "memory");
 }
 
-// event count |diff| // threshold with ATen's floor division (div_floor_count above), the common results
-// 0 / 1 / 2 without a branch: a = |diff| >= 0, b > 0
-template <typename S> __device__ __forceinline__ int32_t div_floor_count_fast(S a, S b) {
-    const S b2 = b + b;
-    int32_t cnt = (int32_t)(a >= b) + (int32_t)(a >= b2);
-    if (a >= b2 && !(a - b2 < b)) cnt = div_floor_count<S>(a, b);     // >= 3 events: rare
-    return cnt;
-}
-
 template <typename S, int FT, int RNG, bool FAST>
 __global__ void __launch_bounds__(kThreads, 3)
 emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_randn,
@@ -924,11 +973,10 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
     if (tid == 0) { s_act_total = 0; s_max = 0; }
     {
         const double ln = (double)lut_v;
-        const double inten01 = ((double)tid + 20.0) / 275.0;
+        const double inten01 = inten01_of((double)tid);
         if (tab) {
-            double eps = inten01 * p.eps_scale;          // emulator_utils.py:84
-            if (eps > 1.0) eps = 1.0;                    // :96
-            s_ta[tid] = 1.0 - eps;                       // :99 (1-eps)
+            const double eps = lp_eps(inten01, p.eps_scale);
+            s_ta[tid] = 1.0 - eps;                       // emulator_utils.py:99 (1-eps)
             s_tb[tid] = eps * ln;                        //     eps*log_new_frame
         } else {
             s_ta[tid] = ln;
@@ -1028,41 +1076,20 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
                     if (tab) {
                         lp[k] = (S)(s_ta[code] * (double)lp[k] + s_tb[code]);
                     } else {
-                        double ln;                           // float32 lin_log value, widened (or raw if hdr)
-                        if (f_hdr) ln = xv;
-                        else ln = is_code ? s_ta[code] : (double)lin_log_eval(xv);
-                        if (sizeof(S) == 8 && f_lp) {
-                            double inten01 = is_code ? s_tb[code] : (xv + 20.0) / 275.0;
-                            double eps = inten01 * p.eps_scale;
-                            if (eps > 1.0) eps = 1.0;
-                            lp[k] = (S)((1.0 - eps) * (double)lp[k] + eps * ln);
-                        } else {
-                            lp[k] = (S)ln;                   // float32 state: exact, ln is a widened float32
-                        }
+                        // float32 lin_log value, widened (or raw if hdr); a uint8 frame's value is its code
+                        const double ln = f_hdr ? xv : lin_log_of<FT>(s_ta, FT == V2E_U8 ? (double)code : xv);
+                        // (a float32 state has no low-pass: its inten01 table is not read)
+                        const double inten01 = sizeof(S) == 8 ? (is_code ? s_tb[code] : inten01_of(xv)) : 0.0;
+                        lp[k] = lp_step<S>(f_lp, lp[k], ln, inten01, p.eps_scale);
                     }
                 }
-                // leak (emulator_utils.py:114-134): float32 products, subtract in S
-                if (f_leak) {
-                    float rate = (d.leak_rate_f * nr[k]) * (1.0f - d.leak_jit_f * lr[k]);
-                    float delta = (p.dt_f * rate) * thp[k];
-                    base[k] = base[k] - (S)delta;
-                }
-                // difference and event counts (emulator.py:748-772, emulator_utils.py:137-173)
-                S diff;
-                // centre-surround: c_minus_s = photoreceptor - surround, diff = c_minus_s - base (emulator.py:751-752)
-                if (f_cs) diff = (lp[k] - su[k]) - base[k];
-                else diff = lp[k] - base[k];
-                S tp, tn;
-                if (sizeof(S) == 8 && !f_pp) { tp = (S)d.pos_nom; tn = (S)d.neg_nom; }
-                else { tp = (S)thp[k]; tn = (S)thn[k]; }
-                // ON iff diff >= tp, OFF iff -diff >= tn (thresholds > 0): one magnitude, one threshold.
-                // Results 0 / 1 / 2 of ATen's floor division without a branch (see div_floor_count)
-                const bool neg = diff < (S)0;
-                const S a = neg ? -diff : diff, b = neg ? tn : tp, b2 = b + b;
-                const int ge1 = a >= b, ge2 = a >= b2;
-                int32_t mag = ge1 + ge2;
-                if (ge2 && !(a - b2 < b)) {                  // >= 3 events: rare
-                    mag = div_floor_count<S>(a, b);
+                if (f_leak) base[k] = leak_step<S>(base[k], d.leak_rate_f * nr[k], d.leak_jit_f, lr[k], p.dt_f, thp[k]);
+                const S diff = diff_of<S>(f_cs, lp[k], su[k], base[k]);
+                const EventCount<S> ec = event_count<S>(diff, thp[k], thn[k], !f_pp, d.pos_nom, d.neg_nom);
+                const bool neg = ec.neg;
+                int32_t mag = ec.mag;
+                if (ec.deep) {                               // >= 3 events: rare
+                    mag = div_floor_count<S>(ec.a, ec.b);
                     // before the clamps: the plan reports > iter_cap. Own pixels only (not the halo rows of a
                     // sharded centre-surround handle, nor the padding after the frame's last pixel)
                     if (i0 + k >= d.own_lo && i0 + k < d.own_hi) {
@@ -1096,7 +1123,8 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
                     if ((i0 + k) < d.n && cand[k]) {
                         const float r = RNG == 1 ? shot_uniform(d.seed, (g0 + k) >> 2, p.frame_index, (int)((g0 + k) & 3u), pref[k])
                                                  : sr[k];
-                        const int flags = shot_flags(d, p.shot_c, xv, r, thp[k], thn[k]);
+                        const int flags = shot_flags(d.shot_inten_m1, d.per_pixel_thres, d.pos_nom, d.neg_nom, p.shot_c,
+                                                     xv, r, thp[k], thn[k]);
                         flg[k] = flags;
                         recs[k] = (short)(recs[k] | flags);
                     }
@@ -1158,10 +1186,7 @@ emu_update_kernel(EmuDev d, FrameParams p, const void *frame, const float *leak_
                     for (int it = 2; it < wmax; it++) {
                         unsigned on = __ballot_sync(0xffffffffu, mags[k] > it && !pols[k]);
                         unsigned off = __ballot_sync(0xffffffffu, mags[k] > it && pols[k]);
-                        if (lane == 0) {
-                            if (on) { if (2 * it < kSegSmem) atomicAdd(&s_hist[2 * it], __popc(on)); else atomicAdd(&hist[2 * it], __popc(on)); }
-                            if (off) { if (2 * it + 1 < kSegSmem) atomicAdd(&s_hist[2 * it + 1], __popc(off)); else atomicAdd(&hist[2 * it + 1], __popc(off)); }
-                        }
+                        if (lane == 0) seg_add(s_hist, hist, it, on, off);
                     }
                 }
             }
@@ -1207,6 +1232,52 @@ __device__ __forceinline__ int warp_walk(int mag, int pol, const TsParams &ts, b
     return fin;
 }
 
+// Row writer of the emission kernels (emu_emit_kernel, emu_fused_emit_kernel). A block claims its rows of every
+// (iteration, polarity) segment below kSegSmem and of the two shot segments in one piece: s_base[i] is the first row of
+// block bin i, s_cnt[i] the rows of it handed out so far. Rows of a segment beyond kSegSmem are claimed warp by warp
+// from the frame's cursor.
+// lane 0: `count` consecutive rows of block bin `bin` (bin >= 0), else of frame segment `seg`
+__device__ __forceinline__ uint32_t claim_rows(const uint32_t *s_base, uint32_t *s_cnt, const uint32_t *segoff,
+                                               uint32_t *cursor, int bin, int seg, unsigned count) {
+    if (bin >= 0) return s_base[bin] + atomicAdd(&s_cnt[bin], count);
+    return segoff[seg] + atomicAdd(&cursor[seg], count);
+}
+// the rows of iteration `it` at time t (a warp_walk step): lane 0 claims the warp's ON and OFF rows through
+// claim(bin, seg, count), every lane whose event passes writes its row
+template <typename C>
+__device__ __forceinline__ void write_iter_rows(C &&claim, float4 *events, uint64_t ev_base, int lane, unsigned lt_mask,
+                                                int it, float t, unsigned on, unsigned off, bool pass, int neg,
+                                                float fx, float fy, float pv) {
+    uint32_t b_on = 0, b_off = 0;
+    if (lane == 0) {
+        if (on) b_on = claim(2 * it < kSegSmem ? 2 * it : -1, 2 * it, __popc(on));
+        if (off) b_off = claim(2 * it + 1 < kSegSmem ? 2 * it + 1 : -1, 2 * it + 1, __popc(off));
+    }
+    b_on = __shfl_sync(0xffffffffu, b_on, 0);
+    b_off = __shfl_sync(0xffffffffu, b_off, 0);
+    if (pass) {
+        const uint64_t row = ev_base + (neg ? b_off + __popc(off & lt_mask) : b_on + __popc(on & lt_mask));
+        events[row] = make_float4(t, fx, fy, pv);
+    }
+}
+// the shot-noise rows of the warp (flags: bit0 ON, bit1 OFF), all at the frame's last timestamp (emulator.py:906-942)
+template <typename C>
+__device__ __forceinline__ void write_shot_rows(C &&claim, float4 *events, uint64_t ev_base, int lane, unsigned lt_mask,
+                                                int flags, float ts_last, float fx, float fy) {
+    const unsigned son = __ballot_sync(0xffffffffu, flags & 1), soff = __ballot_sync(0xffffffffu, flags & 2);
+    if (son | soff) {
+        uint32_t b_on = 0, b_off = 0;
+        if (lane == 0) {
+            if (son) b_on = claim(kSegSmem, 0, __popc(son));
+            if (soff) b_off = claim(kSegSmem + 1, 0, __popc(soff));
+        }
+        b_on = __shfl_sync(0xffffffffu, b_on, 0);
+        b_off = __shfl_sync(0xffffffffu, b_off, 0);
+        if (flags & 1) events[ev_base + b_on + __popc(son & lt_mask)] = make_float4(ts_last, fx, fy, 1.0f);
+        if (flags & 2) events[ev_base + b_off + __popc(soff & lt_mask)] = make_float4(ts_last, fx, fy, -1.0f);
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // filter-count kernel (only when refractory_period_s > 0): filtered histogram over the active-pixel
 // list, no state writes
@@ -1243,10 +1314,7 @@ emu_filter_kernel(EmuDev d, FrameParams p, int slot, int do_plan) {
                 if (mag) tm = d.tmem[idx];
             }
             warp_walk(mag, pol, ts, true, d.refr_f, tm, [&](int it, float, unsigned on, unsigned off, bool) {
-                if (lane == 0) {
-                    if (on) { if (2 * it < kSegSmem) atomicAdd(&s_hist[2 * it], __popc(on)); else atomicAdd(&hist[2 * it], __popc(on)); }
-                    if (off) { if (2 * it + 1 < kSegSmem) atomicAdd(&s_hist[2 * it + 1], __popc(off)); else atomicAdd(&hist[2 * it + 1], __popc(off)); }
-                }
+                if (lane == 0) seg_add(s_hist, hist, it, on, off);
             });
         }
         __syncthreads();
@@ -1283,7 +1351,8 @@ emu_shot_kernel(EmuDev d, FrameParams p, const void *frame, const float *shot_ra
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             if (i0 + k >= d.own_hi || i0 + k < d.own_lo) continue;
-            int flags = shot_flags(d, p.shot_c, x[k], sr[k], thp[k], thn[k]);
+            int flags = shot_flags(d.shot_inten_m1, d.per_pixel_thres, d.pos_nom, d.neg_nom, p.shot_c, x[k], sr[k],
+                                   thp[k], thn[k]);
             if (flags) {
                 const short old = d.rec[i0 + k];
                 if (old == 0) {
@@ -1329,9 +1398,8 @@ emu_emit_kernel(EmuDev d, FrameParams p, int slot, float4 *events) {
     const uint64_t ev_base = c->ev_base;
     const uint32_t *seg_cnt = d.act_count + (size_t)slot * d.n_blocks;
     // lane 0 claims `count` consecutive rows of segment `seg` for this warp
-    auto claim = [&](int seg_smem, int seg, unsigned count) -> uint32_t {
-        if (seg_smem >= 0) return s_base[seg_smem] + atomicAdd(&s_cnt[seg_smem], count);
-        return segoff[seg] + atomicAdd(&cursor[seg], count);
+    auto claim = [&](int bin, int seg, unsigned count) {
+        return claim_rows(s_base, s_cnt, segoff, cursor, bin, seg, count);
     };
     for (int sg = blockIdx.x; sg < d.n_blocks; sg += gridDim.x)
     for (uint32_t base = 0, n_act = seg_cnt[sg]; base < n_act; base += kThreads) {
@@ -1374,7 +1442,7 @@ emu_emit_kernel(EmuDev d, FrameParams p, int slot, float4 *events) {
         if (tid < kSegSmem + 2) {
             const uint32_t n = s_cnt[tid];
             if (n) {
-                const int seg = tid < kSegSmem ? tid : 2 * d.iter_cap + (tid - kSegSmem);
+                const int seg = bin_seg(d, tid);
                 s_base[tid] = segoff[seg] + atomicAdd(&cursor[seg], n);
             }
             s_cnt[tid] = 0;
@@ -1387,38 +1455,11 @@ emu_emit_kernel(EmuDev d, FrameParams p, int slot, float4 *events) {
             float tm = tm0;
             const int fin = warp_walk(mag, pol, ts, filter, d.refr_f, tm,
                                       [&](int it, float t, unsigned on, unsigned off, bool pass) {
-                uint32_t b_on = 0, b_off = 0;
-                if (lane == 0) {
-                    if (on) b_on = claim(2 * it < kSegSmem ? 2 * it : -1, 2 * it, __popc(on));
-                    if (off) b_off = claim(2 * it + 1 < kSegSmem ? 2 * it + 1 : -1, 2 * it + 1, __popc(off));
-                }
-                b_on = __shfl_sync(0xffffffffu, b_on, 0);
-                b_off = __shfl_sync(0xffffffffu, b_off, 0);
-                if (pass) {
-                    const uint64_t row = ev_base + (pol ? b_off + __popc(off & lt_mask) : b_on + __popc(on & lt_mask));
-                    events[row] = make_float4(t, fx, fy, pv);
-                }
+                write_iter_rows(claim, events, ev_base, lane, lt_mask, it, t, on, off, pass, pol, fx, fy, pv);
             });
             if (filter && fin) d.tmem[idx] = tm;
-            if (fin || flags) {
-                S b = b0;
-                const float prod = (float)fin * th;      // int32*float32 -> float32 (emulator.py:936-937)
-                if (pol) b = b - (S)prod; else b = b + (S)prod;
-                if (flags) b = lpv;                      // emulator.py:940-942
-                ((S *)d.base)[idx] = b;
-            }
-            const unsigned son = __ballot_sync(0xffffffffu, flags & 1), soff = __ballot_sync(0xffffffffu, flags & 2);
-            if (son | soff) {
-                uint32_t b_on = 0, b_off = 0;
-                if (lane == 0) {
-                    if (son) b_on = claim(kSegSmem, 0, __popc(son));
-                    if (soff) b_off = claim(kSegSmem + 1, 0, __popc(soff));
-                }
-                b_on = __shfl_sync(0xffffffffu, b_on, 0);
-                b_off = __shfl_sync(0xffffffffu, b_off, 0);
-                if (flags & 1) events[ev_base + b_on + __popc(son & lt_mask)] = make_float4(ts_last, fx, fy, 1.0f);
-                if (flags & 2) events[ev_base + b_off + __popc(soff & lt_mask)] = make_float4(ts_last, fx, fy, -1.0f);
-            }
+            if (fin || flags) ((S *)d.base)[idx] = base_after<S>(b0, fin, th, pol, flags, lpv);
+            write_shot_rows(claim, events, ev_base, lane, lt_mask, flags, ts_last, fx, fy);
         }
         __syncthreads();
     }
@@ -1445,8 +1486,8 @@ emu_emit_kernel(EmuDev d, FrameParams p, int slot, float4 *events) {
 //           the untouched state (v2e_emu_collect does that itself for v2e_emu_step).
 //   emit   (emu_fused_emit_kernel): records -> packed rows with the frame's linspace timestamps.
 //   commit (emu_fused_commit_kernel): alternate lp / base -> the handle's state.
-// Arithmetic per pixel and frame is the update + emit kernels' (same operations in the same order), so the rows,
-// counters and state equal the per-frame path's bit for bit (tests/test_emulator_gpu.py).
+// Arithmetic per pixel and frame is the update + emit kernels' (the same per-pixel step and plan helpers), so the
+// rows, counters and state equal the per-frame path's bit for bit (tests/test_emulator_gpu.py).
 // =============================================================================================
 struct FusedFrame {                     // what pass 1 needs of one frame
     double eps_scale, shot_c;
@@ -1474,12 +1515,7 @@ __device__ __noinline__ int fused_shot_flags(uint64_t seed, double shot_inten_m1
                                              double neg_nom, double shot_c, uint32_t gpx, uint32_t frame_index,
                                              uint32_t pref, int code, float thp, float thn) {
     const float r = shot_uniform(seed, gpx >> 2, frame_index, (int)(gpx & 3u), pref);
-    EmuDev dd;
-    dd.shot_inten_m1 = shot_inten_m1;
-    dd.per_pixel_thres = per_pixel_thres;
-    dd.pos_nom = pos_nom;
-    dd.neg_nom = neg_nom;
-    return shot_flags(dd, shot_c, (double)code, r, thp, thn);
+    return shot_flags(shot_inten_m1, per_pixel_thres, pos_nom, neg_nom, shot_c, (double)code, r, thp, thn);
 }
 
 // frame bytes of a quad that is not 4-byte aligned in its frame, or crosses the end of the frame
@@ -1540,7 +1576,7 @@ fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint
         const uint4 *src = (const uint4 *)ff;
         uint4 *dst = (uint4 *)s_dyn;
         for (int i = tid; i < T * 2; i += WARPS * 32) dst[i] = src[i];
-        for (int i = tid; i < 256; i += WARPS * 32) s_tab[i] = make_double2((double)d.lut[i], ((double)i + 20.0) / 275.0);
+        for (int i = tid; i < 256; i += WARPS * 32) s_tab[i] = make_double2((double)d.lut[i], inten01_of((double)i));
     }
     __syncthreads();
     if (*(volatile int32_t *)d.abort_flag) return;
@@ -1608,22 +1644,10 @@ fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int code = (int)((codes >> (8 * k)) & 0xffu);
-                // photoreceptor low-pass (emulator_utils.py:57-109)
                 const double2 tb = s_tab[code];
-                if (f_lp) {
-                    const double eps = fmin(tb.y * eps_scale, 1.0);             // clamp(max=1), eps is never NaN
-                    lp[k] = (S)((1.0 - eps) * (double)lp[k] + eps * tb.x);
-                } else {
-                    lp[k] = (S)tb.x;
-                }
-                // leak (emulator_utils.py:114-134): float32 products, subtract in S
-                if (f_leak) {
-                    const float rate = lnr[k] * (1.0f - d.leak_jit_f * lr[k]);
-                    const float delta = (dt_f * rate) * thp[k];
-                    base[k] = base[k] - (S)delta;
-                }
-                // difference and event count (emulator.py:748-772, emulator_utils.py:137-173)
-                const S diff = lp[k] - base[k];
+                lp[k] = lp_step<S, lp_eps_code>(f_lp, lp[k], tb.x, tb.y, eps_scale);
+                if (f_leak) base[k] = leak_step<S>(base[k], lnr[k], d.leak_jit_f, lr[k], dt_f, thp[k]);
+                const S diff = diff_of<S>(false, lp[k], (S)0, base[k]);
                 if (PLANES) {
                     if (pl.mask & 1u) pb[0] |= state_byte(pl, 0, (double)code) << (8 * k);
                     if (pl.mask & 2u) pb[1] |= state_byte(pl, 1, tb.x) << (8 * k);
@@ -1631,27 +1655,17 @@ fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint
                     if (pl.mask & 128u) pb[3] |= state_byte(pl, 7, (double)base[k]) << (8 * k);
                     if (pl.mask & 256u) pb[4] |= state_byte(pl, 8, (double)diff) << (8 * k);
                 }
-                const bool neg = diff < (S)0;
-                const float thf = neg ? thn[k] : thp[k];
-                S b;
-                if (sizeof(S) == 8 && !f_pp) b = neg ? tn_nom : tp_nom;
-                else b = (S)thf;
-                const S a = neg ? -diff : diff, b2 = b + b;
-                const int ge2 = a >= b2;
-                int32_t mag = (int)(a >= b) + ge2;
-                if (ge2 && !(a - b2 < b)) mag = fused_deep_count<S>(a, b);          // >= 3 events: rare
+                const EventCount<S> ec = event_count<S>(diff, thp[k], thn[k], !f_pp, tp_nom, tn_nom);
+                const bool neg = ec.neg;
+                int32_t mag = ec.mag;
+                if (ec.deep) mag = fused_deep_count<S>(ec.a, ec.b);                    // >= 3 events: rare
                 int flags = 0;
                 if (f_shot && shot_candidate(pref[k], pref_lo))                        // rare
                     flags = fused_shot_flags(d.seed, d.shot_inten_m1, d.per_pixel_thres, d.pos_nom, d.neg_nom,
                                              s_ff[f].shot_c, g0 + k, frame_index, pref[k], code, thp[k], thn[k]);
                 if (k >= valid) { mag = 0; flags = 0; }
                 // the refractory filter does not run (checked by the plan): every event is emitted
-                // (emulator.py:936-942: int32 * float32 -> float32, then the state's dtype). Selects, not
-                // branches: x + 0.0 would turn a -0.0 into +0.0
-                const S prod = (S)((float)mag * thf);
-                const S moved = base[k] + (neg ? -prod : prod);          // x - p == x + (-p) exactly
-                S bb = mag ? moved : base[k];
-                bb = flags ? lp[k] : bb;
+                const S bb = base_after<S>(base[k], mag, neg ? thn[k] : thp[k], neg, flags, lp[k]);
                 base[k] = bb;
                 if (PROBE && pid[k] >= 0) {
                     V2eProbeSample *ps = pr.out + (size_t)f * pr.n + pid[k];
@@ -1789,10 +1803,7 @@ emu_fused_count_kernel(EmuDev d, int T, int groups, const uint16_t *__restrict__
             for (int it = 0; it < wmax; it++) {
                 const unsigned on = __ballot_sync(0xffffffffu, it < magc && !neg);
                 const unsigned off = __ballot_sync(0xffffffffu, it < magc && neg);
-                if (lane == 0) {
-                    if (on) { if (2 * it < kSegSmem) atomicAdd(&s_hist[2 * it], __popc(on)); else atomicAdd(&hist[2 * it], __popc(on)); }
-                    if (off) { if (2 * it + 1 < kSegSmem) atomicAdd(&s_hist[2 * it + 1], __popc(off)); else atomicAdd(&hist[2 * it + 1], __popc(off)); }
-                }
+                if (lane == 0) seg_add(s_hist, hist, it, on, off);
             }
             const unsigned son = __ballot_sync(0xffffffffu, flags & 1), soff = __ballot_sync(0xffffffffu, flags & 2);
             if (lane == 0) {
@@ -1808,7 +1819,7 @@ emu_fused_count_kernel(EmuDev d, int T, int groups, const uint16_t *__restrict__
     if (tid < kBlkSeg) {
         const uint32_t v = s_hist[tid];
         blk_cnt[(size_t)blockIdx.x * kBlkSeg + tid] = v;
-        if (v) atomicAdd(&hist[tid < kSegSmem ? tid : 2 * d.iter_cap + (tid - kSegSmem)], v);
+        if (v) atomicAdd(&hist[bin_seg(d, tid)], v);
     }
 }
 
@@ -1829,33 +1840,11 @@ emu_fused_plan_kernel(EmuDev d, const FrameParams *__restrict__ fp, int T, uint6
         if (d.refr_on && max_n > 0 && d.refr_d > p.dt / (double)max_n) bad = true;    // emulator.py:792, 830
         const uint32_t *h = d.hist_pre + (size_t)f * d.seg_stride;
         uint32_t *off = d.segoff + (size_t)f * d.seg_stride;
-        const int nseg = bad ? 0 : 2 * max_n;
-        const int s0 = 2 * lane, s1 = 2 * lane + 1;
-        const uint32_t v0 = s0 < nseg ? h[s0] : 0u, v1 = s1 < nseg ? h[s1] : 0u;
-        uint32_t incl = v0 + v1;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-        }
-        const uint32_t excl = incl - (v0 + v1);
-        if (s0 < nseg) off[s0] = excl;
-        if (s1 < nseg) off[s1] = excl + v0;
-        const uint32_t sig = __shfl_sync(0xffffffffu, incl, 31);
-        const uint32_t sig_on = __reduce_add_sync(0xffffffffu, v0);
+        uint32_t sig, sig_on;
+        warp_seg_scan(h, off, bad ? 0 : 2 * max_n, lane, sig, sig_on);
         if (lane == 0) {
-            const uint32_t shot_on = h[2 * d.iter_cap], shot_off = h[2 * d.iter_cap + 1];
-            off[2 * d.iter_cap] = sig;
-            off[2 * d.iter_cap + 1] = sig + shot_on;
-            const uint32_t total = sig + shot_on + shot_off;
             c->max_n = max_n;
-            c->filter_active = 0;
-            c->n_on = sig_on + shot_on;
-            c->n_off = (sig - sig_on) + shot_off;
-            c->n_shot_on = shot_on;
-            c->n_shot_off = shot_off;
-            c->n_events = total;
-            s_tot[f] = total;
+            s_tot[f] = write_frame_counts(d, c, h, off, sig, sig_on, 0);
             if (bad) atomicMin(&s_bad, f);
         }
     }
@@ -1902,14 +1891,13 @@ emu_fused_emit_kernel(EmuDev d, const FrameParams *__restrict__ fp, int T, int g
         const uint32_t nb = blk_cnt[(size_t)blockIdx.x * kBlkSeg + tid];
         s_cnt[tid] = 0;
         if (nb) {
-            const int seg = tid < kSegSmem ? tid : 2 * d.iter_cap + (tid - kSegSmem);
+            const int seg = bin_seg(d, tid);
             s_base[tid] = segoff[seg] + atomicAdd(&cursor[seg], nb);
         }
     }
     __syncthreads();
-    auto claim = [&](int seg_smem, int seg, unsigned count) -> uint32_t {
-        if (seg_smem >= 0) return s_base[seg_smem] + atomicAdd(&s_cnt[seg_smem], count);
-        return segoff[seg] + atomicAdd(&cursor[seg], count);
+    auto claim = [&](int bin, int seg, unsigned count) {
+        return claim_rows(s_base, s_cnt, segoff, cursor, bin, seg, count);
     };
     const int ue = min(d.units, (g + 1) * kFusedGroup);
     for (int ub = g * kFusedGroup + warp * 8; ub < ue; ub += kWarps * 8) {
@@ -1929,36 +1917,11 @@ emu_fused_emit_kernel(EmuDev d, const FrameParams *__restrict__ fp, int T, int g
             const int idx = (ub + k) * kUnitPx + (int)(r & 127u);
             const float fx = (float)(idx % d.W), fy = (float)(idx / d.W);
             const float pv = neg ? -1.0f : 1.0f;
-            const int wmax = __reduce_max_sync(0xffffffffu, mag);
-            for (int it = 0; it < wmax; it++) {
-                const float t = linspace_f32(ts, it);
-                const bool pass = it < mag;
-                const unsigned on = __ballot_sync(0xffffffffu, pass && !neg);
-                const unsigned off = __ballot_sync(0xffffffffu, pass && neg);
-                uint32_t b_on = 0, b_off = 0;
-                if (lane == 0) {
-                    if (on) b_on = claim(2 * it < kSegSmem ? 2 * it : -1, 2 * it, __popc(on));
-                    if (off) b_off = claim(2 * it + 1 < kSegSmem ? 2 * it + 1 : -1, 2 * it + 1, __popc(off));
-                }
-                b_on = __shfl_sync(0xffffffffu, b_on, 0);
-                b_off = __shfl_sync(0xffffffffu, b_off, 0);
-                if (pass) {
-                    const uint64_t row = ev_base + (neg ? b_off + __popc(off & lt_mask) : b_on + __popc(on & lt_mask));
-                    events[row] = make_float4(t, fx, fy, pv);
-                }
-            }
-            const unsigned son = __ballot_sync(0xffffffffu, flags & 1), soff = __ballot_sync(0xffffffffu, flags & 2);
-            if (son | soff) {
-                uint32_t b_on = 0, b_off = 0;
-                if (lane == 0) {
-                    if (son) b_on = claim(kSegSmem, 0, __popc(son));
-                    if (soff) b_off = claim(kSegSmem + 1, 0, __popc(soff));
-                }
-                b_on = __shfl_sync(0xffffffffu, b_on, 0);
-                b_off = __shfl_sync(0xffffffffu, b_off, 0);
-                if (flags & 1) events[ev_base + b_on + __popc(son & lt_mask)] = make_float4(ts_last, fx, fy, 1.0f);
-                if (flags & 2) events[ev_base + b_off + __popc(soff & lt_mask)] = make_float4(ts_last, fx, fy, -1.0f);
-            }
+            float tm = 0.f;                      // the refractory filter does not run in an accepted chunk
+            warp_walk(mag, neg, ts, false, 0.f, tm, [&](int it, float t, unsigned on, unsigned off, bool pass) {
+                write_iter_rows(claim, events, ev_base, lane, lt_mask, it, t, on, off, pass, neg, fx, fy, pv);
+            });
+            write_shot_rows(claim, events, ev_base, lane, lt_mask, flags, ts_last, fx, fy);
         }
     }
 }
@@ -1978,8 +1941,8 @@ emu_fused_commit_kernel(EmuDev d, const uint4 *__restrict__ lp_alt, const uint4 
 // while probes are set). Both leave when the emit kernel does (abort, frame not planned), so a frame whose emission
 // is re-run after a capacity abort is recorded by the re-run.
 // Before the emission: the update kernel's inputs are still in memory (lp, base after the leak, the surround, pr_eff,
-// the record, timestamp_mem), so diff and the counts that survive the refractory filter are recomputed with the same
-// operations as emu_update_kernel / warp_walk.
+// the record, timestamp_mem), so diff and the counts that survive the refractory filter are recomputed through what
+// emu_update_kernel and emu_emit_kernel call: lin_log_of, diff_of and warp_walk.
 template <typename S> struct PreEmit {
     double xv, ln;                      // new_frame, log_new_frame
     S lp, sur, cms, base, diff;         // lp_log_frame, cs_surround_frame, c_minus_s_frame, base after the leak, diff
@@ -1989,44 +1952,36 @@ __device__ __forceinline__ PreEmit<S> pre_emit_state(const EmuDev &d, int idx, c
     PreEmit<S> e;
     e.xv = dtype == V2E_U8 ? (double)((const uint8_t *)frame)[idx]
          : dtype == V2E_F32 ? (double)((const float *)frame)[idx] : ((const double *)frame)[idx];
-    e.ln = d.hdr ? e.xv
-         : (double)((e.xv >= 0.0 && e.xv <= 255.0 && e.xv == floor(e.xv)) ? d.lut[(int)e.xv] : lin_log_eval(e.xv));
+    e.ln = d.hdr ? e.xv : (double)lin_log_of<V2E_F64>(d.lut, e.xv);
     e.lp = ((const S *)d.lp)[idx];
     e.base = ((const S *)d.base)[idx];
     // what the change amplifier saw (emu_update_kernel: pr_eff exists iff the front kernel ran, which sets lp_done)
     const S src = d.pr_eff ? ((const S *)d.pr_eff)[idx] : e.lp;
     e.sur = d.csdvs ? cs_buf<S>(d, *d.cs_cur)[idx] : (S)0;
     e.cms = src - e.sur;
-    e.diff = d.csdvs ? e.cms - e.base : src - e.base;
+    e.diff = diff_of<S>(d.csdvs, src, e.sur, e.base);
     return e;
 }
 
 template <typename S>
+// Launched as whole warps (64 threads, up to 64 probes): every lane takes part in warp_walk, lanes without a probe
+// with no events.
 __global__ void emu_probe_pre_kernel(EmuDev d, FrameParams p, int slot, const void *frame, int dtype, ProbeDev pr) {
     const int i = threadIdx.x;
-    if (i >= pr.n) return;
     if (*(volatile int32_t *)d.abort_flag) return;
     const FrameCtrl *c = d.ctrl + slot;
     if (!c->planned) return;
-    const int idx = pr.px[i];
-    const PreEmit<S> e = pre_emit_state<S>(d, idx, frame, dtype);
-    const double xv = e.xv, ln = e.ln;
-    const S lp = e.lp, diff = e.diff;
-    const int cnt = d.rec[idx] >> kRecShift;
+    const int idx = i < pr.n ? pr.px[i] : 0;
+    const int cnt = i < pr.n ? d.rec[idx] >> kRecShift : 0;
     const int mag = cnt < 0 ? -cnt : cnt, pol = cnt < 0;
     const TsParams ts = make_ts(p, c->max_n, d.refr_d);
     const bool filter = ts.filter_active && d.refr_on;
     float tm = (filter && mag) ? d.tmem[idx] : 0.f;
-    int fin = 0;
-    for (int it = 0; it < mag; it++) {
-        bool pass = true;
-        if (filter) {
-            const float t = linspace_f32(ts, it);
-            pass = (t - tm) > d.refr_f;
-            if (pass) tm = t;
-        }
-        fin += pass;
-    }
+    const int fin = warp_walk(mag, pol, ts, filter, d.refr_f, tm, [](int, float, unsigned, unsigned, bool) {});
+    if (i >= pr.n) return;
+    const PreEmit<S> e = pre_emit_state<S>(d, idx, frame, dtype);
+    const double xv = e.xv, ln = e.ln;
+    const S lp = e.lp, diff = e.diff;
     V2eProbeSample *ps = pr.out + i;
     ps->new_frame = xv;
     ps->log_new_frame = ln;
@@ -2505,24 +2460,30 @@ extern "C" int v2e_emu_set_pr_noise(V2eEmu *h, const float *pr_randn_dev, const 
 static inline int list_grid(const EmuDev &d) { return d.n_blocks < 1184 ? d.n_blocks : 1184; }
 static inline int grid_for(const EmuDev &d) { return (d.n_pad / kVec + kThreads - 1) / kThreads; }
 
-template <typename S>
-static int launch_first(V2eEmu *h, const FrameParams &p, const void *frame, int dt, cudaStream_t st) {
-    int g = grid_for(h->d);
-    switch (dt) {
-        case V2E_U8: emu_first_frame_kernel<S, V2E_U8><<<g, kThreads, 0, st>>>(h->d, p, frame); break;
-        case V2E_F32: emu_first_frame_kernel<S, V2E_F32><<<g, kThreads, 0, st>>>(h->d, p, frame); break;
-        case V2E_F64: emu_first_frame_kernel<S, V2E_F64><<<g, kThreads, 0, st>>>(h->d, p, frame); break;
+// The kernels are templates over the frame dtype (FT) and the state dtype (S). with_frame_type calls f(ft) with
+// decltype(ft)::value the frame dtype; with_state_type calls f(s) with decltype(s) the handle's state dtype (double,
+// or float when cutoff_hz == 0) and returns what f returns.
+template <typename F> static int with_frame_type(int dtype, F &&f) {
+    switch (dtype) {
+        case V2E_U8: f(std::integral_constant<int, V2E_U8>()); return V2E_OK;
+        case V2E_F32: f(std::integral_constant<int, V2E_F32>()); return V2E_OK;
+        case V2E_F64: f(std::integral_constant<int, V2E_F64>()); return V2E_OK;
         default: return fail(V2E_E_INVALID, "bad frame dtype");
     }
-    return V2E_OK;
 }
+template <typename F> static auto with_state_type(const EmuDev &d, F &&f) { return d.state_f64 ? f(0.0) : f(0.0f); }
 
 extern "C" int v2e_emu_first_frame(V2eEmu *h, const void *frame, int dtype, double t_frame,
                                    double t_previous, void *stream) {
     if (!h || !frame) return fail(V2E_E_INVALID, "null argument");
-    FrameParams p = make_params(h, t_frame, t_previous, 0, 0);
-    int rc = h->d.state_f64 ? launch_first<double>(h, p, frame, dtype, (cudaStream_t)stream)
-                            : launch_first<float>(h, p, frame, dtype, (cudaStream_t)stream);
+    const FrameParams p = make_params(h, t_frame, t_previous, 0, 0);
+    const EmuDev &d = h->d;
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc = with_state_type(d, [&](auto s) {
+        return with_frame_type(dtype, [&](auto ft) {
+            emu_first_frame_kernel<decltype(s), decltype(ft)::value><<<grid_for(d), kThreads, 0, st>>>(d, p, frame);
+        });
+    });
     if (rc) return rc;
     if (h->d.csdvs) CU(cudaMemsetAsync(h->d.cs_cur, 0, sizeof(int32_t), (cudaStream_t)stream));
     CU(cudaGetLastError());
@@ -2551,31 +2512,25 @@ static int launch_update_r(V2eEmu *h, const FrameParams &p, const void *frame, i
         emu_update_kernel<double, V2E_U8, 1, true><<<g, kThreads, sm, st>>>(h->d, p, frame, lr, sr, slot, do_plan, 0);
         return V2E_OK;
     }
-    switch (dt) {
-        case V2E_U8: emu_update_kernel<S, V2E_U8, RNG, false><<<g, kThreads, sm, st>>>(h->d, p, frame, lr, sr, slot, do_plan, lp_done); break;
-        case V2E_F32: emu_update_kernel<S, V2E_F32, RNG, false><<<g, kThreads, sm, st>>>(h->d, p, frame, lr, sr, slot, do_plan, lp_done); break;
-        case V2E_F64: emu_update_kernel<S, V2E_F64, RNG, false><<<g, kThreads, sm, st>>>(h->d, p, frame, lr, sr, slot, do_plan, lp_done); break;
-        default: return fail(V2E_E_INVALID, "bad frame dtype");
-    }
-    return V2E_OK;
+    return with_frame_type(dt, [&](auto ft) {
+        emu_update_kernel<S, decltype(ft)::value, RNG, false><<<g, kThreads, sm, st>>>(h->d, p, frame, lr, sr, slot, do_plan,
+                                                                                       lp_done);
+    });
 }
-template <typename S>
 static int launch_update(V2eEmu *h, const FrameParams &p, const void *frame, int dt, const float *lr,
                          const float *sr, int slot, int do_plan, int lp_done, cudaStream_t st) {
-    return h->d.rng_mode == 1 ? launch_update_r<S, 1>(h, p, frame, dt, lr, sr, slot, do_plan, lp_done, st)
-                              : launch_update_r<S, 0>(h, p, frame, dt, lr, sr, slot, do_plan, lp_done, st);
+    return with_state_type(h->d, [&](auto s) {
+        using S = decltype(s);
+        return h->d.rng_mode == 1 ? launch_update_r<S, 1>(h, p, frame, dt, lr, sr, slot, do_plan, lp_done, st)
+                                  : launch_update_r<S, 0>(h, p, frame, dt, lr, sr, slot, do_plan, lp_done, st);
+    });
 }
 
 static int launch_shot(V2eEmu *h, const FrameParams &p, const void *frame, int dt, const float *sr,
                        int slot, cudaStream_t st) {
-    int g = grid_for(h->d);
-    switch (dt) {
-        case V2E_U8: emu_shot_kernel<V2E_U8><<<g, kThreads, 0, st>>>(h->d, p, frame, sr, slot); break;
-        case V2E_F32: emu_shot_kernel<V2E_F32><<<g, kThreads, 0, st>>>(h->d, p, frame, sr, slot); break;
-        case V2E_F64: emu_shot_kernel<V2E_F64><<<g, kThreads, 0, st>>>(h->d, p, frame, sr, slot); break;
-        default: return fail(V2E_E_INVALID, "bad frame dtype");
-    }
-    return V2E_OK;
+    return with_frame_type(dt, [&](auto ft) {
+        emu_shot_kernel<decltype(ft)::value><<<grid_for(h->d), kThreads, 0, st>>>(h->d, p, frame, sr, slot);
+    });
 }
 
 struct ProfScope {
@@ -2634,24 +2589,16 @@ static void cs_run_steps(V2eEmu *h, double alpha_p, float alpha_h, int s0, int s
     h->n_cs_step++;
 }
 static void cs_steps(V2eEmu *h, double alpha_p, float alpha_h, int s0, int s1, int sharded, int slot, cudaStream_t st) {
-    if (h->d.state_f64) cs_run_steps<double>(h, alpha_p, alpha_h, s0, s1, sharded, slot, st);
-    else cs_run_steps<float>(h, alpha_p, alpha_h, s0, s1, sharded, slot, st);
+    with_state_type(h->d, [&](auto s) { cs_run_steps<decltype(s)>(h, alpha_p, alpha_h, s0, s1, sharded, slot, st); });
 }
 
 // photoreceptor low-pass of the centre-surround model, ahead of the Euler steps
-template <typename S>
-static int launch_lp_s(const EmuDev &d, const FrameParams &p, const void *frame, int dtype, cudaStream_t st) {
-    const int g = grid_for(d);
-    switch (dtype) {
-        case V2E_U8: emu_lp_kernel<S, V2E_U8><<<g, kThreads, 0, st>>>(d, p, frame); break;
-        case V2E_F32: emu_lp_kernel<S, V2E_F32><<<g, kThreads, 0, st>>>(d, p, frame); break;
-        case V2E_F64: emu_lp_kernel<S, V2E_F64><<<g, kThreads, 0, st>>>(d, p, frame); break;
-        default: return fail(V2E_E_INVALID, "bad frame dtype");
-    }
-    return V2E_OK;
-}
 static int launch_lp(const EmuDev &d, const FrameParams &p, const void *frame, int dtype, cudaStream_t st) {
-    return d.state_f64 ? launch_lp_s<double>(d, p, frame, dtype, st) : launch_lp_s<float>(d, p, frame, dtype, st);
+    return with_state_type(d, [&](auto s) {
+        return with_frame_type(dtype, [&](auto ft) {
+            emu_lp_kernel<decltype(s), decltype(ft)::value><<<grid_for(d), kThreads, 0, st>>>(d, p, frame);
+        });
+    });
 }
 
 // Euler-step plan of one frame of the centre-surround model (emulator.py:1068-1096)
@@ -2675,17 +2622,12 @@ static int cs_plan(const V2eEmu *h, const FrameParams &p, int *num_steps, double
 // high-pass -> pr_eff, which the update kernel then reads with lp_done = 1
 static int enqueue_front(const EmuDev &d, const FrameParams &p, const void *frame, int dtype, const float *pr_randn,
                          int lp_done, cudaStream_t st) {
-    const int g = grid_for(d);
-#define FRONT(S_)                                                                                                  \
-    switch (dtype) {                                                                                                \
-        case V2E_U8: emu_front_kernel<S_, V2E_U8><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break;   \
-        case V2E_F32: emu_front_kernel<S_, V2E_F32><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break; \
-        case V2E_F64: emu_front_kernel<S_, V2E_F64><<<g, kThreads, 0, st>>>(d, p, frame, pr_randn, lp_done); break; \
-        default: return fail(V2E_E_INVALID, "bad frame dtype");                                                     \
-    }
-    if (d.state_f64) { FRONT(double) } else { FRONT(float) }
-#undef FRONT
-    return V2E_OK;
+    return with_state_type(d, [&](auto s) {
+        return with_frame_type(dtype, [&](auto ft) {
+            emu_front_kernel<decltype(s), decltype(ft)::value><<<grid_for(d), kThreads, 0, st>>>(d, p, frame, pr_randn,
+                                                                                                 lp_done);
+        });
+    });
 }
 
 // the photoreceptor-noise inputs of a single-frame step (v2e_emu_set_pr_noise): amplitude into p, the replay field
@@ -2759,8 +2701,7 @@ static int enqueue_count(V2eEmu *h, const FrameParams &p, const void *frame, int
     }
     {
         ProfScope ps(h, slot, 0, st);
-        rc = d.state_f64 ? launch_update<double>(h, p, frame, dtype, lr, sr, slot, plan_in_update, lp_done, st)
-                         : launch_update<float>(h, p, frame, dtype, lr, sr, slot, plan_in_update, lp_done, st);
+        rc = launch_update(h, p, frame, dtype, lr, sr, slot, plan_in_update, lp_done, st);
     }
     if (rc) return rc;
     if (d.refr_on) {
@@ -2774,25 +2715,21 @@ static int enqueue_emit(V2eEmu *h, const FrameParams &p, int slot, float *events
     const EmuDev &d = h->d;
     h->ord.events = events;
     const ProbeDev pr = probe_dev(h, slot);
-    if (pr.n) {
-        if (d.state_f64) emu_probe_pre_kernel<double><<<1, 64, 0, st>>>(d, p, slot, h->probe.frame[slot], h->probe.dtype[slot], pr);
-        else emu_probe_pre_kernel<float><<<1, 64, 0, st>>>(d, p, slot, h->probe.frame[slot], h->probe.dtype[slot], pr);
-    }
-    if (h->ms.mask) {
-        const PlaneDev pl = plane_dev(h, slot);
-        const int g = (pl.npx + kThreads - 1) / kThreads;
-        if (d.state_f64) emu_model_state_kernel<double><<<g, kThreads, 0, st>>>(d, slot, h->probe.frame[slot], h->probe.dtype[slot], pl);
-        else emu_model_state_kernel<float><<<g, kThreads, 0, st>>>(d, slot, h->probe.frame[slot], h->probe.dtype[slot], pl);
-    }
-    {
-        ProfScope ps(h, slot, 2, st);
-        if (d.state_f64) emu_emit_kernel<double><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
-        else emu_emit_kernel<float><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
-    }
-    if (pr.n) {
-        if (d.state_f64) emu_probe_post_kernel<double><<<1, 64, 0, st>>>(d, slot, pr);
-        else emu_probe_post_kernel<float><<<1, 64, 0, st>>>(d, slot, pr);
-    }
+    const void *frame = h->probe.frame[slot];
+    const int dtype = h->probe.dtype[slot];
+    with_state_type(d, [&](auto s) {
+        using S = decltype(s);
+        if (pr.n) emu_probe_pre_kernel<S><<<1, 64, 0, st>>>(d, p, slot, frame, dtype, pr);
+        if (h->ms.mask) {
+            const PlaneDev pl = plane_dev(h, slot);
+            emu_model_state_kernel<S><<<(pl.npx + kThreads - 1) / kThreads, kThreads, 0, st>>>(d, slot, frame, dtype, pl);
+        }
+        {
+            ProfScope ps(h, slot, 2, st);
+            emu_emit_kernel<S><<<list_grid(d), kThreads, 0, st>>>(d, p, slot, (float4 *)events);
+        }
+        if (pr.n) emu_probe_post_kernel<S><<<1, 64, 0, st>>>(d, slot, pr);
+    });
     return V2E_OK;
 }
 static void enqueue_null_bracket(V2eEmu *h, int slot, cudaStream_t st) {
@@ -2896,16 +2833,18 @@ static void launch_fused_update_f(V2eEmu *h, const EmuDev &d, const FusedFrame *
     }
 }
 // frames [a, a + T) of the step (d shifted to slot a)
-template <typename S>
 static int launch_fused_update(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, int a,
                                cudaStream_t st) {
     const size_t sm = (size_t)T * sizeof(FusedFrame);
-    const bool fast = sizeof(S) == 8 && d.rng_mode == 1 && d.per_pixel_thres && d.leak_on && d.shot_on;
     if (sm > 40 * 1024) return fail(V2E_E_INVALID, "fused path: too many frames per step");
     const ProbeDev pr = probe_dev(h, a);
     const PlaneDev pl = plane_dev(h, a);
-    if (fast) launch_fused_update_f<S, true>(h, d, ff, frames, T, sm, pr, pl, st);
-    else launch_fused_update_f<S, false>(h, d, ff, frames, T, sm, pr, pl, st);
+    with_state_type(d, [&](auto s) {
+        using S = decltype(s);
+        const bool fast = sizeof(S) == 8 && d.rng_mode == 1 && d.per_pixel_thres && d.leak_on && d.shot_on;
+        if (fast) launch_fused_update_f<S, true>(h, d, ff, frames, T, sm, pr, pl, st);
+        else launch_fused_update_f<S, false>(h, d, ff, frames, T, sm, pr, pl, st);
+    });
     return V2E_OK;
 }
 
@@ -2957,8 +2896,7 @@ static int enqueue_fused_count(V2eEmu *h, const void *frames, int T, cudaStream_
     int rc;
     {
         ProfScope ps(h, 0, 0, st);
-        rc = d.state_f64 ? launch_fused_update<double>(h, d, h->ff_dev + a, fr, T, a, st)
-                         : launch_fused_update<float>(h, d, h->ff_dev + a, fr, T, a, st);
+        rc = launch_fused_update(h, d, h->ff_dev + a, fr, T, a, st);
     }
     if (rc) return rc;
     {
@@ -3000,6 +2938,16 @@ static void remember_step(V2eEmu *h, const void *frames, int dtype, int T, const
 static int step_classic(V2eEmu *h, const void *frames, int dtype, int T, const double *t_frames, double t_previous,
                         const float *leak_randn, const float *shot_rand, float *events, uint64_t capacity,
                         uint64_t ev_base_start, int first, int resume_emit, void *stream, int last = -1);
+
+// the arguments of v2e_emu_step
+static int check_step(const V2eEmu *h, const void *frames, int T, const double *t_frames, const float *events,
+                      uint64_t capacity, int first) {
+    if (!h || !frames || !t_frames || (!events && capacity)) return fail(V2E_E_INVALID, "null argument");
+    if (!h->first_done) return fail(V2E_E_STATE, "v2e_emu_first_frame must run before v2e_emu_step");
+    if (T < 1 || T > h->d.max_slots || first < 0 || first >= T) return fail(V2E_E_INVALID, "bad T / first");
+    if (((uintptr_t)events & 15) != 0) return fail(V2E_E_INVALID, "events_out must be 16-byte aligned");
+    return V2E_OK;
+}
 
 // Runs segments [from, n_seg) of the handle's schedule over the remembered step (h->ls); Philox frame indices are
 // step_base + frame. The first segment of the step starts at ls.ev_base_start, every other one where the previous
@@ -3120,16 +3068,13 @@ static int step_classic(V2eEmu *h, const void *frames, int dtype, int T, const d
                             double t_previous, const float *leak_randn, const float *shot_rand,
                             float *events, uint64_t capacity, uint64_t ev_base_start, int first,
                             int resume_emit, void *stream, int last) {
-    if (!h || !frames || !t_frames || (!events && capacity)) return fail(V2E_E_INVALID, "null argument");
-    if (!h->first_done) return fail(V2E_E_STATE, "v2e_emu_first_frame must run before v2e_emu_step");
-    if (T < 1 || T > h->d.max_slots || first < 0 || first >= T) return fail(V2E_E_INVALID, "bad T / first");
-    if (((uintptr_t)events & 15) != 0) return fail(V2E_E_INVALID, "events_out must be 16-byte aligned");
+    int rc;
+    if ((rc = check_step(h, frames, T, t_frames, events, capacity, first))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const EmuDev &d = h->d;
     const size_t fbytes = (size_t)d.n * frame_elem(dtype);
     if (last < 0 || last > T) last = T;
     if (first >= last) return fail(V2E_E_INVALID, "bad frame range");
-    int rc;
     if (resume_emit) {
         // frame `first` was counted but not emitted (capacity abort): clear the abort and the slots
         // after it, keep slot `first`'s histograms, re-plan it against the new capacity.
@@ -3183,13 +3128,10 @@ extern "C" int v2e_emu_step(V2eEmu *h, const void *frames, int dtype, int T, con
                             double t_previous, const float *leak_randn, const float *shot_rand,
                             float *events, uint64_t capacity, uint64_t ev_base_start, int first,
                             int resume_emit, void *stream) {
-    if (!h || !frames || !t_frames || (!events && capacity)) return fail(V2E_E_INVALID, "null argument");
-    if (!h->first_done) return fail(V2E_E_STATE, "v2e_emu_first_frame must run before v2e_emu_step");
-    if (T < 1 || T > h->d.max_slots || first < 0 || first >= T) return fail(V2E_E_INVALID, "bad T / first");
-    if (((uintptr_t)events & 15) != 0) return fail(V2E_E_INVALID, "events_out must be 16-byte aligned");
+    int rc;
+    if ((rc = check_step(h, frames, T, t_frames, events, capacity, first))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const EmuDev &d = h->d;
-    int rc;
     if (resume_emit && h->last_fused == 1 && h->n_seg > 0) {
         // capacity abort at frame `first` of a scheduled step (the abort is sticky: nothing after it ran). The segment
         // that holds `first` is finished into the larger buffer -- a multi-frame segment still has its records and is
@@ -3404,6 +3346,27 @@ extern "C" int v2e_emu_collect(V2eEmu *h, V2eFrameInfo *info, int T, int *frames
 
 extern "C" int v2e_probe_sample_size(void) { return (int)sizeof(V2eProbeSample); }
 
+// Makes the handle's device current for the rest of the scope, whichever device is current for the caller, and
+// restores the caller's at its end: the probe and model-state buffers belong on the handle's device.
+struct OnHandleDevice {
+    int cur = 0, dev;
+    cudaError_t err;
+    explicit OnHandleDevice(const V2eEmu *h) : dev(h->probe.device) {
+        err = cudaGetDevice(&cur);
+        if (err != cudaSuccess) cur = dev;
+        else if (cur != dev) err = cudaSetDevice(dev);
+    }
+    ~OnHandleDevice() { if (cur != dev) cudaSetDevice(cur); }
+};
+
+// the device a buffer of the handle lives on; -1 while it does not exist
+static int buffer_device(const void *p) {
+    if (!p) return -1;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) return fail(V2E_E_CUDA, "cudaPointerGetAttributes failed");
+    return a.device;
+}
+
 extern "C" int v2e_emu_set_probes(V2eEmu *h, const int32_t *pixels_host, int n) {
     if (!h) return fail(V2E_E_INVALID, "null handle");
     if (n < 0 || n > 64 || (n > 0 && !pixels_host)) return fail(V2E_E_INVALID, "probes: 0 <= n <= 64 pixels");
@@ -3412,19 +3375,15 @@ extern "C" int v2e_emu_set_probes(V2eEmu *h, const int32_t *pixels_host, int n) 
         for (int k = 0; k < i; k++)
             if (pixels_host[k] == pixels_host[i]) return fail(V2E_E_INVALID, "probe pixels must be distinct");
     }
-    // the buffers belong on the handle's device, whichever device is current for the caller
-    int cur = 0;
-    CU(cudaGetDevice(&cur));
-    if (cur != h->probe.device) CU(cudaSetDevice(h->probe.device));
+    const OnHandleDevice on(h);
     const size_t per_slot = (size_t)h->d.max_slots * 64;
-    cudaError_t e = cudaSuccess;
-    if (n > 0 && !h->probe.px) {
+    cudaError_t e = on.err;
+    if (e == cudaSuccess && n > 0 && !h->probe.px) {
         e = cudaMalloc((void **)&h->probe.px, 64 * sizeof(int32_t));
         if (e == cudaSuccess) e = cudaMalloc((void **)&h->probe.samples, per_slot * sizeof(V2eProbeSample));
         if (e == cudaSuccess) e = cudaMallocHost((void **)&h->probe.host, per_slot * sizeof(V2eProbeSample));
     }
     if (e == cudaSuccess && n > 0) e = cudaMemcpy(h->probe.px, pixels_host, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice);
-    if (cur != h->probe.device) cudaSetDevice(cur);
     if (e != cudaSuccess) return fail(V2E_E_CUDA, "v2e_emu_set_probes: %s", cudaGetErrorString(e));
     h->probe.n = n;
     h->probe.ready = 0;
@@ -3432,11 +3391,7 @@ extern "C" int v2e_emu_set_probes(V2eEmu *h, const int32_t *pixels_host, int n) 
 }
 
 extern "C" int v2e_emu_probe_device(V2eEmu *h) {
-    if (!h) return fail(V2E_E_INVALID, "null handle");
-    if (!h->probe.samples) return -1;
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, h->probe.samples) != cudaSuccess) return fail(V2E_E_CUDA, "cudaPointerGetAttributes failed");
-    return a.device;
+    return h ? buffer_device(h->probe.samples) : fail(V2E_E_INVALID, "null handle");
 }
 
 extern "C" int v2e_emu_set_model_states(V2eEmu *h, uint32_t mask, const double *lo_span_host) {
@@ -3453,16 +3408,13 @@ extern "C" int v2e_emu_set_model_states(V2eEmu *h, uint32_t mask, const double *
     }
     const size_t need = (size_t)h->d.max_slots * nst * (size_t)(h->d.own_hi - h->d.own_lo);
     if (need > h->ms.cap) {
-        // the buffer belongs on the handle's device, whichever device is current for the caller
-        int cur = 0;
-        CU(cudaGetDevice(&cur));
-        if (cur != h->probe.device) CU(cudaSetDevice(h->probe.device));
+        const OnHandleDevice on(h);
+        if (on.err != cudaSuccess) return fail(V2E_E_CUDA, "v2e_emu_set_model_states: %s", cudaGetErrorString(on.err));
         if (h->ms.planes) cudaFree(h->ms.planes);
         h->ms.cap = 0;
         cudaError_t e = cudaMalloc((void **)&h->ms.planes, need);
-        if (e != cudaSuccess) h->ms.planes = nullptr;
-        if (cur != h->probe.device) cudaSetDevice(cur);
         if (e != cudaSuccess) {
+            h->ms.planes = nullptr;
             h->ms.mask = 0;
             h->ms.nst = 0;
             return fail(V2E_E_CUDA, "v2e_emu_set_model_states: %s", cudaGetErrorString(e));
@@ -3489,11 +3441,7 @@ extern "C" int v2e_emu_model_state_read(V2eEmu *h, void *dst_dev, uint64_t cap, 
 }
 
 extern "C" int v2e_emu_model_state_device(V2eEmu *h) {
-    if (!h) return fail(V2E_E_INVALID, "null handle");
-    if (!h->ms.planes) return -1;
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, h->ms.planes) != cudaSuccess) return fail(V2E_E_CUDA, "cudaPointerGetAttributes failed");
-    return a.device;
+    return h ? buffer_device(h->ms.planes) : fail(V2E_E_INVALID, "null handle");
 }
 
 extern "C" int v2e_emu_probe_read(V2eEmu *h, V2eProbeSample *out_host, int cap, int *n_frames, void *stream) {
@@ -3538,9 +3486,7 @@ extern "C" int v2e_emu_time_fused(V2eEmu *h, const void *frames, int dtype, int 
     cudaEventRecord(e[1], st);
     if (!rc) rc = reset_slots(h, 0, T, st);
     cudaEventRecord(e[2], st);
-    for (int k = 0; k < K && !rc; k++)
-        rc = h->d.state_f64 ? launch_fused_update<double>(h, h->d, h->ff_dev, (const uint8_t *)frames, T, 0, st)
-                            : launch_fused_update<float>(h, h->d, h->ff_dev, (const uint8_t *)frames, T, 0, st);
+    for (int k = 0; k < K && !rc; k++) rc = launch_fused_update(h, h->d, h->ff_dev, (const uint8_t *)frames, T, 0, st);
     cudaEventRecord(e[3], st);
     h->profile = prof;
     if (!rc) rc = reset_slots(h, 0, T, st);
@@ -3557,6 +3503,18 @@ extern "C" int v2e_emu_time_fused(V2eEmu *h, const void *frames, int dtype, int 
 }
 
 // ---- single-frame phases (slot 0) ---------------------------------------------------------------
+// the start of a single-frame step: slot 0 cleared, its first row, the frame's parameters (the next Philox frame index)
+static int begin_single_frame(V2eEmu *h, double t_frame, double t_previous, uint64_t capacity, uint64_t ev_base_start,
+                              cudaStream_t st, FrameParams *p) {
+    int rc;
+    if ((rc = reset_slots(h, 0, 1, st))) return rc;
+    emu_begin_step_kernel<<<1, 1, 0, st>>>(h->d, 0, ev_base_start);
+    *p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
+    h->ord.frame_index[0] = p->frame_index;
+    h->last_dt = p->dt;
+    return V2E_OK;
+}
+
 extern "C" int v2e_emu_phase_count(V2eEmu *h, const void *frame, int dtype, double t_frame,
                                    double t_previous, const float *lr, const float *sr, int shot_pending,
                                    uint64_t capacity, uint64_t ev_base_start, void *stream) {
@@ -3565,11 +3523,8 @@ extern "C" int v2e_emu_phase_count(V2eEmu *h, const void *frame, int dtype, doub
     if (t_frame < t_previous) return fail(V2E_E_INVALID, "frame times must be non-decreasing");
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    if ((rc = reset_slots(h, 0, 1, st))) return rc;
-    emu_begin_step_kernel<<<1, 1, 0, st>>>(h->d, 0, ev_base_start);
-    FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
-    h->ord.frame_index[0] = p.frame_index;
-    h->last_dt = p.dt;
+    FrameParams p;
+    if ((rc = begin_single_frame(h, t_frame, t_previous, capacity, ev_base_start, st, &p))) return rc;
     const float *prn = nullptr;
     if ((rc = take_pr_noise(h, p, &prn, "v2e_emu_phase_count"))) return rc;
     if ((rc = enqueue_count(h, p, frame, dtype, lr, sr, shot_pending, 0, st, prn))) return rc;
@@ -3588,11 +3543,8 @@ extern "C" int v2e_emu_phase_update(V2eEmu *h, const void *frame, int dtype, dou
     if (t_frame < t_previous) return fail(V2E_E_INVALID, "frame times must be non-decreasing");
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    if ((rc = reset_slots(h, 0, 1, st))) return rc;
-    emu_begin_step_kernel<<<1, 1, 0, st>>>(h->d, 0, ev_base_start);
-    FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
-    h->ord.frame_index[0] = p.frame_index;
-    h->last_dt = p.dt;
+    FrameParams p;
+    if ((rc = begin_single_frame(h, t_frame, t_previous, capacity, ev_base_start, st, &p))) return rc;
     // shot_pending = 1 makes enqueue_count run the update kernel alone when there is no refractory
     // period; with one, the filter must wait for the reduced max, so launch the update kernel directly
     const EmuDev &d = h->d;
@@ -3607,9 +3559,7 @@ extern "C" int v2e_emu_phase_update(V2eEmu *h, const void *frame, int dtype, dou
         if ((rc = enqueue_front(d, p, frame, dtype, prn, 0, st))) return rc;
         lp_done = 1;
     }
-    rc = d.state_f64 ? launch_update<double>(h, p, frame, dtype, lr, sr, 0, 0, lp_done, st)
-                     : launch_update<float>(h, p, frame, dtype, lr, sr, 0, 0, lp_done, st);
-    if (rc) return rc;
+    if ((rc = launch_update(h, p, frame, dtype, lr, sr, 0, 0, lp_done, st))) return rc;
     CU(cudaGetLastError());
     h->scidvs_started = 1;
     h->last_T = 1;
@@ -3628,11 +3578,8 @@ extern "C" int v2e_emu_cs_begin(V2eEmu *h, const void *frame, int dtype, double 
     cudaStream_t st = (cudaStream_t)stream;
     const EmuDev &d = h->d;
     int rc;
-    if ((rc = reset_slots(h, 0, 1, st))) return rc;
-    emu_begin_step_kernel<<<1, 1, 0, st>>>(d, 0, ev_base_start);
-    FrameParams p = make_params(h, t_frame, t_previous, h->frame_counter++, capacity);
-    h->ord.frame_index[0] = p.frame_index;
-    h->last_dt = p.dt;
+    FrameParams p;
+    if ((rc = begin_single_frame(h, t_frame, t_previous, capacity, ev_base_start, st, &p))) return rc;
     if ((rc = cs_plan(h, p, &h->cs_num_steps, &h->cs_alpha_p, &h->cs_alpha_h))) return rc;
     if ((rc = launch_lp(d, p, frame, dtype, st))) return rc;
     if (d.scidvs || d.pr_noise) {
@@ -3657,18 +3604,20 @@ extern "C" void *v2e_emu_cs_send_dev(V2eEmu *h) { return h ? h->cs_send : nullpt
 extern "C" uint64_t *v2e_emu_cs_max_dev(V2eEmu *h) { return h ? (uint64_t *)h->d.cs_max : nullptr; }
 extern "C" int v2e_emu_cs_pack(V2eEmu *h, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
-    if (h->d.state_f64) emu_csdvs_pack_kernel<double><<<132, 256, 0, (cudaStream_t)stream>>>(h->d, (double *)h->cs_send, h->cs_K);
-    else emu_csdvs_pack_kernel<float><<<132, 256, 0, (cudaStream_t)stream>>>(h->d, (float *)h->cs_send, h->cs_K);
+    with_state_type(h->d, [&](auto s) {
+        using S = decltype(s);
+        emu_csdvs_pack_kernel<S><<<132, 256, 0, (cudaStream_t)stream>>>(h->d, (S *)h->cs_send, h->cs_K);
+    });
     CU(cudaGetLastError());
     return V2E_OK;
 }
 extern "C" int v2e_emu_cs_unpack_from(V2eEmu *h, const void *rows_above_dev, const void *rows_below_dev, void *stream) {
     if (!h || !h->cs_K) return fail(V2E_E_STATE, "not a pixel-sharded centre-surround handle");
     cudaStream_t st = (cudaStream_t)stream;
-    if (h->d.state_f64)
-        emu_csdvs_unpack_kernel<double><<<132, 256, 0, st>>>(h->d, (const double *)rows_above_dev, (const double *)rows_below_dev, h->cs_K);
-    else
-        emu_csdvs_unpack_kernel<float><<<132, 256, 0, st>>>(h->d, (const float *)rows_above_dev, (const float *)rows_below_dev, h->cs_K);
+    with_state_type(h->d, [&](auto s) {
+        using S = decltype(s);
+        emu_csdvs_unpack_kernel<S><<<132, 256, 0, st>>>(h->d, (const S *)rows_above_dev, (const S *)rows_below_dev, h->cs_K);
+    });
     CU(cudaGetLastError());
     return V2E_OK;
 }
@@ -3692,9 +3641,8 @@ extern "C" int v2e_emu_cs_update(V2eEmu *h, const void *frame, int dtype, const 
     if (d.rng_mode == 0 && d.leak_on && !lr) return fail(V2E_E_INVALID, "leak_randn field required in replay mode");
     cudaStream_t st = (cudaStream_t)stream;
     probe_note_frame(h, 0, frame, dtype);
-    int rc = d.state_f64 ? launch_update<double>(h, h->cs_p, frame, dtype, lr, sr, 0, 0, 1, st)
-                         : launch_update<float>(h, h->cs_p, frame, dtype, lr, sr, 0, 0, 1, st);
-    if (rc) return rc;
+    int rc;
+    if ((rc = launch_update(h, h->cs_p, frame, dtype, lr, sr, 0, 0, 1, st))) return rc;
     CU(cudaGetLastError());
     h->cs_pending = 0;
     return V2E_OK;
