@@ -1,5 +1,6 @@
-"""Per-layer timing of the per-tap convolution's tiles (csrc/conv_tc.cu): the 128 x 128 tile against the wide tiles,
-with and without weight multicast over CTA pairs, at the shapes the headline runs them at.
+"""Per-layer timing of the per-tap convolution's tiles (csrc/conv_tc.cu): the 128 x 128 tile ("legacy") against the
+wide tile the layer's shape calls for ("wide": 256 x 128 at 128 output channels, else 128 x 256), at the shapes the
+headline runs them at.
 
     python bench_conv.py [--size 1280|320] [--iters 100] [--warmup 20] [--layers down4.c1,up1.c2]
 
@@ -7,7 +8,7 @@ For every per-tap layer of the UNets the variants are launched in turn, each tim
 back-to-back launches after --warmup launches, and the rounds alternate (--rounds) so that clock drift hits every
 variant alike; the median round is reported. Per layer and variant: ms per launch, TFLOP/s (2 * pixels * Cout * Cin *
 9 / time) and the bytes the CTAs request from L2 into shared memory per second, counted from the tiling: launched
-CTAs x (tap, slab) stages x bytes issued per stage (A window + the weight slab, or half of it when multicast). The
+CTAs x (tap, slab) stages x bytes issued per stage (A window + the weight slab). The
 card's name, power limit and SM clock are read in the same process. One JSON line at the end."""
 import argparse
 import ctypes
@@ -34,15 +35,13 @@ TAP_LAYERS = [("down2.c1", 64, 0, 128, 2), ("down2.c2", 128, 0, 128, 2),
 SIZES = {"1280": (8, 704, 1280), "320": (30, 256, 320)}
 
 
-def l2_bytes(tile, mc, N, H, W, C, Cout):
+def l2_bytes(tile, N, H, W, C, Cout):
     """CTAs x stages x bytes per stage the producers issue (KC = 64 for every per-tap layer)."""
     mh, bn = {LEGACY: (1, min(Cout, 128)), T256x128: (2, 128), T128x256: (1, 256)}[tile]
     tiles = -(-W // 16) * -(-H // (8 * mh)) * N
-    if tile != LEGACY and mc:
-        tiles += tiles & 1
     ctas = tiles * (Cout // bn)
     a = 128 * mh * 64 * 2
-    b = bn * 64 * 2 // (2 if (tile != LEGACY and mc) else 1)
+    b = bn * 64 * 2
     return ctas * 9 * (C // 64) * (a + b), ctas
 
 
@@ -87,39 +86,39 @@ def main():
         b = torch.zeros(co, device="cuda:0")
         out = torch.empty((N, H, W, co), dtype=torch.float16, device="cuda:0")
         wide = T256x128 if co == 128 else T128x256
-        variants = [("legacy", LEGACY, 0), ("wide", wide, 1), ("wide_unicast", wide, 0)]
+        variants = [("legacy", LEGACY), ("wide", wide)]
 
-        def launch(tile, mc):
+        def launch(tile):
             _lib.check(L.v2e_conv2d_lrelu_sm100_tile(p(x1), c1, p(x2), c2, p(w), p(b), co, 3, 3, N, H, W, p(out), co,
-                                                     0, co, ctypes.c_float(0.1), tile, mc, stp))
+                                                     0, co, ctypes.c_float(0.1), tile, stp))
 
         times = {v[0]: [] for v in variants}
         for _ in range(a.rounds):
-            for vn, tile, mc in variants:
+            for vn, tile in variants:
                 for _ in range(a.warmup):
-                    launch(tile, mc)
+                    launch(tile)
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record(st)
                 for _ in range(a.iters):
-                    launch(tile, mc)
+                    launch(tile)
                 e1.record(st)
                 e1.synchronize()
                 times[vn].append(e0.elapsed_time(e1) / a.iters)
         flops = 2.0 * N * H * W * co * (c1 + c2) * 9
         row = {"layer": name, "shape": [N, H, W, c1 + c2, co]}
-        for vn, tile, mc in variants:
+        for vn, tile in variants:
             ms = sorted(times[vn])[len(times[vn]) // 2]
-            by, ctas = l2_bytes(tile, mc, N, H, W, c1 + c2, co)
+            by, ctas = l2_bytes(tile, N, H, W, c1 + c2, co)
             row[vn] = {"ms": round(ms, 4), "tflops": round(flops / ms / 1e9, 1), "l2_tb_s": round(by / ms / 1e9, 2),
                        "ctas": ctas, "spread_ms": round(max(times[vn]) - min(times[vn]), 4)}
         rows.append(row)
         print("%-9s %-22s" % (name, "x".join(map(str, row["shape"]))) +
               "".join("  %s %.3f ms %5.0f TF/s %4.2f TB/s" % (vn, row[vn]["ms"], row[vn]["tflops"], row[vn]["l2_tb_s"])
-                      for vn, _, _ in variants), flush=True)
+                      for vn, _ in variants), flush=True)
         del x1, x2, w, out
     res = {"what": "per-tap convolution tiles at %s (batch %d)" % (a.size, N), "card": card_before,
            "card_after": card(), "iters": a.iters, "rounds": a.rounds, "layers": rows}
-    for vn in ("legacy", "wide", "wide_unicast"):
+    for vn in ("legacy", "wide"):
         res["total_ms_" + vn] = round(sum(r[vn]["ms"] for r in rows), 3)
     print(json.dumps(res))
 

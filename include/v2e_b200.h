@@ -375,10 +375,8 @@ int v2e_conv2d_lrelu_sm100(const void *x1_dev, int C1, const void *x2_dev, int C
 
 /* Per-tap tiles of v2e_conv2d_lrelu_sm100 (output pixels x output channels per CTA). AUTO: the tile
  * v2e_conv_pick_tile chooses for the layer on the current device, what v2e_conv2d_lrelu_sm100 and the SloMo
- * networks run (the multicast argument is then ignored). LEGACY: 128 x min(Cout_pad, 128). The wide tiles need
- * 64-channel slabs (C1, C2 multiples of 64), fp16 output (out_mode 0) and Cout_pad a multiple of their width; with
- * multicast != 0 their CTAs run in pairs (clusters of 2) that share one weight slab per stage. Every tile gives the
- * same output bit for bit. */
+ * networks run. LEGACY: 128 x min(Cout_pad, 128). The wide tiles need 64-channel slabs (C1, C2 multiples of 64),
+ * fp16 output (out_mode 0) and Cout_pad a multiple of their width. Every tile gives the same output bit for bit. */
 enum {
     V2E_CONV_TILE_AUTO = -1,
     V2E_CONV_TILE_LEGACY = 0,
@@ -388,7 +386,7 @@ enum {
 int v2e_conv2d_lrelu_sm100_tile(const void *x1_dev, int C1, const void *x2_dev, int C2,
                                 const void *wgt_dev, const float *bias_dev, int Cout_pad, int KH, int KW,
                                 int N, int H, int W, void *out_dev, int out_cstride, int out_mode,
-                                int co_real, float slope, int tile, int multicast, void *stream);
+                                int co_real, float slope, int tile, void *stream);
 /* The tile AUTO picks for a layer on a device with n_sms SMs (wave-aware cost; no GPU needed). */
 int v2e_conv_pick_tile(int C1, int C2, int Cout_pad, int KH, int KW, int N, int H, int W, int n_sms);
 
@@ -448,9 +446,8 @@ int v2e_slomo_interp(V2eSlomo *h, double t, uint8_t *out_u8_dev, float *out_f32_
  * visibility) or blended pixel was inf / nan -- what fp16 activations beyond 65504 turn into. Resets the flag.
  * Synchronises. The Python class raises FloatingPointError on it (no silent garbage frames). */
 int v2e_slomo_check_finite(V2eSlomo *h, int *nonfinite_host, void *stream);
-/* option 0: force the per-tap convolution kernel for every layer; option 1: do not fold the up-sampling into
- * up5.conv1; option 2: do not fuse the average pools into the epilogues of conv2 / down1.conv2 (A/B measurements
- * and bit-identity tests: the fused pool must equal the separate kernel exactly), value 0/1;
+/* option 2: do not fuse the average pools into the epilogues of conv2 / down1.conv2 (the bit-identity test: the
+ * fused pool must equal the separate kernel exactly), value 0/1;
  * option 3: plan every later launch (per-tap tile pick, strip and up-sampling grids and their segmentation) as if
  * the device had `value` SMs, 1 <= value <= the device's count; 0 restores the device's count (the default). A test
  * hook: the outputs must not depend on it. Other values: V2E_E_INVALID. */

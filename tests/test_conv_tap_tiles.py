@@ -2,7 +2,7 @@
 
 Both accumulate every output element's terms in the same (tap, slab, k16) order, so the fp16 outputs are equal bit
 for bit; the GPU tests compare them with torch.equal at the shapes the UNets run them at and at edge cases of the
-cluster-pair grid. The CPU tests pin the tile v2e_conv_pick_tile chooses per layer and read the compiled kernels'
+wide tiles' grid. The CPU tests pin the tile v2e_conv_pick_tile chooses per layer and read the compiled kernels'
 SASS (asynchronous wgmma chains, no local-memory spills)."""
 import ctypes
 import os
@@ -94,16 +94,16 @@ def _wide_sass():
     return funcs
 
 
-def test_wide_kernels_chain_their_wgmmas_and_do_not_spill():
+def test_both_wide_kernels_chain_their_wgmmas_and_do_not_spill():
     funcs = _wide_sass()
-    assert len(funcs) == 4, sorted(funcs)          # {256x128, 128x256} x {multicast, not}
+    assert len(funcs) == 2, sorted(funcs)          # 256x128, 128x256
     bad = {k: v for k, v in funcs.items() if v["depbar"] >= v["hgmma"] or v["local"]}
     assert not bad, "serialised wgmma chains or local-memory spills: %r" % bad
 
 
 # ---- GPU: wide tiles equal the 128 x 128 tile bit for bit ---------------------------------------------------------
 def _run(case, tiles, seed):
-    """One random layer (N, H, W, C1, C2, Cout) through each (tile, multicast) of `tiles`; the fp16 outputs."""
+    """One random layer (N, H, W, C1, C2, Cout) through each tile of `tiles`; the fp16 outputs."""
     import torch
     N, H, W, C1, C2, Cout = case
     L = _lib.load()
@@ -116,10 +116,10 @@ def _run(case, tiles, seed):
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     p = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
     outs = []
-    for tile, mc in tiles:
+    for tile in tiles:
         out = torch.full((N, H, W, Cout), float("nan"), dtype=torch.float16, device="cuda:0")
         _lib.check(L.v2e_conv2d_lrelu_sm100_tile(p(x1), C1, p(x2), C2, p(w), p(b), Cout, 3, 3, N, H, W, p(out), Cout,
-                                                 0, Cout, ctypes.c_float(0.1), tile, mc, st))
+                                                 0, Cout, ctypes.c_float(0.1), tile, st))
         outs.append(out)
     torch.cuda.synchronize()
     return outs
@@ -129,8 +129,8 @@ def _assert_all_equal(case, tiles, seed=0):
     import torch
     outs = _run(case, tiles, seed)
     assert not torch.isnan(outs[0]).any()
-    for (tile, mc), o in zip(tiles[1:], outs[1:]):
-        assert torch.equal(o, outs[0]), "tile %d multicast %d differs from the 128 x 128 tile at %r" % (tile, mc, case)
+    for tile, o in zip(tiles[1:], outs[1:]):
+        assert torch.equal(o, outs[0]), "tile %d differs from the 128 x 128 tile at %r" % (tile, case)
 
 
 @pytest.mark.gpu
@@ -141,17 +141,17 @@ def test_wide_tiles_equal_the_legacy_tile_at_production_shapes(layer, size):
     N, H, W = SIZES[size]
     case = (N, H >> lvl, W >> lvl, c1, c2, co)
     wt = wide_tile(co)
-    _assert_all_equal(case, [(LEGACY, 0), (wt, 1), (wt, 0), (AUTO, 1)], seed=lvl * 131 + co + c2)
+    _assert_all_equal(case, [LEGACY, wt, AUTO], seed=lvl * 131 + co + c2)
 
 
 EDGE_CASES = [
     # N, H, W, C1, C2, Cout
-    (1, 24, 48, 256, 0, 256),        # 3 x 3 = 9 tiles of 8x16: odd count, one padding CTA in the cluster grid
+    (1, 24, 48, 256, 0, 256),        # 3 x 3 = 9 tiles of 8x16, one output-channel block
     (1, 40, 48, 128, 0, 128),        # 3 x 3 = 9 tiles of 16x16 (H not a multiple of 16), one output-channel block
-    (3, 36, 36, 64, 64, 128),        # concatenated inputs, 16x16 tiles cut at both edges, odd count (27 + pad)
+    (3, 36, 36, 64, 64, 128),        # concatenated inputs, 16x16 tiles cut at both edges, 3 x 9 tiles
     (1, 9, 23, 256, 256, 512),       # concatenated inputs, 8x16 tiles cut at both edges, two channel blocks
     (1, 16, 32, 512, 0, 512),        # one wave: 2 tiles x 2 channel blocks
-    (1, 8, 16, 128, 0, 256),         # a single tile: the pair is the tile and its padding CTA
+    (1, 8, 16, 128, 0, 256),         # a single tile
     (2, 5, 7, 64, 0, 128),           # smaller than one tile
 ]
 
@@ -159,12 +159,12 @@ EDGE_CASES = [
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", EDGE_CASES)
 def test_wide_tiles_equal_the_legacy_tile_at_edge_cases(case):
-    _assert_all_equal(case, [(LEGACY, 0), (wide_tile(case[5]), 1), (wide_tile(case[5]), 0)])
+    _assert_all_equal(case, [LEGACY, wide_tile(case[5])])
 
 
 @pytest.mark.gpu
 def test_128x256_tile_at_cout_128_is_refused_and_256x128_runs_at_cout_512():
     """Cout_pad must be a multiple of the tile width; the 16x16 tile also runs where the pick does not choose it."""
     with pytest.raises(Exception):
-        _run((1, 8, 16, 64, 0, 128), [(T128x256, 1)], 0)
-    _assert_all_equal((2, 44, 80, 256, 0, 512), [(LEGACY, 0), (T256x128, 1), (T256x128, 0)])
+        _run((1, 8, 16, 64, 0, 128), [T128x256], 0)
+    _assert_all_equal((2, 44, 80, 256, 0, 512), [LEGACY, T256x128])

@@ -10,7 +10,6 @@ independent numpy restatement of the streams (oracle/philox.py).
 """
 import collections
 import ctypes
-import hashlib
 import math
 
 import numpy as np
@@ -280,61 +279,6 @@ def test_headline_cli_defaults_1280x720(headline):
     # shot rate 0.001 Hz: about 20 shot events per polarity in the clip; c3_1280x720 runs the same kernels with
     # tens of thousands
     report("headline_cli_1280x720", dev, "-")
-
-
-def _digest(rows, counts, state):
-    h = hashlib.sha1()
-    for r in rows:
-        h.update(np.ascontiguousarray(r).tobytes())
-    h.update(repr(counts).encode())
-    for k in sorted(state):
-        h.update(k.encode() + np.ascontiguousarray(state[k]).tobytes())
-    return h.hexdigest()
-
-
-def _fused_cfg_worker(cfg, q):
-    import os
-    os.environ["V2E_FUSED_CFG"] = str(cfg)         # read once per process, at the first multi-frame launch
-    out = {}
-    for name, (kw, make, opts) in _FUSED_CFG_CASES.items():
-        frames, ts = make()
-        em, dev = run_device(kw, frames, ts, **opts)
-        out[name] = (_digest(dev["rows"], dev["counts"], dev["state"]), dev["chunks"], dev["rejected"])
-        em.cleanup()
-    q.put((cfg, out))
-
-
-_FUSED_CFG_CASES = {
-    "headline": (CLI_DEFAULTS, lambda: (smooth_clip(720, 1280, 25, seed=11), [k / 300. for k in range(25)]),
-                 dict(mfps=24)),
-    "sigma0_37x53": (CASES["sigma0_37x53"][0], CASES["sigma0_37x53"][1], CASES["sigma0_37x53"][2]),
-}
-
-
-def test_fused_block_shapes_equal_oracle(headline):
-    """V2E_FUSED_CFG 0..3 (block shapes of the multi-frame update kernel; read once per process): each in a fresh
-    spawned process, the headline and a 37x53 clip must give the oracle's rows, counters and state."""
-    import torch.multiprocessing as mp
-    want = {"headline": _digest(headline["ref"]["rows"], headline["ref"]["counts"], headline["ref"]["state"])}
-    kw, make, opts = _FUSED_CFG_CASES["sigma0_37x53"]
-    frames, ts = make()
-    em, _ = run_device(kw, frames, ts, **opts)
-    ref = run_oracle(em, kw, frames, ts)
-    want["sigma0_37x53"] = _digest(ref["rows"], ref["counts"], ref["state"])
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_fused_cfg_worker, args=(c, q)) for c in range(4)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=600) for _ in procs)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
-    for c in range(4):
-        for name in want:
-            digest, chunks, rejected = got[c][name]
-            assert digest == want[name], (c, name)
-            assert chunks >= 1 and rejected == 0, (c, name, chunks, rejected)
 
 
 # ---- call paths: the frame-index contract --------------------------------------------------------------------------

@@ -52,7 +52,7 @@ class V2eProbeSample(ctypes.Structure):
 
 V2E_OK, V2E_E_INVALID, V2E_E_CUDA, V2E_E_CAPACITY, V2E_E_ITER_CAP, V2E_E_STATE, V2E_E_UNSUPPORTED, V2E_E_FALLBACK = \
     0, -1, -2, -3, -4, -5, -6, -7
-ABI_VERSION = 203
+ABI_VERSION = 204
 U8, F32, F64 = 0, 1, 2
 
 _vp, _i, _d, _u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint64
@@ -100,7 +100,7 @@ _SIGS = {
     "v2e_conv2d_lrelu_sm100": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
                                     ctypes.c_float, _vp]),
     "v2e_conv2d_lrelu_sm100_tile": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
-                                         ctypes.c_float, _i, _i, _vp]),
+                                         ctypes.c_float, _i, _vp]),
     "v2e_conv_pick_tile": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _i]),
     "v2e_conv2d_lrelu_sm100_strip": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
                                           ctypes.c_float, _vp]),

@@ -27,7 +27,6 @@
 #include <stdio.h>
 #include <string.h>
 #include <vector>
-#include <stdlib.h>
 
 #include "../../include/v2e_b200.h"
 #include "common.cuh"
@@ -50,7 +49,7 @@ struct ConvParams {
     int stages;                 // depth of the producer / consumer ring (<= kStages)
     int co_fast;                // grid order: 1 = output-channel blocks in gridDim.x
     int tiles_x, tiles_y;
-    int n_tiles;                // pixel tiles (conv_wide_kernel: the grid may hold one padding CTA more)
+    int n_tiles;                // pixel tiles
     int out_cstride;            // channel stride (elements) of the fp16 NHWC output
     int out_mode;               // 0: fp16 NHWC; 1: fp32 [N,H,W,8], first co_real channels
     int co_real;
@@ -182,15 +181,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 //   MH = 1: 128 pixels (8x16) x BN = 256 channels; a warpgroup runs one m64n256 chain over its 64 pixels,
 //   MH = 2: 256 pixels (16x16) x BN = 128 channels; a warpgroup runs two m64n128 chains (its two 64-pixel quarters)
 //           over the same B slab.
-// MC: the CTAs of a cluster pair share the output-channel block and take neighbouring pixel tiles; each producer
-// loads half of the weight slab and multicasts it to both CTAs, so a stage costs A + B/2 bytes from L2 per CTA.
-// A stage is refilled only when the consumers of BOTH CTAs have released it (each consumer warp arrives on its own
-// and on the peer's empty barrier, 16 arrivals), and both CTAs pass a cluster barrier before they exit (the peer's
-// multicasts and remote arrivals target this CTA's shared memory). A grid with an odd pixel-tile count gets one
-// padding CTA, which loads the last tile's window and multicasts its half of the weights but stores nothing.
 // Every output element accumulates its terms in the order (tap, slab, k16) of conv_tc_kernel.
 // ---------------------------------------------------------------------------------------------
-template <int MH, int BN, bool MC>
+template <int MH, int BN>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                  const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
@@ -203,22 +196,16 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tile_g = p.co_fast ? blockIdx.y : blockIdx.x;
-    const bool live = tile_g < p.n_tiles;             // false: the padding CTA of an odd tile count
-    const int tile = live ? tile_g : p.n_tiles - 1;
+    const int tile = p.co_fast ? blockIdx.y : blockIdx.x;
     const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, n = tile / (p.tiles_x * p.tiles_y);
     const int x0 = tx * kTileW, y0 = ty * TH;
     const int n0 = (p.co_fast ? blockIdx.x : blockIdx.y) * BN;
     const int Ctot = p.C1 + p.C2;
     const int slabs = Ctot / p.KC;
     const int k_iters = p.KH * p.KW * slabs;
-    const uint32_t crank = MC ? cluster_ctarank() : 0u;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; s++) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], (MC ? 2 : 1) * kConsumerWarps);
-        }
+        for (int s = 0; s < kStages; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
         fence_barrier_init();
     }
     if (warp == kProducerWarp && lane == 0) {
@@ -226,9 +213,7 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (p.C2) prefetch_tmap(&tmA2);
         prefetch_tmap(&tmB);
     }
-    // the peer multicasts into this CTA's stages and arrives on its barriers: both CTAs' barriers are initialised first
-    if constexpr (MC) cluster_sync();
-    else __syncthreads();
+    __syncthreads();
 
     if (warp == kProducerWarp) {
         // ===== TMA producer =====
@@ -245,11 +230,7 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     const int c = sl * p.KC;
                     if (c < p.C1) tma_load_4d(sa, &tmA, &full_bar[stage], c, x0 + s - pw, y0 + r - ph, n);
                     else tma_load_4d(sa, &tmA2, &full_bar[stage], c - p.C1, x0 + s - pw, y0 + r - ph, n);
-                    if constexpr (MC)
-                        tma_load_2d_multicast(sb + crank * (b_bytes / 2), &tmB, &full_bar[stage], tap * Ctot + c,
-                                              n0 + (int)crank * (BN / 2), (uint16_t)0x3);
-                    else
-                        tma_load_2d(sb, &tmB, &full_bar[stage], tap * Ctot + c, n0);
+                    tma_load_2d(sb, &tmB, &full_bar[stage], tap * Ctot + c, n0);
                     if (++stage == p.stages) { stage = 0; phase ^= 1; }
                 }
             }
@@ -281,49 +262,40 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
             wgmma_commit();
             wgmma_wait<1>();                 // the stage before this one has been read: hand it back
-            if (prev >= 0) {
-                __syncwarp();
-                if (lane == 0) {
-                    mbar_arrive(&empty_bar[prev]);
-                    if constexpr (MC) mbar_arrive_cluster(&empty_bar[prev], crank ^ 1u);
-                }
-            }
+            if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
             prev = stage;
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
         }
         wgmma_wait<0>();
 #pragma unroll
         for (int h = 0; h < MH; h++) wgmma_fence_regs(acc[h]);
-        if (live) {
-            // bias + LeakyReLU + fp16 store of both rows of each 8-column group at once (one bias load per group
-            // keeps the 128 accumulators and the addresses within the register budget)
-            const float *bias = p.bias + n0;
-            __half *out = (__half *)p.out + n0;
+        // bias + LeakyReLU + fp16 store of both rows of each 8-column group at once (one bias load per group keeps the
+        // 128 accumulators and the addresses within the register budget)
+        const float *bias = p.bias + n0;
+        __half *out = (__half *)p.out + n0;
 #pragma unroll
-            for (int h = 0; h < MH; h++) {
-                size_t pix[2];
-                bool inb[2];
+        for (int h = 0; h < MH; h++) {
+            size_t pix[2];
+            bool inb[2];
 #pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const int m = 64 * (g * MH + h) + 16 * (warp & 3) + (lane >> 2) + 8 * i;
-                    const int py = y0 + m / kTileW, px = x0 + m % kTileW;
-                    inb[i] = py < p.H && px < p.W;
-                    pix[i] = (((size_t)n * p.H + py) * p.W + px) * p.out_cstride;
-                }
+            for (int i = 0; i < 2; i++) {
+                const int m = 64 * (g * MH + h) + 16 * (warp & 3) + (lane >> 2) + 8 * i;
+                const int py = y0 + m / kTileW, px = x0 + m % kTileW;
+                inb[i] = py < p.H && px < p.W;
+                pix[i] = (((size_t)n * p.H + py) * p.W + px) * p.out_cstride;
+            }
 #pragma unroll
-                for (int j = 0; j < BN / 8; j++) {
-                    const int c = 8 * j + 2 * (lane & 3);
-                    const float2 b = __ldg((const float2 *)(bias + c));
+            for (int j = 0; j < BN / 8; j++) {
+                const int c = 8 * j + 2 * (lane & 3);
+                const float2 b = __ldg((const float2 *)(bias + c));
 #pragma unroll
-                    for (int i = 0; i < 2; i++)
-                        if (inb[i])
-                            *(__half2 *)(out + pix[i] + c) = __floats2half2_rn(lrelu(acc[h][4 * j + 2 * i] + b.x, p.slope),
-                                                                               lrelu(acc[h][4 * j + 2 * i + 1] + b.y, p.slope));
-                }
+                for (int i = 0; i < 2; i++)
+                    if (inb[i])
+                        *(__half2 *)(out + pix[i] + c) = __floats2half2_rn(lrelu(acc[h][4 * j + 2 * i] + b.x, p.slope),
+                                                                           lrelu(acc[h][4 * j + 2 * i + 1] + b.y, p.slope));
             }
         }
     }
-    if constexpr (MC) cluster_sync();
 }
 
 
@@ -724,9 +696,9 @@ conv_up2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 // 1.4 % of the layer's pixels; the partial sums are ~0.2 in magnitude, fp16 rounding of them stays below
 // 1e-3 absolute), widened to float32 for the cross-lane reduction: a halving butterfly after which lane co holds
 // output channel co.
-// latency-bound (a warp's pixel is a serial chain of gathers, half2 FMAs and shuffles); block shape by template so
-// that occupancy against registers can be measured (V2E_BORDER_CFG: 0 = 4 warps x 4 blocks/SM, 1 = 4 x 5, 2 = 8 x 3)
-template <int kBorderThreads, int kBorderBlocks>
+// Latency-bound (a warp's pixel is a serial chain of gathers, half2 FMAs and shuffles): 4 warps x 4 blocks per SM.
+constexpr int kBorderThreads = 128, kBorderBlocks = 4;
+
 __global__ void __launch_bounds__(kBorderThreads, kBorderBlocks)
 conv_up2_border_kernel(const __half *__restrict__ L, const __half *__restrict__ wgt, const float *__restrict__ bias,
                        __half *__restrict__ out, int N, int H, int W, int out_cstride, float slope) {
@@ -881,7 +853,7 @@ static void tile_shape(int tile, int Cout_pad, int *mh, int *bn) {
     *bn = tile == V2E_CONV_TILE_128x256 ? 256 : (tile == V2E_CONV_TILE_256x128 ? 128 : v2e_conv_pick_bn(Cout_pad));
 }
 
-// Wave-aware choice of the tile (wide tiles without multicast, the default). A CTA's time per (tap, slab) stage is
+// Wave-aware choice of the tile. A CTA's time per (tap, slab) stage is
 // the larger of its L2-to-shared-memory bytes at ~24 B/clk per SM (6-7 TB/s over 132 SMs, the rate the 128 x 128
 // tile runs at) and its MMAs at 4096 dense fp16 FLOP/clk per SM; every tile runs the same stages per CTA, so a layer
 // costs waves x (time per stage). One CTA per SM (the stages fill the shared memory). Ties go to the 128 x 128 tile.
@@ -913,33 +885,17 @@ extern "C" int v2e_conv_pick_tile(int C1, int C2, int Cout_pad, int KH, int KW, 
 struct V2eConvLaunch {
     CUtensorMap tmA, tmA2, tmB;
     ConvParams p;
-    dim3 grid, cluster;
-    int mh, multicast;
+    dim3 grid;
+    int mh;
     size_t smem;
 };
 
-// V2E_CONV_TILE (A/B measurements): "legacy" = the 128 x 128 tile for every layer, "multicast" = the picked tiles,
-// the wide ones with weight multicast over CTA pairs; unset = the picked tiles without multicast (on an H100 the
-// pairs took about 1.5x as long as unicast wide tiles, DESIGN.md section 5)
-static int conv_tile_env() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("V2E_CONV_TILE");
-        v = !e ? 0 : (!strcmp(e, "legacy") ? 1 : (!strcmp(e, "multicast") ? 2 : 0));
-    }
-    return v;
-}
-
 int v2e_conv_prepare(V2eConvLaunch *L, const void *x1, int C1, const void *x2, int C2, const void *wgt,
                      const float *bias, int Cout_pad, int KH, int KW, int N, int H, int W, void *out,
-                     int out_cstride, int out_mode, int co_real, float slope, int tile, int multicast, int n_sms) {
+                     int out_cstride, int out_mode, int co_real, float slope, int tile, int n_sms) {
     if (C1 % 16 || C2 % 16 || !(Cout_pad == 16 || Cout_pad == 32 || Cout_pad == 64 || (Cout_pad > 0 && Cout_pad % 128 == 0)))
         return v2e_set_error(V2E_E_INVALID, "conv: channel counts must be padded to 16 (Cout to 16/32/64/128k)%s", "");
-    if (tile == V2E_CONV_TILE_AUTO) {
-        const int env = conv_tile_env();
-        tile = env == 1 ? V2E_CONV_TILE_LEGACY : v2e_conv_pick_tile(C1, C2, Cout_pad, KH, KW, N, H, W, n_sms);
-        multicast = env == 2;
-    }
+    if (tile == V2E_CONV_TILE_AUTO) tile = v2e_conv_pick_tile(C1, C2, Cout_pad, KH, KW, N, H, W, n_sms);
     if (tile < V2E_CONV_TILE_LEGACY || tile > V2E_CONV_TILE_128x256)
         return v2e_set_error(V2E_E_INVALID, "conv: unknown tile%s", "");
     memset(L, 0, sizeof(*L));
@@ -959,21 +915,14 @@ int v2e_conv_prepare(V2eConvLaunch *L, const void *x1, int C1, const void *x2, i
     p.out_cstride = out_cstride; p.out_mode = out_mode; p.co_real = co_real; p.slope = slope;
     p.bias = bias; p.out = out;
     L->mh = mh;
-    L->multicast = wide && multicast;
     int rc;
     if ((rc = make_act_tmap_h(&L->tmA, x1, N, H, W, C1, p.KC, kTileH * mh))) return rc;
     if (C2) { if ((rc = make_act_tmap_h(&L->tmA2, x2, N, H, W, C2, p.KC, kTileH * mh))) return rc; }
     else L->tmA2 = L->tmA;
-    if ((rc = v2e_make_wgt_tmap(&L->tmB, wgt, Cout_pad, KH * KW * (C1 + C2), p.KC, L->multicast ? bn / 2 : bn))) return rc;
-    {
-        static int co_fast = -1;
-        if (co_fast < 0) { const char *e = getenv("V2E_CONV_CO_FAST"); co_fast = e ? atoi(e) : 1; }
-        // a multicast pair is two neighbouring pixel tiles: an odd count gets one padding CTA
-        const unsigned tiles = (unsigned)(L->multicast ? (p.n_tiles + 1) & ~1 : p.n_tiles), cob = (unsigned)(Cout_pad / p.BN);
-        p.co_fast = (co_fast && cob > 1 && tiles <= 65535u) ? 1 : 0;
-        L->grid = p.co_fast ? dim3(cob, tiles, 1) : dim3(tiles, cob, 1);
-        L->cluster = !L->multicast ? dim3(1, 1, 1) : (p.co_fast ? dim3(1, 2, 1) : dim3(2, 1, 1));
-    }
+    if ((rc = v2e_make_wgt_tmap(&L->tmB, wgt, Cout_pad, KH * KW * (C1 + C2), p.KC, bn))) return rc;
+    const unsigned tiles = (unsigned)p.n_tiles, cob = (unsigned)(Cout_pad / p.BN);
+    p.co_fast = (cob > 1 && tiles <= 65535u) ? 1 : 0;
+    L->grid = p.co_fast ? dim3(cob, tiles, 1) : dim3(tiles, cob, 1);
     size_t stage = (size_t)kBM * mh * p.KC * 2 + (((size_t)p.BN * p.KC * 2 + 1023) & ~(size_t)1023);
     L->smem = stage * p.stages + 1024;
     return V2E_OK;
@@ -987,30 +936,19 @@ static cudaError_t conv_launch_bn(const V2eConvLaunch *L, cudaStream_t st) {
     return cudaGetLastError();
 }
 
-template <int MH, int BN, bool MC>
+template <int MH, int BN>
 static cudaError_t conv_launch_wide(const V2eConvLaunch *L, cudaStream_t st) {
     static PerDeviceOnce attr_once;
     if (attr_once.first())
-        cudaFuncSetAttribute(conv_wide_kernel<MH, BN, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = L->grid;
-    cfg.blockDim = dim3(kConvThreads, 1, 1);
-    cfg.dynamicSmemBytes = L->smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = L->cluster.x;
-    attr[0].val.clusterDim.y = L->cluster.y;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, conv_wide_kernel<MH, BN, MC>, L->tmA, L->tmA2, L->tmB, L->p);
+        cudaFuncSetAttribute(conv_wide_kernel<MH, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    conv_wide_kernel<MH, BN><<<L->grid, kConvThreads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p);
+    return cudaGetLastError();
 }
 
 int v2e_conv_launch(const V2eConvLaunch *L, cudaStream_t st) {
     cudaError_t e;
-    if (L->mh == 2 && L->p.BN == 128) e = L->multicast ? conv_launch_wide<2, 128, true>(L, st) : conv_launch_wide<2, 128, false>(L, st);
-    else if (L->mh == 1 && L->p.BN == 256) e = L->multicast ? conv_launch_wide<1, 256, true>(L, st) : conv_launch_wide<1, 256, false>(L, st);
+    if (L->mh == 2 && L->p.BN == 128) e = conv_launch_wide<2, 128>(L, st);
+    else if (L->mh == 1 && L->p.BN == 256) e = conv_launch_wide<1, 256>(L, st);
     else switch (L->p.BN) {
         case 16: e = conv_launch_bn<16>(L, st); break;
         case 32: e = conv_launch_bn<32>(L, st); break;
@@ -1035,10 +973,10 @@ static int device_sms() {
 extern "C" int v2e_conv2d_lrelu_sm100_tile(const void *x1_dev, int C1, const void *x2_dev, int C2,
                                            const void *wgt_dev, const float *bias_dev, int Cout_pad, int KH, int KW,
                                            int N, int H, int W, void *out_dev, int out_cstride, int out_mode,
-                                           int co_real, float slope, int tile, int multicast, void *stream) {
+                                           int co_real, float slope, int tile, void *stream) {
     V2eConvLaunch L;
     int rc = v2e_conv_prepare(&L, x1_dev, C1, x2_dev, C2, wgt_dev, bias_dev, Cout_pad, KH, KW, N, H, W, out_dev,
-                              out_cstride, out_mode, co_real, slope, tile, multicast, device_sms());
+                              out_cstride, out_mode, co_real, slope, tile, device_sms());
     if (rc) return rc;
     return v2e_conv_launch(&L, (cudaStream_t)stream);
 }
@@ -1048,7 +986,7 @@ extern "C" int v2e_conv2d_lrelu_sm100(const void *x1_dev, int C1, const void *x2
                                       int N, int H, int W, void *out_dev, int out_cstride, int out_mode,
                                       int co_real, float slope, void *stream) {
     return v2e_conv2d_lrelu_sm100_tile(x1_dev, C1, x2_dev, C2, wgt_dev, bias_dev, Cout_pad, KH, KW, N, H, W, out_dev,
-                                       out_cstride, out_mode, co_real, slope, V2E_CONV_TILE_AUTO, 0, stream);
+                                       out_cstride, out_mode, co_real, slope, V2E_CONV_TILE_AUTO, stream);
 }
 
 // ---- strip kernel host side ------------------------------------------------------------------------
@@ -1100,21 +1038,13 @@ static int strip_config(int C1, int C2, int Cout_pad, int KH, int KW, int kc, in
     return 0;
 }
 
-static int strip_min_w() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("V2E_STRIP_MIN_W");
-        v = e ? atoi(e) : 2 * kRowTile;
-        if (v < kRowTile) v = kRowTile;
-    }
-    return v;
-}
+// wide layers only: narrow rows waste part of the last 128-pixel strip (320 = 2.5 strips) and the per-tap kernel's
+// 8x16 tiles take over
+constexpr int kStripMinW = 2 * kRowTile;
 
 // Slab width for the strip kernel; returns KC (0: layer does not qualify), *nslot_out.
 int v2e_strip_pick(int C1, int C2, int Cout_pad, int KH, int KW, int W, int *nslot_out) {
-    // wide layers only: narrow rows waste part of the last 128-pixel strip (320 = 2.5 strips) and the per-tap
-    // kernel's 8x16 tiles take over. V2E_STRIP_MIN_W overrides the threshold for A/B measurements.
-    if (Cout_pad > 64 || KH != KW || W < strip_min_w() || (KW != 3 && KW != 5 && KW != 7)) return 0;
+    if (Cout_pad > 64 || KH != KW || W < kStripMinW || (KW != 3 && KW != 5 && KW != 7)) return 0;
     const int g = C2 ? (C1 < C2 ? C1 : C2) : C1;
     const int kc = g % 64 == 0 ? 64 : (g % 32 == 0 ? 32 : 16);
     int ns, cps, nsp;
@@ -1262,7 +1192,7 @@ struct V2eUpLaunch {
 
 // 64-channel slabs, Cout_pad = 32, folded weights resident: slabs * 36 tiles of 32 x 64 fp16, + 3 ring rows
 int v2e_conv_up2_supported(int C, int Cout_pad, int W_out) {
-    if (C != 64 || Cout_pad != 32 || W_out % 2 || W_out < 2 * strip_min_w()) return 0;   // the frame kernel is written for C = 64
+    if (C != 64 || Cout_pad != 32 || W_out % 2 || W_out < 2 * kStripMinW) return 0;   // the frame kernel is written for C = 64
     const size_t wb = (size_t)(C / 64) * 2 * 3 * kUpBlocks * Cout_pad * 64 * 2;
     const size_t slab = ((size_t)(kRowTile + 2) * 64 * 2 + 1023) & ~(size_t)1023;
     return wb + 2048 + 3 * slab * (C / 64) <= kSmemFull;
@@ -1356,24 +1286,11 @@ int v2e_conv_up2_launch(const V2eUpLaunch *L, cudaStream_t st) {
     conv_up2_kernel<<<L->grid, kStripThreads, L->smem, st>>>(L->tmA, L->tmB, L->p);
     // the 2-pixel frame, where clamping / zero padding break the shift invariance the folding relies on
     const StripParams &p = L->p;
-    static int skip_frame = -1;                                   // measurement only: time the main kernel alone
-    if (skip_frame < 0) skip_frame = getenv("V2E_UP2_NO_FRAME") ? 1 : 0;
-    if (skip_frame) return V2E_OK;
-    static PerDeviceOnce battr_once;
-    if (battr_once.first()) {
-        cudaFuncSetAttribute(conv_up2_border_kernel<128, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 9 * 64 * 2);
-        cudaFuncSetAttribute(conv_up2_border_kernel<128, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 9 * 64 * 2);
-        cudaFuncSetAttribute(conv_up2_border_kernel<256, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 9 * 64 * 2);
-    }
-    static int bcfg = -1;
-    if (bcfg < 0) { const char *e = getenv("V2E_BORDER_CFG"); bcfg = e ? atoi(e) : 0; }
     const size_t bsm = 32 * 9 * 64 * 2;
-    if (bcfg == 1)
-        conv_up2_border_kernel<128, 5><<<L->grid * 5, 128, bsm, st>>>(L->low, L->w_plain, p.bias, (__half *)p.out, p.N, p.H, p.W, p.out_cstride, p.slope);
-    else if (bcfg == 2)
-        conv_up2_border_kernel<256, 3><<<L->grid * 3, 256, bsm, st>>>(L->low, L->w_plain, p.bias, (__half *)p.out, p.N, p.H, p.W, p.out_cstride, p.slope);
-    else
-        conv_up2_border_kernel<128, 4><<<L->grid * 4, 128, bsm, st>>>(L->low, L->w_plain, p.bias, (__half *)p.out, p.N, p.H, p.W, p.out_cstride, p.slope);
+    static PerDeviceOnce battr_once;
+    if (battr_once.first()) cudaFuncSetAttribute(conv_up2_border_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bsm);
+    conv_up2_border_kernel<<<L->grid * kBorderBlocks, kBorderThreads, bsm, st>>>(L->low, L->w_plain, p.bias, (__half *)p.out,
+                                                                                 p.N, p.H, p.W, p.out_cstride, p.slope);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "conv_up2_kernel launch: %s", cudaGetErrorString(e));
     return V2E_OK;

@@ -1554,12 +1554,16 @@ __device__ __forceinline__ uint32_t state_byte(const PlaneDev &pl, int s, double
     return np_u8(((x - pl.lo[s]) / pl.span[s]) * 255.0);
 }
 
+// Block shape of pass 1: 4 warps per block, 5 blocks per SM (20 resident warps, 96 registers). The kernel is bound by
+// dependent-instruction latency, so what matters is (resident warps) against (units per warp, an integer).
+constexpr int kFusedWarps = 4, kFusedMinBlocks = 5;
+
 // The multi-frame update (pass 1), shared by the kernel without planes (emu_fused_update_kernel) and the one that
 // writes them (emu_fused_update_planes_kernel). PROBE: the thread that owns a probe pixel writes that pixel's sample of
 // every frame from its registers. PLANES: every thread writes its quad's bytes of the shown states of every frame
 // from its registers (new_frame, log_new_frame, lp_log_frame, the zero photoreceptor_noise_arr, base_log_frame after
 // the leak and before the events, diff_frame: the states that exist where the multi-frame kernels run).
-template <typename S, bool FAST, int WARPS, bool PROBE, bool PLANES>
+template <typename S, bool FAST, bool PROBE, bool PLANES>
 __device__ __forceinline__ void
 fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
                   S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
@@ -1575,8 +1579,8 @@ fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint
     {
         const uint4 *src = (const uint4 *)ff;
         uint4 *dst = (uint4 *)s_dyn;
-        for (int i = tid; i < T * 2; i += WARPS * 32) dst[i] = src[i];
-        for (int i = tid; i < 256; i += WARPS * 32) s_tab[i] = make_double2((double)d.lut[i], inten01_of((double)i));
+        for (int i = tid; i < T * 2; i += kFusedWarps * 32) dst[i] = src[i];
+        for (int i = tid; i < 256; i += kFusedWarps * 32) s_tab[i] = make_double2((double)d.lut[i], inten01_of((double)i));
     }
     __syncthreads();
     if (*(volatile int32_t *)d.abort_flag) return;
@@ -1587,7 +1591,7 @@ fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint
     const S tp_nom = (S)d.pos_nom, tn_nom = (S)d.neg_nom;
     // every frame's row of bytes at a quad is 4-byte aligned iff the frame size is a multiple of 4 (and the base is)
     const bool al = ((n & 3) == 0) && ((((uintptr_t)frames) & 3) == 0);
-    for (int unit = u0 + warp; unit < u1; unit += WARPS) {
+    for (int unit = u0 + warp; unit < u1; unit += kFusedWarps) {
         const int i0 = unit * kUnitPx + lane * kVec;
         const int valid = i0 < d.n ? min(4, d.n - i0) : 0;          // pixels of this quad inside the frame
         const uint8_t *pf0 = frames + i0;
@@ -1718,24 +1722,23 @@ fused_update_body(const EmuDev &d, const FusedFrame *__restrict__ ff, const uint
     }
 }
 
-// WARPS warps per block, MINB blocks per SM: the register budget / occupancy / tail trade-off is picked on the host
-// (launch_fused_update). Units are dealt evenly to blocks and, inside a block, to warps. PROBE = false compiles to the
-// kernel without probes; the instantiation with them is launched only while probes are set.
-template <typename S, bool FAST, int WARPS, int MINB, bool PROBE>
-__global__ void __launch_bounds__(WARPS * 32, MINB)
+// Units are dealt evenly to blocks and, inside a block, to warps. PROBE = false compiles to the kernel without probes;
+// the instantiation with them is launched only while probes are set.
+template <typename S, bool FAST, bool PROBE>
+__global__ void __launch_bounds__(kFusedWarps * 32, kFusedMinBlocks)
 emu_fused_update_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
                         S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
                         uint32_t *__restrict__ rec_cnt, ProbeDev pr) {
     const PlaneDev pl{};
-    fused_update_body<S, FAST, WARPS, PROBE, false>(d, ff, frames, T, lp_out, base_out, rec_list, rec_cnt, pr, pl);
+    fused_update_body<S, FAST, PROBE, false>(d, ff, frames, T, lp_out, base_out, rec_list, rec_cnt, pr, pl);
 }
 // The same update writing the model-state planes (launched only while states are shown; probes may be set too).
-template <typename S, bool FAST, int WARPS, int MINB>
-__global__ void __launch_bounds__(WARPS * 32, MINB)
+template <typename S, bool FAST>
+__global__ void __launch_bounds__(kFusedWarps * 32, kFusedMinBlocks)
 emu_fused_update_planes_kernel(EmuDev d, const FusedFrame *__restrict__ ff, const uint8_t *__restrict__ frames, int T,
                                S *__restrict__ lp_out, S *__restrict__ base_out, uint16_t *__restrict__ rec_list,
                                uint32_t *__restrict__ rec_cnt, ProbeDev pr, PlaneDev pl) {
-    fused_update_body<S, FAST, WARPS, true, true>(d, ff, frames, T, lp_out, base_out, rec_list, rec_cnt, pr, pl);
+    fused_update_body<S, FAST, true, true>(d, ff, frames, T, lp_out, base_out, rec_list, rec_cnt, pr, pl);
 }
 
 // the records of up to 8 consecutive units of one frame as one list: off[k] = first list position of unit k
@@ -2180,9 +2183,9 @@ static int fail(int code, const char *fmt, const char *detail = "") {
 
 int v2e_set_error(int code, const char *fmt, const char *detail) { return fail(code, fmt, detail); }
 extern "C" const char *v2e_last_error(void) { return g_err; }
-extern "C" int v2e_version(void) { return 203; }
+extern "C" int v2e_version(void) { return 204; }
 extern "C" int v2e_abi_info(int *version, int *emu_cfg_size, int *frame_info_size, int *unet_weights_size) {
-    if (version) *version = 203;
+    if (version) *version = v2e_version();
     if (emu_cfg_size) *emu_cfg_size = (int)sizeof(V2eEmuCfg);
     if (frame_info_size) *frame_info_size = (int)sizeof(V2eFrameInfo);
     if (unet_weights_size) *unet_weights_size = (int)sizeof(V2eUNetWeights);
@@ -2790,47 +2793,25 @@ static int fused_alloc(V2eEmu *h) {
     return V2E_OK;
 }
 
-// Block shape of pass 1. The kernel is bound by dependent-instruction latency, so what matters is (resident warps)
-// against (units per warp, an integer): 0 = 8 warps x 3 blocks/SM (24 warps, 80 registers), 1 = 4 x 5 (20 warps,
-// 96 registers), 2 = 4 x 7 (28 warps, 72 registers), 3 = 8 x 2 (16 warps, 128 registers). V2E_FUSED_CFG overrides.
-static int fused_cfg() {
-    static int cfg = -1;
-    if (cfg < 0) {
-        const char *e = getenv("V2E_FUSED_CFG");
-        cfg = e ? atoi(e) : 1;
-        if (cfg < 0 || cfg > 3) cfg = 1;
-    }
-    return cfg;
-}
-template <typename S, bool FAST, int WARPS, int MINB>
-static void launch_fused_update_cfg(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, size_t sm,
-                                    const ProbeDev &pr, const PlaneDev &pl, cudaStream_t st) {
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int blocks = sms * MINB;
-    const int min_units = 2 * WARPS;                       // small frames: at least two units per warp
-    if (blocks > (d.units + min_units - 1) / min_units) blocks = (d.units + min_units - 1) / min_units;
-    if (blocks < 1) blocks = 1;
-    if (pl.mask)
-        emu_fused_update_planes_kernel<S, FAST, WARPS, MINB><<<blocks, WARPS * 32, sm, st>>>(
-            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr, pl);
-    else if (pr.n)
-        emu_fused_update_kernel<S, FAST, WARPS, MINB, true><<<blocks, WARPS * 32, sm, st>>>(
-            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr);
-    else
-        emu_fused_update_kernel<S, FAST, WARPS, MINB, false><<<blocks, WARPS * 32, sm, st>>>(
-            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr);
-}
 template <typename S, bool FAST>
 static void launch_fused_update_f(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, size_t sm,
                                   const ProbeDev &pr, const PlaneDev &pl, cudaStream_t st) {
-    switch (fused_cfg()) {
-        case 0: launch_fused_update_cfg<S, FAST, 8, 3>(h, d, ff, frames, T, sm, pr, pl, st); break;
-        case 2: launch_fused_update_cfg<S, FAST, 4, 7>(h, d, ff, frames, T, sm, pr, pl, st); break;
-        case 3: launch_fused_update_cfg<S, FAST, 8, 2>(h, d, ff, frames, T, sm, pr, pl, st); break;
-        default: launch_fused_update_cfg<S, FAST, 4, 5>(h, d, ff, frames, T, sm, pr, pl, st); break;
-    }
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int blocks = sms * kFusedMinBlocks;
+    const int min_units = 2 * kFusedWarps;                 // small frames: at least two units per warp
+    if (blocks > (d.units + min_units - 1) / min_units) blocks = (d.units + min_units - 1) / min_units;
+    if (blocks < 1) blocks = 1;
+    if (pl.mask)
+        emu_fused_update_planes_kernel<S, FAST><<<blocks, kFusedWarps * 32, sm, st>>>(
+            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr, pl);
+    else if (pr.n)
+        emu_fused_update_kernel<S, FAST, true><<<blocks, kFusedWarps * 32, sm, st>>>(
+            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr);
+    else
+        emu_fused_update_kernel<S, FAST, false><<<blocks, kFusedWarps * 32, sm, st>>>(
+            d, ff, frames, T, (S *)h->lp_alt, (S *)h->base_alt, h->rec_list, h->rec_cnt, pr);
 }
 // frames [a, a + T) of the step (d shifted to slot a)
 static int launch_fused_update(V2eEmu *h, const EmuDev &d, const FusedFrame *ff, const uint8_t *frames, int T, int a,

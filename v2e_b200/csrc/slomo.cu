@@ -17,7 +17,6 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
-#include <stdlib.h>
 
 #include <vector>
 
@@ -28,7 +27,7 @@
 struct V2eConvLaunch;
 int v2e_conv_prepare(V2eConvLaunch *L, const void *x1, int C1, const void *x2, int C2, const void *wgt,
                      const float *bias, int Cout_pad, int KH, int KW, int N, int H, int W, void *out,
-                     int out_cstride, int out_mode, int co_real, float slope, int tile, int multicast, int n_sms);
+                     int out_cstride, int out_mode, int co_real, float slope, int tile, int n_sms);
 int v2e_conv_launch(const V2eConvLaunch *L, cudaStream_t st);
 size_t v2e_conv_launch_size(void);
 struct V2eStripLaunch;
@@ -376,7 +375,7 @@ struct V2eSlomo {
     int *nonfinite;               // device flag: a network head or a blended pixel was inf / nan
     int curB;
     std::vector<char> launch_mem, row_mem, up_mem;
-    int n_sms, force_tap_kernel, no_fused_up, no_fused_pool;
+    int n_sms, no_fused_pool;
     int dev_sms;                  // the device's SM count; n_sms plans the launches (option 3 lowers it)
     int8_t ran[2][23];            // [flow, interp][layer]: V2E_SLOMO_KERNEL_* of the last launch (test hook)
     // measurement hooks: CUDA events around every conv launch
@@ -484,9 +483,7 @@ extern "C" int v2e_slomo_create(int H, int W, int max_batch, const V2eUNetWeight
     h->row_mem.resize(v2e_strip_launch_size());
     { int dev = 0; cudaGetDevice(&dev); h->n_sms = 132; cudaDeviceGetAttribute(&h->n_sms, cudaDevAttrMultiProcessorCount, dev); }
     h->dev_sms = h->n_sms;
-    h->force_tap_kernel = 0;
-    h->no_fused_up = getenv("V2E_NO_FUSED_UP") ? 1 : 0;        // A/B measurements
-    h->no_fused_pool = getenv("V2E_NO_FUSED_POOL") ? 1 : 0;
+    h->no_fused_pool = 0;
     h->up_mem.resize(v2e_conv_up2_launch_size());
     memset(h->ran, V2E_SLOMO_KERNEL_NONE, sizeof(h->ran));
     *out = h;
@@ -512,7 +509,7 @@ extern "C" int v2e_slomo_destroy(V2eSlomo *h) {
 static int conv(V2eSlomo *h, const UNet &u, int li, const __half *x1, const __half *x2, int B, int H, int W, void *out,
                 int out_mode, cudaStream_t st, __half *pool_out = nullptr) {
     int rc;
-    const bool row = u.row_kc[li] != 0 && !h->force_tap_kernel;
+    const bool row = u.row_kc[li] != 0;
     V2eConvLaunch *L = (V2eConvLaunch *)h->launch_mem.data();
     V2eStripLaunch *R = (V2eStripLaunch *)h->row_mem.data();
     h->ran[&u == &h->interp][li] = row ? (pool_out ? V2E_SLOMO_KERNEL_STRIP_POOL : V2E_SLOMO_KERNEL_STRIP)
@@ -524,7 +521,7 @@ static int conv(V2eSlomo *h, const UNet &u, int li, const __half *x1, const __ha
     else
         rc = v2e_conv_prepare(L, x1, u.c1p[li], x2, x2 ? u.c2p[li] : 0, u.w[li], u.b[li], u.cout_pad[li], u.L[li].k,
                               u.L[li].k, B, H, W, out, u.cout_pad[li], out_mode, u.L[li].cout, kSlope,
-                              V2E_CONV_TILE_AUTO, 0, h->n_sms);
+                              V2E_CONV_TILE_AUTO, h->n_sms);
     if (rc) return rc;
     if (h->profile) {
         if (h->ev_used + 2 > h->ev.size()) {
@@ -576,7 +573,7 @@ static int conv_up2(V2eSlomo *h, const UNet &u, int li, const __half *x_low, int
 
 // the average pool that opens a down block (model.py:71) can ride in the epilogue of the convolution before it
 static bool pool_fusable(const V2eSlomo *h, const UNet &u, int li, int H, int W) {
-    if (h->no_fused_pool || h->force_tap_kernel || !u.row_kc[li] || u.cout_pad[li] != u.L[li].cout) return false;
+    if (h->no_fused_pool || !u.row_kc[li] || u.cout_pad[li] != u.L[li].cout) return false;
     return v2e_strip_pool_supported(u.c1p[li], u.c2p[li], u.cout_pad[li], u.L[li].k, u.L[li].k, H, W) != 0;
 }
 
@@ -607,7 +604,7 @@ static int unet_forward(V2eSlomo *h, const UNet &u, const __half *in, float *out
         const int hi = H >> lvl, wi = W >> lvl, ho = hi * 2, wo = wi * 2;
         const __half *skip = k < 4 ? h->s[3 - k] : h->s1;
         const int li = 12 + 2 * k;
-        if (u.w_fold[li] && !h->no_fused_up && !h->force_tap_kernel) {
+        if (u.w_fold[li]) {
             // interpolate + conv1 in one kernel: the up-sampled tensor is never written
             if ((rc = conv_up2(h, u, li, x, B, ho, wo, h->ua[k], st))) return rc;
         } else {
@@ -675,8 +672,6 @@ extern "C" int v2e_slomo_check_finite(V2eSlomo *h, int *nonfinite_host, void *st
 
 extern "C" int v2e_slomo_set_option(V2eSlomo *h, int option, int value) {
     if (!h) return v2e_set_error(V2E_E_INVALID, "null handle%s", "");
-    if (option == 0) { h->force_tap_kernel = value; return V2E_OK; }
-    if (option == 1) { h->no_fused_up = value; return V2E_OK; }
     if (option == 2) { h->no_fused_pool = value; return V2E_OK; }
     if (option == 3) {
         // plan as if the device had `value` SMs; never more than it has, so a persistent grid cannot oversubscribe it

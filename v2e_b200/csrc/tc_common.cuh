@@ -46,33 +46,6 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *tm, ui
         ::"r"(smem_u32(dst)), "l"((uint64_t)tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 
-// ---- clusters ------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-// every thread of every CTA of the cluster arrives (release) and waits (acquire)
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-        ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
-// the 2-D box lands at the same shared-memory offset in every CTA of `mask`, and completes bytes on the mbarrier at
-// the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_multicast(void *dst, const CUtensorMap *tm, uint64_t *bar, int c0, int c1,
-                                                      uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(dst)), "l"((uint64_t)tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
-}
-
 // 1 in exactly one lane of a converged warp
 __device__ __forceinline__ uint32_t elect_one() {
     uint32_t pred;
