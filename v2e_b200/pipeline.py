@@ -5,11 +5,15 @@ The reference hands frames from SloMo to the emulator as 8-bit PNG files in a te
 (slomo.py:440-444 -> v2e.py:832 read_image); here the uint8 frames stay in HBM. Times follow
 v2e.py:794-797: interpTimes (units of source-frame intervals) scaled to the clip's duration.
 """
+import logging
+
 import numpy as np
 import torch
 
 from .emulator import EventEmulator
 from .slomo import SuperSloMo
+
+logger = logging.getLogger(__name__)
 
 
 class V2EPipeline:
@@ -38,7 +42,8 @@ class V2EPipeline:
         Returns (rows [M_r, 4] float32 host array of THIS rank's pixel rows (global y), interp_times_s,
         n_interp_frames), and with return_labels (needs label_signal_noise=True) the labels of those rows after them.
         Union over ranks = the events of the clip; parallel.gather_event_streams / merge_by_time assemble them where
-        one stream is wanted."""
+        one stream is wanted. Every rank holds only its own frame pairs, so the upsampler writes no vid_orig /
+        vid_slomo video here (rank 0 logs a warning when video_path is set)."""
         import torch.distributed as dist
         from . import parallel
         from .slomo import clip_times
@@ -53,10 +58,13 @@ class V2EPipeline:
         n, H, W = frames_u8.shape
         if n - 1 < world:
             raise ValueError("fewer frame pairs than ranks")
+        if rank == 0 and self.slomo.writes_video():
+            logger.warning("video_path ignored: a clip sharded over ranks writes no upsampler video")
         if self.slomo.auto_upsample:
             bs = max(1, min(int(self.slomo.batch_size), n - 1))
             p0, p1 = parallel.batch_pair_range(n - 1, bs, rank, world)
-            local, _, _, ups_l = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1], return_ups=True)
+            local, _, _, ups_l = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1], return_ups=True,
+                                                              write_video=False)
             # every rank's per-batch U's (a few ints; each rank knows how many batches every rank holds)
             nb = [-(-(b - a) // bs) for a, b in (parallel.batch_pair_range(n - 1, bs, r, world) for r in range(world))]
             send = torch.zeros(max(nb), dtype=torch.int64, device=local.device)
@@ -67,7 +75,7 @@ class V2EPipeline:
             times, _ = clip_times(ups, n - 1, bs)
         else:
             p0, p1 = parallel.pair_range(n - 1, rank, world)
-            local, times_l, _ = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1])
+            local, times_l, _ = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1], write_video=False)
             U = int(self.slomo.upsampling_factor)
             times = np.arange((n - 1) * U) * (1.0 / U)                       # slomo.py:391-395 for the whole clip
             assert np.allclose(times_l + p0, times[p0 * U:p1 * U])

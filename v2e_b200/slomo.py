@@ -12,6 +12,11 @@ interpolated frames out (device tensors), no temp folders -- what the event emul
 
 The reference's CPU branch skips the 0.428 mean normalisation (slomo.py:154-156); like the
 reference on a CUDA machine, this class always applies it.
+
+With `video_path` set, both paths write the reference's two videos (slomo.py:288-303, 468-491): `vid_orig`, the
+source frames, and `vid_slomo`, the interpolated frames in output order, each converted GRAY2BGR on the host and
+written through v2ecore.v2e_utils.video_writer (its codec) when that imports; otherwise a warning and no files.
+`preview` windows are not opened.
 """
 import atexit
 import ctypes
@@ -62,6 +67,17 @@ def clip_times(ups, n_pairs, batch_size):
         raise ValueError("%d U's for %d batches" % (len(ups), len(starts)))
     times = [batch_times(a, min(bs, n_pairs - a), int(U)) for a, U in zip(starts, ups)]
     return np.concatenate(times), sum(ups) / len(ups)
+
+
+def _write_gray(writer, frames):
+    """Writes host [H, W] uint8 frames to a video writer as cv2.cvtColor(frame, GRAY2BGR) (slomo.py:480-490): the
+    three channels are made on the host, so the device-to-host copy moves one. Returns how many were written."""
+    import cv2
+    n = 0
+    for f in frames:
+        writer.write(cv2.cvtColor(f, cv2.COLOR_GRAY2BGR))
+        n += 1
+    return n
 
 
 def _weights_struct(state_dict, in_ch, out_ch, keep):
@@ -228,19 +244,57 @@ class SuperSloMo(object):
                              .format(upsampling_factor))
         self.upsampling_factor = upsampling_factor
         self.auto_upsample = auto_upsample
-        if video_path is not None or preview:
-            raise NotImplementedError("AVI writers / preview window are host-side sinks (out of scope)")
+        if preview:
+            logger.warning("preview windows are out of scope here: ignored")
         self.video_path, self.vid_orig, self.vid_slomo = video_path, vid_orig, vid_slomo
         self.preview, self.avi_frame_rate = preview, avi_frame_rate
+        self.ori_writer = self.slomo_writer = None      # opened on the first batch (slomo.py:288-303)
+        self._writers_opened = False
+        self.numOrigVideoFramesWritten = self.numSlomoVideoFramesWritten = 0
         self._state_dicts = state_dicts
         self._engine = None
         self.model_loaded = False
         atexit.register(self.cleanup)
 
     def cleanup(self):
+        """slomo.py:127-138: logs the video frame counts and releases the writers; frees the device engine."""
+        if self.ori_writer is not None:
+            logger.info('closing original video AVI {} after writing {} frames'.format(
+                self.vid_orig, self.numOrigVideoFramesWritten))
+            self.ori_writer.release()
+            self.ori_writer = None
+        if self.slomo_writer is not None:
+            logger.info('closing slomo video AVI {} after writing {} frames'.format(
+                self.vid_slomo, self.numSlomoVideoFramesWritten))
+            self.slomo_writer.release()
+            self.slomo_writer = None
         if self._engine is not None:
             self._engine.close()
             self._engine = None
+
+    # -- vid_orig / vid_slomo ------------------------------------------------------------------
+    def writes_video(self):
+        """True when video_path and at least one of vid_orig / vid_slomo are set."""
+        return self.video_path is not None and (self.vid_orig is not None or self.vid_slomo is not None)
+
+    def _open_writers(self, H, W):
+        """slomo.py:288-303: the reference's video_writer for each of vid_orig / vid_slomo that is set, at the output
+        frame size. Once per object: later calls append to the same writers, and after cleanup() nothing reopens (and
+        so truncates) a finished file."""
+        if self._writers_opened or not self.writes_video():
+            return
+        self._writers_opened = True
+        try:
+            from v2ecore.v2e_utils import video_writer
+        except ImportError as e:
+            logger.warning("video_path ignored: v2ecore.v2e_utils is not importable (%s)", e)
+            return
+        if self.vid_orig is not None:
+            self.ori_writer = video_writer(os.path.join(self.video_path, self.vid_orig), H, W,
+                                           frame_rate=self.avi_frame_rate)
+        if self.vid_slomo is not None:
+            self.slomo_writer = video_writer(os.path.join(self.video_path, self.vid_slomo), H, W,
+                                             frame_rate=self.avi_frame_rate)
 
     # -- model ---------------------------------------------------------------------------------
     def _load_state(self):
@@ -294,12 +348,16 @@ class SuperSloMo(object):
             yield blk, batch_times(in_ctr, b, U), U                     # slomo.py:391-395
             in_ctr += b
 
-    def interpolate_frames(self, frames, out=None, return_ups=False):
+    def interpolate_frames(self, frames, out=None, return_ups=False, write_video=True):
         """frames: [N, H, W] uint8 (ndarray or tensor, host or device), N >= 2.
         Returns (out_u8 [M, H, W] device tensor, interpTimes [M] float64, avgUpsampling), and with return_ups the
         list of per-batch U's after them. Frame order and times follow slomo.py:391-400, 440: output index =
         counter + U*b + k holds the frame synthesised at t=(k+0.5)/U between source frames b and b+1, labelled with
-        time b + k/U."""
+        time b + k/U.
+
+        With video_path set (and write_video), vid_slomo gets the returned frames in order, one device-to-host copy
+        per batch, and vid_orig the N source frames; the writes are synchronous. write_video=False writes neither:
+        a rank of a sharded clip holds only part of it."""
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(np.ascontiguousarray(frames))
         if frames.dtype != torch.uint8 or frames.dim() != 3:
@@ -316,8 +374,14 @@ class SuperSloMo(object):
             ups.append(U)
             if fixed is None:
                 chunks.append(blk)
+            if write_video:
+                self._open_writers(H, W)
+                if self.slomo_writer is not None:
+                    self.numSlomoVideoFramesWritten += _write_gray(self.slomo_writer, blk.cpu().numpy())
         if fixed is None:
             out = torch.cat(chunks, 0)
+        if write_video and self.ori_writer is not None:
+            self.numOrigVideoFramesWritten += _write_gray(self.ori_writer, frames.cpu().numpy())
         self._engine.check_finite()
         if return_ups:
             return out, np.concatenate(times), sum(ups) / len(ups), ups
@@ -326,7 +390,12 @@ class SuperSloMo(object):
     # -- reference file API ----------------------------------------------------------------------
     def interpolate(self, source_frame_path, output_folder, frame_size):
         """slomo.py:231: .npy frames in, <idx>.png frames out; returns (interpTimes, avgUpsampling). Streams batch by
-        batch like the reference: only one batch of source frames and its interpolated frames are resident."""
+        batch like the reference: only one batch of source frames and its interpolated frames are resident.
+
+        With video_path set, vid_orig gets every source .npy frame in sorted order after the last batch
+        (slomo.py:471-482) and vid_slomo the frames this call writes as PNG, in output-index order, from the host copy
+        each batch makes for the PNGs. The reference instead re-reads every PNG in output_folder (slomo.py:484-490);
+        the two agree unless output_folder held PNGs before the call (v2e.py passes a fresh temporary directory)."""
         from PIL import Image
         if not output_folder:
             raise ValueError('output_folder is None; it must be supplied to store the interpolated frames')
@@ -352,12 +421,17 @@ class SuperSloMo(object):
         os.makedirs(output_folder, exist_ok=True)
         times, ups, out_ctr = [], [], 0
         for blk, tt, U in self._batches(get_frames, len(files), H, W):
+            self._open_writers(H, W)
             host = blk.cpu().numpy()
             for i in range(host.shape[0]):
                 Image.fromarray(host[i]).save(os.path.join(output_folder, str(out_ctr + i) + ".png"))
+            if self.slomo_writer is not None:
+                self.numSlomoVideoFramesWritten += _write_gray(self.slomo_writer, host)
             out_ctr += host.shape[0]
             times.append(tt)
             ups.append(U)
+        if self.ori_writer is not None:
+            self.numOrigVideoFramesWritten += _write_gray(self.ori_writer, (np.load(f) for f in files))
         self._engine.check_finite()
         interp_times, avg = np.concatenate(times), sum(ups) / len(ups)
         logger.info('Wrote {} frames and returning {} frame times.\nAverage upsampling factor={:5.1f}'.format(
