@@ -37,7 +37,7 @@ typedef enum V2eStatus {
 typedef enum V2eFrameDtype { V2E_U8 = 0, V2E_F32 = 1, V2E_F64 = 2 } V2eFrameDtype;
 
 const char *v2e_last_error(void);
-int v2e_version(void);
+int v2e_version(void);    /* the ABI version, 205 (205: v2e_merge_bands) */
 /* ABI guard for bindings that mirror the structs (ctypes): version and the sizes of V2eEmuCfg / V2eFrameInfo /
  * V2eUNetWeights as this library was compiled. A binding whose own sizes differ must refuse to load. */
 int v2e_abi_info(int *version, int *emu_cfg_size, int *frame_info_size, int *unet_weights_size);
@@ -549,6 +549,18 @@ int v2e_events_to_text(const float *events_dev, uint64_t n, const uint8_t *label
  * noise; n_rows = offsets_dev[n_frames]. */
 int v2e_signnoise_labels(const int64_t *offsets_dev, const uint32_t *n_noise_dev, int n_frames, uint64_t n_rows,
                          uint8_t *labels_dev, void *stream);
+/* Merge of the row bands of ONE pixel-sharded clip into the stream one GPU produces with the same row_order
+ * (v2e_b200.parallel.merge_by_key): per frame every band's signal rows by (t, key, y, x, p < 0), then every band's shot
+ * rows by (key, y, x, p < 0), equal tuples in band order. rows_dev [n][4] float32 / keys_dev [n] uint64: the bands'
+ * rows and sort keys one band after another. band_offsets_dev [n_bands][n_frames + 1] int64: absolute row offsets of
+ * every band's frames (band q holds rows [band_offsets[q][0], band_offsets[q][n_frames]), band q + 1 starting where
+ * band q ends, band 0 at row 0, the last band ending at n). n_shot_dev [n_bands][n_frames] int64: the shot rows that
+ * end each band frame. Every band frame's signal rows must be sorted by that tuple and its shot rows likewise (what a
+ * band generated with row_order returns). out_rows_dev [n][4] (not aliasing rows_dev), out_offsets_dev
+ * [n_frames + 1] int64: the merged frames' offsets. Enqueue only. */
+int v2e_merge_bands(const float *rows_dev, const uint64_t *keys_dev, uint64_t n, int n_bands, int n_frames,
+                    const int64_t *band_offsets_dev, const int64_t *n_shot_dev, float *out_rows_dev,
+                    int64_t *out_offsets_dev, void *stream);
 
 /* ------------------------------------------------------------------------- */
 /* DVS frame rendering (SURVEY.md 8f rank 4): the histogram of EventRenderer.render_events_to_frames

@@ -52,7 +52,7 @@ class V2eProbeSample(ctypes.Structure):
 
 V2E_OK, V2E_E_INVALID, V2E_E_CUDA, V2E_E_CAPACITY, V2E_E_ITER_CAP, V2E_E_STATE, V2E_E_UNSUPPORTED, V2E_E_FALLBACK = \
     0, -1, -2, -3, -4, -5, -6, -7
-ABI_VERSION = 204
+ABI_VERSION = 205
 U8, F32, F64 = 0, 1, 2
 
 _vp, _i, _d, _u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint64
@@ -142,6 +142,7 @@ _SIGS = {
     "v2e_events_to_text_layout": (_i, [_vp, _u64, _vp, _vp, _vp]),
     "v2e_events_to_text": (_i, [_vp, _u64, _vp, _vp, _vp, _vp]),
     "v2e_signnoise_labels": (_i, [_vp, _vp, _i, _u64, _vp, _vp]),
+    "v2e_merge_bands": (_i, [_vp, _vp, _u64, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "v2e_emu_profile": (_i, [_vp, _i]),
     "v2e_emu_profile_read4": (_i, [_vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(_i), _vp]),
     "v2e_emu_state_is_f64": (_i, [_vp]),

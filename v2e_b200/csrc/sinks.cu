@@ -9,6 +9,8 @@
 //   v2ecore/output/ae_text_output.py:68-101  DVS text (RPG events.txt) lines 't x y p[ label]\n'
 //   v2ecore/emulator.py:889-923              signal / shot-noise labels of the rows (1 = signal, 0 = noise)
 // File headers, h5py and the '#'-first-byte check of aedat2_output.py:166-172 stay with the caller.
+// A sharded clip's row bands are merged back into the one-GPU row order here too (v2e_merge_bands), so that the file
+// is written from device rows.
 // The HDF5 and AEDAT-2.0 conversions are pure streaming (16 B read per event): HBM bound, one thread per event.
 // The text body takes three launches (DESIGN.md 4.3): line lengths summed per block, one scan of the block sums,
 // then each block formats its lines into shared memory and stores its bytes contiguously at the block's offset.
@@ -211,6 +213,77 @@ signnoise_labels_kernel(const int64_t *__restrict__ offsets, const uint32_t *__r
     labels[i] = i < (uint64_t)offsets[lo + 1] - n_noise[lo] ? 1 : 0;
 }
 
+// ---- merge of a sharded clip's row bands (v2e_b200.parallel.merge_by_key) -------------------------------------------
+// Per frame the merged stream holds every band's signal rows by (t, key, y, x, p < 0), then every band's shot rows by
+// (key, y, x, p < 0); equal tuples keep band order. Each band's frame segment is already sorted that way (a band orders
+// its signal rows strictly by (t, key) and its shot rows by key), so a row's place is a co-rank: its index in its own
+// segment plus, for every other band, how many rows of that band's segment of the same frame and class precede it --
+// one binary search per other band. One thread per row; the rows are scattered to their places (DESIGN.md 4.3).
+// bo: [n_bands][n_frames + 1] absolute row offsets of the bands' frames; shot: [n_bands][n_frames].
+struct MergeRow {
+    float4 e;
+    uint64_t key;
+};
+
+// a before b in the merged order of one frame's signal (or, ignoring t, shot) rows
+__device__ __forceinline__ bool merge_less(const MergeRow &a, const MergeRow &b, bool shot) {
+    if (!shot && a.e.x != b.e.x) return a.e.x < b.e.x;
+    if (a.key != b.key) return a.key < b.key;
+    if (a.e.z != b.e.z) return a.e.z < b.e.z;
+    if (a.e.y != b.e.y) return a.e.y < b.e.y;
+    return (a.e.w < 0.0f) < (b.e.w < 0.0f);
+}
+
+__global__ void __launch_bounds__(256) merge_offsets_kernel(const int64_t *__restrict__ bo, int n_bands, int n_frames,
+                                                            int64_t *__restrict__ out_offsets) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f > n_frames) return;
+    int64_t s = 0;
+    for (int q = 0; q < n_bands; ++q) s += bo[(int64_t)q * (n_frames + 1) + f] - bo[(int64_t)q * (n_frames + 1)];
+    out_offsets[f] = s;
+}
+
+__global__ void __launch_bounds__(256)
+merge_bands_kernel(const float4 *__restrict__ rows, const uint64_t *__restrict__ keys, uint64_t n, int n_bands,
+                   int n_frames, const int64_t *__restrict__ bo, const int64_t *__restrict__ shot,
+                   float4 *__restrict__ out) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t stride = n_frames + 1;
+    int r = 0;                                   // the band holding row i (empty bands hold none)
+    while ((uint64_t)bo[r * stride + n_frames] <= i) ++r;
+    const int64_t *o = bo + r * stride;
+    int lo = 0, hi = n_frames - 1;               // the last frame f with o[f] <= i
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if ((uint64_t)o[mid] <= i) lo = mid;
+        else hi = mid - 1;
+    }
+    const int f = lo;
+    const int64_t s_r = o[f + 1] - shot[r * n_frames + f];
+    const bool is_shot = (int64_t)i >= s_r;
+    const MergeRow me{rows[i], keys[i]};
+    int64_t pos = (int64_t)i - (is_shot ? s_r : o[f]);
+    for (int q = 0; q < n_bands; ++q) {
+        const int64_t *oq = bo + q * stride;
+        const int64_t sq = oq[f + 1] - shot[q * n_frames + f];
+        pos += oq[f] - oq[0];                                    // the merged frame's first row
+        if (is_shot) pos += sq - oq[f];                          // after every band's signal rows of the frame
+        if (q == r) continue;
+        // rows of band q's segment before me: strictly smaller ones, and equal ones of an earlier band
+        int64_t a = is_shot ? sq : oq[f], b = is_shot ? oq[f + 1] : sq;
+        while (a < b) {
+            const int64_t mid = a + ((b - a) >> 1);
+            const MergeRow other{rows[mid], keys[mid]};
+            const bool before = q < r ? !merge_less(me, other, is_shot) : merge_less(other, me, is_shot);
+            if (before) a = mid + 1;
+            else b = mid;
+        }
+        pos += a - (is_shot ? sq : oq[f]);
+    }
+    out[pos] = me.e;
+}
+
 }  // namespace
 
 extern "C" int v2e_events_to_h5_rows(const float *events_dev, uint64_t n, uint32_t *rows_dev, void *stream) {
@@ -287,5 +360,27 @@ extern "C" int v2e_signnoise_labels(const int64_t *offsets_dev, const uint32_t *
                                                                                 n_rows, labels_dev);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "signnoise_labels_kernel: %s", cudaGetErrorString(e));
+    return V2E_OK;
+}
+
+extern "C" int v2e_merge_bands(const float *rows_dev, const uint64_t *keys_dev, uint64_t n, int n_bands, int n_frames,
+                               const int64_t *band_offsets_dev, const int64_t *n_shot_dev, float *out_rows_dev,
+                               int64_t *out_offsets_dev, void *stream) {
+    if (n_bands < 1 || n_frames < 0 || !band_offsets_dev || !out_offsets_dev || (n_frames && !n_shot_dev))
+        return v2e_set_error(V2E_E_INVALID, "bad band / frame counts or null argument%s", "");
+    if (n && (!rows_dev || !keys_dev || !out_rows_dev || n_frames < 1))
+        return v2e_set_error(V2E_E_INVALID, "null argument or no frames%s", "");
+    if (((uintptr_t)rows_dev | (uintptr_t)out_rows_dev) & 15) return v2e_set_error(V2E_E_INVALID, "rows must be 16-byte aligned%s", "");
+    if (((uintptr_t)keys_dev | (uintptr_t)band_offsets_dev | (uintptr_t)n_shot_dev | (uintptr_t)out_offsets_dev) & 7)
+        return v2e_set_error(V2E_E_INVALID, "misaligned keys or offsets%s", "");
+    const uint64_t blocks = (n + 255) / 256;
+    if (blocks > 0x7fffffffull) return v2e_set_error(V2E_E_INVALID, "too many events for one call%s", "");
+    cudaStream_t st = (cudaStream_t)stream;
+    merge_offsets_kernel<<<(n_frames + 256) / 256, 256, 0, st>>>(band_offsets_dev, n_bands, n_frames, out_offsets_dev);
+    if (n)
+        merge_bands_kernel<<<(unsigned)blocks, 256, 0, st>>>((const float4 *)rows_dev, keys_dev, n, n_bands, n_frames,
+                                                             band_offsets_dev, n_shot_dev, (float4 *)out_rows_dev);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return v2e_set_error(V2E_E_CUDA, "merge_bands_kernel: %s", cudaGetErrorString(e));
     return V2E_OK;
 }

@@ -29,10 +29,13 @@ clip is a subsequence of the one-GPU stream (v2e_b200.parallel.merge_by_key puts
 Sink keywords (dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text; emulator.py:325-357): the files are opened by the
 reference's own writer classes (v2ecore.output.*, h5py) when those import, and fed the way the reference feeds
 them (emulator.py:953-975); when they do not import the keyword is ignored with a warning. The DVS text body is
-formatted on the device (v2e_b200.sinks.events_to_text) and written to the writer's file. label_signal_noise
-labels every returned row signal (1) or shot noise (0) -- `last_signnoise_label`, generate_events_batch(...,
-return_labels=True) -- and passes the labels to the text and AEDAT-2.0 sinks. A pixel-sharded emulator labels its own
-rows (generate_events_band(_batch)(..., return_labels=True)) and writes no sink: a file needs the merged stream.
+formatted on the device (v2e_b200.sinks.events_to_text) and written to the writer's file. generate_events feeds the
+sinks frame by frame; generate_events_batch once per call through write_events, which builds the text, AEDAT-2.0 and
+HDF5 bytes on the device and copies only those. label_signal_noise labels every returned row signal (1) or shot noise
+(0) -- `last_signnoise_label`, generate_events_batch(..., return_labels=True) -- and passes the labels to the text and
+AEDAT-2.0 sinks. A pixel-sharded emulator labels its own rows (generate_events_band(_batch)(..., return_labels=True))
+and writes no sink itself: a file needs the merged stream, which V2EPipeline.run_clip_sharded(..., write_sinks=True)
+builds on the group's first rank and writes through that rank's write_events.
 
 show_dvs_model_state=[names] (or ['all']) captures, like the reference (emulator.py:41-50, 580-617, 756-767), every
 frame but the first: each shown state after the low-pass, noise, SCIDVS, surround and leak updates and before the
@@ -178,6 +181,30 @@ class _Sinks:
                 except Exception:
                     pass
         self.h5 = self.h5_dataset = self.aedat2 = self.aedat4 = self.text = None
+
+
+def _append_aedat2(w, ev, labels):
+    """AEDat2Output.appendEvents (aedat2_output.py:133-188) for device rows `ev` (labels: uint8 CUDA tensor or None):
+    the words come from the device and are the only bytes copied; while nothing has been written, leading 8-byte
+    records whose first byte is '#' are dropped (they would read as a header line) but still counted."""
+    from . import sinks
+    if w.file is None:
+        return
+    n = ev.shape[0]
+    words, n_on = sinks.events_to_aedat2(ev, w.sizex, w.sizey, labels=labels)
+    body = words.cpu().numpy().view(np.uint8)
+    if w.numEventsWritten == 0:
+        hashes = body[0::8] == 0x23
+        k = n if hashes.all() else int(np.argmin(hashes))
+        for _ in range(k):
+            logger.warning('first event would write a # comment char, dropping it')
+        body = body[8 * k:]
+    w.file.write(body.tobytes())
+    w.numEventsWritten += n
+    on = int(n_on.item())
+    w.numOnEvents += on
+    w.numOffEvents += n - on
+    w.file.flush()
 
 
 def _finalize(lib, box, sinks, spx, ms_writers=None):
@@ -1357,7 +1384,8 @@ class EventEmulator(object):
         call); with copy=False the host rows are a view of the pinned staging buffer (same lifetime). The first frame of a fresh emulator only initialises state (zero rows), as in the
         reference. Needs rng_mode="device" when leak or shot noise is on.
         return_labels=True (needs label_signal_noise=True) returns (rows, offsets, labels): labels [N], 1 for a signal
-        row and 0 for a shot-noise row, as a uint8 CUDA tensor with return_device, else a bool ndarray."""
+        row and 0 for a shot-noise row, as a uint8 CUDA tensor with return_device, else a bool ndarray.
+        The call's rows (and, with label_signal_noise, their labels) go to the open sinks through write_events."""
         if return_labels and not self.label_signal_noise:
             raise ValueError("return_labels=True needs label_signal_noise=True")
         if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
@@ -1392,11 +1420,16 @@ class EventEmulator(object):
             f = e
         offs = np.asarray(offs, np.int64)
         labels = None
-        if return_labels:
+        if return_labels or (self._sinks is not None and self.label_signal_noise):
             from .sinks import signnoise_labels
             labels = signnoise_labels(offs, n_shot, self.device)
-            if not return_device:
-                labels = labels.cpu().numpy().astype(bool)
+        if self._sinks is not None:
+            # the call's rows, straight from the device buffer, to the open sinks
+            self.write_events(self._ev_dev[:row] if row else torch.zeros((0, 4), dtype=torch.float32), labels)
+        if not return_labels:
+            labels = None
+        elif not return_device:
+            labels = labels.cpu().numpy().astype(bool)
         if return_device:
             if self._ev_dev is None:
                 rows = torch.zeros((0, 4), dtype=torch.float32, device=self.device)
@@ -1405,6 +1438,48 @@ class EventEmulator(object):
         else:
             rows = self._rows_to_host(row, copy=copy)
         return (rows, offs, labels) if return_labels else (rows, offs)
+
+    def write_events(self, rows, labels=None):
+        """Appends event rows to this emulator's open sinks (dvs_text, dvs_aedat2, dvs_h5, dvs_aedat4) and returns their
+        count N: what generate_events_batch does with the rows of every call, for rows that come from elsewhere (e.g.
+        the merged bands of a sharded clip). rows: [N, 4] float32 [t, x, y, +-1], a CUDA tensor or a host ndarray;
+        labels: [N] (1 = signal, 0 = shot noise) or None, used only with label_signal_noise. The files get the bytes the
+        reference's writers write for one appendEvents(rows, labels) call (emulator.py:953-975): the text and AEDAT-2.0
+        bodies and the HDF5 rows are built on the device and only they are copied to the host; AEDAT-4 gets host rows.
+        Without sinks nothing is written. Raises ValueError for rows that are not [N, 4] float32 or labels that are not
+        [N]."""
+        if isinstance(rows, torch.Tensor):
+            ok = rows.dtype == torch.float32
+        else:
+            ok = isinstance(rows, np.ndarray) and rows.dtype == np.float32
+        if not (ok and rows.ndim == 2 and rows.shape[1] == 4):
+            raise ValueError("rows must be a float32 [N, 4] CUDA tensor or ndarray")
+        n = int(rows.shape[0])
+        if labels is not None and (np.ndim(labels) != 1 or len(labels) != n):
+            raise ValueError("labels must be [N] for N rows")
+        sk = self._sinks
+        if sk is None or n == 0:
+            return n
+        from . import sinks
+        if isinstance(rows, torch.Tensor):
+            ev = rows.to(self.device).contiguous()
+        else:
+            ev = torch.from_numpy(np.ascontiguousarray(rows)).to(self.device)
+        lab = sinks._labels(labels, ev) if self.label_signal_noise and labels is not None else None
+        with torch.cuda.device(self.device):
+            if sk.h5 is not None:
+                tmp = sinks.events_to_h5_rows(ev).cpu().numpy().view(np.uint32)
+                sk.h5_dataset.resize(sk.h5_dataset.shape[0] + n, axis=0)
+                sk.h5_dataset[-n:] = tmp
+            if sk.aedat2 is not None:
+                _append_aedat2(sk.aedat2, ev, lab)
+            if sk.aedat4 is not None:
+                sk.aedat4.appendEvents(ev.cpu().numpy(), signnoise_label=None)
+            if sk.text is not None:
+                if sk.text.file is None:
+                    raise Exception('output file closed already')
+                sk.text.numEventsWritten += sinks.write_text(sk.text.file, ev, lab)
+        return n
 
     # state tensors by the reference's attribute names (emulator.py:756-764 reads them via getattr)
     def _state(self, name):

@@ -11,6 +11,8 @@ one all-reduce(MAX) of an int32 per frame, emulator.py:773-775); in between ever
 every frame: `exchange_frame_bands`, one all-to-all of uint8 row bands.
 Nothing here touches model arithmetic.
 """
+import ctypes
+
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -122,6 +124,94 @@ def gather_event_streams(rows, clip_ids=None, dst=0, group=None):
         return [b[:c] for b, c in zip(bufs, counts)]
     dist.gather(pad, None, dst=dst, group=group)
     return None
+
+
+def gather_band_outputs(rows, keys, offsets, n_shot, dst=0, group=None):
+    """Gathers on group rank `dst` what every rank's generate_events_band_batch(..., return_keys=True) returned for
+    its band of ONE clip: rows [N_r, 4] float32, keys [N_r] (int64 tensor or uint64 ndarray), offsets [T + 1] and the
+    band's `last_n_shot` [T]. NCCL moves CUDA tensors; other backends (gloo) move host tensors. Returns on `dst`
+    (rows, keys, offsets, n_shot), lists in rank order -- rows and keys as int64 tensors on the input rows' device,
+    offsets and n_shot as int64 ndarrays --, elsewhere None. Raises ValueError on every rank when the ranks' frame
+    counts differ."""
+    world = dist.get_world_size(group)
+    rank = dist.get_rank(group)
+    home = rows.device if isinstance(rows, torch.Tensor) else torch.device("cpu")
+    comm = home if dist.get_backend(group) == "nccl" else torch.device("cpu")
+    rows = torch.as_tensor(rows, dtype=torch.float32).reshape(-1, 4).to(comm)
+    if not isinstance(keys, torch.Tensor):
+        keys = torch.from_numpy(np.ascontiguousarray(keys, np.uint64).view(np.int64))
+    keys = keys.to(comm, torch.int64)
+    if keys.shape[0] != rows.shape[0]:
+        raise ValueError("one key per row")
+    meta = torch.from_numpy(np.concatenate([np.asarray(offsets, np.int64), np.asarray(n_shot, np.int64)])).to(comm)
+    n = torch.tensor([rows.shape[0], meta.shape[0]], dtype=torch.int64, device=comm)
+    counts = [torch.zeros_like(n) for _ in range(world)]
+    dist.all_gather(counts, n, group=group)
+    counts = [c.tolist() for c in counts]
+    if len({m for _, m in counts}) != 1:
+        raise ValueError("the ranks' bands hold different numbers of frames")
+    mx = max(c for c, _ in counts)
+    pad_rows = torch.zeros((mx, 4), dtype=torch.float32, device=comm)
+    pad_rows[:rows.shape[0]] = rows
+    pad_keys = torch.zeros((mx,), dtype=torch.int64, device=comm)
+    pad_keys[:keys.shape[0]] = keys
+    out = []
+    for t in (pad_rows, pad_keys, meta):
+        bufs = [torch.empty_like(t) for _ in range(world)] if rank == dst else None
+        dist.gather(t, bufs, group=group, group_dst=dst)
+        out.append(bufs)
+    if rank != dst:
+        return None
+    T = (counts[0][1] - 1) // 2
+    return ([b[:c].to(home) for b, (c, _) in zip(out[0], counts)],
+            [b[:c].to(home) for b, (c, _) in zip(out[1], counts)],
+            [b[:T + 1].cpu().numpy() for b in out[2]], [b[T + 1:].cpu().numpy() for b in out[2]])
+
+
+def merge_by_key_device(streams, keys, offsets, n_shot, device=None):
+    """merge_by_key on the device (v2e_merge_bands, DESIGN.md 4.3): the same arguments, the same rows and offsets bit
+    for bit, as CUDA tensors (rows [N, 4] float32, offsets [T + 1] int64) on `device` (default: the first CUDA stream's
+    device, else the current CUDA device). Rows and keys may be CUDA or host tensors or ndarrays (keys: int64 tensors
+    holding the uint64 bits, or uint64 ndarrays); offsets and n_shot are small and checked on the host."""
+    from . import _lib
+    if not (len(streams) == len(keys) == len(offsets) == len(n_shot)) or not streams:
+        raise ValueError("one stream, key array, offset array and shot-count array per rank")
+    if device is None:
+        device = next((s.device for s in streams if isinstance(s, torch.Tensor) and s.is_cuda),
+                      torch.device("cuda", torch.cuda.current_device()))
+    device = torch.device(device)
+    as_np = lambda a: (a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)).astype(np.int64)
+    offsets, n_shot = [as_np(o) for o in offsets], [as_np(s) for s in n_shot]
+    rows, ks = [], []
+    for r, k in zip(streams, keys):
+        r = torch.as_tensor(r, dtype=torch.float32).reshape(-1, 4)
+        if not isinstance(k, torch.Tensor):
+            k = torch.from_numpy(np.ascontiguousarray(k, np.uint64).view(np.int64))
+        rows.append(r.to(device))
+        ks.append(k.to(device, torch.int64).reshape(-1))
+    T = len(offsets[0]) - 1
+    band_offsets = np.zeros((len(rows), T + 1), np.int64)
+    start = 0
+    for q, (r, k, o, s) in enumerate(zip(rows, ks, offsets, n_shot)):
+        d = np.diff(o)
+        if (o.ndim != 1 or len(o) != T + 1 or s.shape != (T,) or o[0] != 0 or o[-1] != r.shape[0]
+                or k.shape[0] != r.shape[0] or np.any(d < 0) or np.any(s < 0) or np.any(s > d)):
+            raise ValueError("streams, keys, offsets and n_shot do not fit together")
+        band_offsets[q] = o + start
+        start += r.shape[0]
+    rows_in = torch.cat(rows, 0).contiguous()
+    keys_in = torch.cat(ks, 0).contiguous()
+    out = torch.empty_like(rows_in)
+    out_offsets = torch.empty((T + 1,), dtype=torch.int64, device=device)
+    bo = torch.from_numpy(band_offsets).to(device)
+    sh = torch.from_numpy(np.ascontiguousarray(np.stack(n_shot), np.int64).reshape(len(rows), T)).to(device)
+    lib = _lib.load()
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t.numel() else None
+    with torch.cuda.device(device):
+        st = ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(lib.v2e_merge_bands(p(rows_in), p(keys_in), rows_in.shape[0], len(rows), T, p(bo), p(sh), p(out),
+                                       p(out_offsets), st))
+    return out, out_offsets
 
 
 def merge_by_time(streams):

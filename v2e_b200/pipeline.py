@@ -31,7 +31,8 @@ class V2EPipeline:
         ev, offs = self.emulator.generate_events_batch(interp, t, return_device=return_device, copy=copy)
         return ev, offs, t, interp.shape[0]
 
-    def run_clip_sharded(self, frames_u8, src_duration_s, t_offset=0.0, group=None, return_labels=False):
+    def run_clip_sharded(self, frames_u8, src_duration_s, t_offset=0.0, group=None, return_labels=False,
+                         write_sinks=False):
         """ONE clip over the ranks of `group` (BASELINE config 5 layout; SURVEY.md 8e). Every rank passes the
         same source frames; the emulator must have been built with shard=(rank, world, group).
           1. SloMo over this rank's frame pairs (parallel.pair_range) -- no halo, weights replicated. With
@@ -43,7 +44,14 @@ class V2EPipeline:
         n_interp_frames), and with return_labels (needs label_signal_noise=True) the labels of those rows after them.
         Union over ranks = the events of the clip; parallel.gather_event_streams / merge_by_time assemble them where
         one stream is wanted. Every rank holds only its own frame pairs, so the upsampler writes no vid_orig /
-        vid_slomo video here (rank 0 logs a warning when video_path is set)."""
+        vid_slomo video here (rank 0 logs a warning when video_path is set).
+        write_sinks=True (needs row_order) writes the clip's event files: every rank's rows, sort keys, frame offsets and
+        shot counts are gathered on the group's first rank (parallel.gather_band_outputs), which merges the bands on the
+        device into the one-GPU stream (parallel.merge_by_key_device) and passes it, with its labels, to its own
+        emulator's write_events -- the files a single-GPU V2EPipeline.run writes. Only that rank's emulator may be built
+        with sink keywords (dvs_text, dvs_aedat2, ...); the others are built without, since they would open, and
+        truncate, the same paths. The ranks check this together before any data moves and all raise ValueError when
+        another rank holds sinks. The return values are those of write_sinks=False."""
         import torch.distributed as dist
         from . import parallel
         from .slomo import clip_times
@@ -53,6 +61,22 @@ class V2EPipeline:
             raise RuntimeError("run_clip_sharded needs EventEmulator(shard=(rank, world, group))")
         if return_labels and not em.label_signal_noise:
             raise ValueError("return_labels=True needs label_signal_noise=True")
+        if write_sinks:
+            if em.row_order is None:
+                raise ValueError("write_sinks=True needs EventEmulator(row_order='canonical' or 'shuffled'): the bands "
+                                 "are merged by their sort keys")
+            # every rank learns who holds sinks, so that all of them raise (none waits in a collective)
+            nccl = dist.get_backend(group) == "nccl"
+            flag = torch.tensor([0 if em._sinks is None else 1], dtype=torch.int64,
+                                device=em.device if nccl else "cpu")
+            flags = [torch.zeros_like(flag) for _ in range(world)]
+            dist.all_gather(flags, flag, group=group)
+            flags = [int(f.item()) for f in flags]
+            bad = [r for r in range(1, world) if flags[r]]
+            if bad:
+                raise ValueError("write_sinks=True: only the group's first rank may hold sinks, ranks %s do; build "
+                                 "their emulators without dvs_* keywords" % bad)
+            write_sinks = bool(flags[0])
         if isinstance(frames_u8, np.ndarray):
             frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
         n, H, W = frames_u8.shape
@@ -87,8 +111,15 @@ class V2EPipeline:
             # chunks of frames through the multi-frame kernels: one all-reduce(MAX) of the frame maxima per chunk
             # (frame by frame -- one all-reduce each -- for a chunk the refractory filter touches, for the
             # centre-surround model, whose Euler iteration exchanges halo rows, and for SCIDVS / photoreceptor noise)
-            res = em.generate_events_band_batch(bands, t, H, **extra)
-            return (res[0], t, bands.shape[0]) + tuple(res[2:])
+            if not write_sinks:
+                res = em.generate_events_band_batch(bands, t, H, **extra)
+                return (res[0], t, bands.shape[0]) + tuple(res[2:])
+            rows, offs, *labels, keys = em.generate_events_band_batch(bands, t, H, return_device=True,
+                                                                      return_keys=True, **extra)
+            self._write_merged(rows, keys, offs, group)
+            labels = [labels[0].cpu().numpy().astype(bool)] if labels else []
+            return (rows.cpu().numpy(), t, bands.shape[0]) + tuple(labels)
+        assert not write_sinks, "row_order needs rng_mode='device', which takes the batched path"
         out, labs = [], []
         for k in range(bands.shape[0]):
             ev = em.generate_events_band(bands[k], t[k], H)
@@ -99,3 +130,16 @@ class V2EPipeline:
         if return_labels:
             return rows, t, bands.shape[0], (np.concatenate(labs) if labs else np.zeros((0,), bool))
         return rows, t, bands.shape[0]
+
+    def _write_merged(self, rows, keys, offs, group):
+        """write_sinks: the bands of every rank to the group's first rank, merged there and written to its sinks."""
+        from . import parallel
+        from .sinks import signnoise_labels
+        em = self.emulator
+        g = parallel.gather_band_outputs(rows, keys, offs, em.last_n_shot, dst=0, group=group)
+        if g is None:
+            return
+        streams, ks, os_, ss = g
+        merged, moffs = parallel.merge_by_key_device(streams, ks, os_, ss, device=em.device)
+        labels = signnoise_labels(moffs, np.sum(ss, axis=0), em.device) if em.label_signal_noise else None
+        em.write_events(merged, labels)
