@@ -183,17 +183,20 @@ class _Sinks:
         self.h5 = self.h5_dataset = self.aedat2 = self.aedat4 = self.text = None
 
 
-def _append_aedat2(w, ev, labels):
+def _append_aedat2(w, ev, labels, dropping=None):
     """AEDat2Output.appendEvents (aedat2_output.py:133-188) for device rows `ev` (labels: uint8 CUDA tensor or None):
     the words come from the device and are the only bytes copied; while nothing has been written, leading 8-byte
-    records whose first byte is '#' are dropped (they would read as a header line) but still counted."""
+    records whose first byte is '#' are dropped (they would read as a header line) but still counted. dropping=True
+    applies that rule to a call that continues an earlier one which dropped all its records. Returns True when this
+    call applied the rule and dropped every record."""
     from . import sinks
     if w.file is None:
-        return
+        return False
     n = ev.shape[0]
     words, n_on = sinks.events_to_aedat2(ev, w.sizex, w.sizey, labels=labels)
     body = words.cpu().numpy().view(np.uint8)
-    if w.numEventsWritten == 0:
+    k = 0
+    if w.numEventsWritten == 0 or dropping:
         hashes = body[0::8] == 0x23
         k = n if hashes.all() else int(np.argmin(hashes))
         for _ in range(k):
@@ -205,6 +208,7 @@ def _append_aedat2(w, ev, labels):
     w.numOnEvents += on
     w.numOffEvents += n - on
     w.file.flush()
+    return k == n
 
 
 def _finalize(lib, box, sinks, spx, ms_writers=None):
@@ -462,6 +466,10 @@ class EventEmulator(object):
         # sink keywords: delegated to the reference's writers when they import (emulator.py:325-357)
         self.dvs_h5 = self.dvs_aedat2 = self.dvs_aedat4 = self.dvs_text = None
         self._sinks = None
+        # set by V2EPipeline.run_segments: the next write continues the last one, so AEDAT-2.0 keeps dropping leading
+        # '#' records while every record so far was dropped, as one write of both would
+        self._sinks_continue = False
+        self._aedat2_dropped_all = False
         if dvs_h5 or dvs_aedat2 or dvs_aedat4 or dvs_text:
             sk = _Sinks(output_folder, dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text, output_width, output_height,
                         label_signal_noise, self.device)
@@ -1376,6 +1384,17 @@ class EventEmulator(object):
             self.last_frame_info = info[T - 1]
             return total, offsets, n_shot
 
+    def check_batch_path(self):
+        """Raises RuntimeError where generate_events_batch cannot run this emulator: replay mode with per-frame noise,
+        or a sharded emulator."""
+        if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
+                                          self.photoreceptor_noise):
+            raise RuntimeError("generate_events_batch with per-frame noise needs rng_mode='device' "
+                               "(replay mode must interleave host draws frame by frame)")
+        if self.shard is not None:
+            raise RuntimeError("generate_events_batch runs whole frames; a sharded emulator takes "
+                               "generate_events_band_batch")
+
     def generate_events_batch(self, frames, t_frames, return_device=False, copy=True, return_labels=False):
         """Fast path (not in the reference): all frames of a clip in a few launches per frame and no
         per-frame host synchronisation. frames: [T,H,W]; t_frames: [T] seconds, non-decreasing.
@@ -1388,13 +1407,7 @@ class EventEmulator(object):
         The call's rows (and, with label_signal_noise, their labels) go to the open sinks through write_events."""
         if return_labels and not self.label_signal_noise:
             raise ValueError("return_labels=True needs label_signal_noise=True")
-        if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
-                                          self.photoreceptor_noise):
-            raise RuntimeError("generate_events_batch with per-frame noise needs rng_mode='device' "
-                               "(replay mode must interleave host draws frame by frame)")
-        if self.shard is not None:
-            raise RuntimeError("generate_events_batch runs whole frames; a sharded emulator takes "
-                               "generate_events_band_batch")
+        self.check_batch_path()
         fr, code = self._to_device_frames(frames)
         if fr.dim() != 3:
             raise ValueError("frames must be [T, height, width]")
@@ -1472,7 +1485,8 @@ class EventEmulator(object):
                 sk.h5_dataset.resize(sk.h5_dataset.shape[0] + n, axis=0)
                 sk.h5_dataset[-n:] = tmp
             if sk.aedat2 is not None:
-                _append_aedat2(sk.aedat2, ev, lab)
+                self._aedat2_dropped_all = _append_aedat2(sk.aedat2, ev, lab,
+                                                          self._sinks_continue and self._aedat2_dropped_all)
             if sk.aedat4 is not None:
                 sk.aedat4.appendEvents(ev.cpu().numpy(), signnoise_label=None)
             if sk.text is not None:

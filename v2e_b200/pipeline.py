@@ -11,9 +11,39 @@ import numpy as np
 import torch
 
 from .emulator import EventEmulator
-from .slomo import SuperSloMo
+from .slomo import SuperSloMo, clip_span
 
 logger = logging.getLogger(__name__)
+
+# Source frame pairs per segment of V2EPipeline.run_segments. Each segment adds one event read-back and one finiteness
+# check (two stream synchronisations) to the SloMo work of its pairs; at 64 pairs that is ~640 interpolated frames at
+# U = 10, enough to hide them at small frame sizes too. At 1280x720, U = 10 and 0.11 events/px/frame a segment of 64
+# pairs adds ~3 GB of device memory (its frames, and an event buffer grown to twice what overflowed it), and
+# bench_stream.py measures the same time per frame at 16, 64 and 256 pairs as one run.
+DEFAULT_SEGMENT_PAIRS = 64
+
+
+def segment_plan(n_frames, batch_size, segment_pairs=None):
+    """The segments V2EPipeline.run_segments runs a clip of n_frames source frames in, as pair ranges [(p0, p1)]:
+    segment k interpolates pairs p0 .. p1-1 from source frames p0 .. p1, so consecutive segments share one source
+    frame. segment_pairs (default DEFAULT_SEGMENT_PAIRS) is rounded up to a multiple of batch_size, which puts every
+    boundary on a SloMo batch boundary of the clip; the last segment takes the pairs that are left."""
+    n_frames = int(n_frames)
+    if n_frames < 2:
+        raise ValueError("n_frames=%d: a clip needs at least two source frames" % n_frames)
+    sp = DEFAULT_SEGMENT_PAIRS if segment_pairs is None else int(segment_pairs)
+    if sp < 1:
+        raise ValueError("segment_pairs=%d: a segment needs at least one frame pair" % sp)
+    bs = max(1, int(batch_size))
+    sp = -(-sp // bs) * bs
+    n_pairs = n_frames - 1
+    return [(p0, min(p0 + sp, n_pairs)) for p0 in range(0, n_pairs, sp)]
+
+
+def _describe(x):
+    if isinstance(x, (np.ndarray, torch.Tensor)):
+        return "%s %s %s" % (type(x).__name__, str(x.dtype).replace("torch.", ""), list(x.shape))
+    return type(x).__name__
 
 
 class V2EPipeline:
@@ -24,12 +54,92 @@ class V2EPipeline:
     def run(self, frames_u8, src_duration_s, t_offset=0.0, return_device=False, copy=False):
         """frames_u8: [N,H,W] uint8 source frames covering `src_duration_s` seconds.
         Returns (events [M,4] float32, frame offsets, interp_times_s, n_interp_frames). Host rows are a
-        view of the emulator's pinned staging buffer unless copy=True (valid until the next call)."""
-        interp, times, avg_u = self.slomo.interpolate_frames(frames_u8)
-        f = src_duration_s / (np.max(times) - np.min(times))          # v2e.py:794-797
-        t = t_offset + f * times
-        ev, offs = self.emulator.generate_events_batch(interp, t, return_device=return_device, copy=copy)
-        return ev, offs, t, interp.shape[0]
+        view of the emulator's pinned staging buffer unless copy=True (valid until the next call).
+        The clip is run_segments' single segment."""
+        if isinstance(frames_u8, np.ndarray):
+            frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
+        n = frames_u8.shape[0]
+        (res,) = self.run_segments(lambda a, b: frames_u8[a:b], n, src_duration_s, t_offset,
+                                   segment_pairs=max(n - 1, 1), return_device=return_device, copy=copy)
+        return res
+
+    def run_segments(self, get_frames, n_frames, src_duration_s, t_offset=0.0, segment_pairs=None,
+                     return_device=False, copy=False):
+        """Runs a clip of any length segment by segment: a generator that yields, per segment,
+        (events [M,4] float32, frame offsets [T+1], interp_times_s [T], n_interp_frames T) -- what run returns, for
+        that segment's interpolated frames only (offsets start at 0 in every segment). Concatenated, the segments are
+        what one run(all frames, src_duration_s, t_offset) returns on a fresh pipeline: the same frames, times,
+        rows, offsets and emulator counters, and the same vid_orig / vid_slomo videos and event files.
+
+        get_frames(a, b) returns source frames a .. b-1 as uint8 [b-a, H, W], an ndarray or a tensor, on the host or
+        the device (for an array: lambda a, b: frames[a:b]; raw BGR video goes through InputPrep inside it).
+        n_frames >= 2 is the clip's source frame count, src_duration_s its duration.
+
+        segment_pairs: source frame pairs per segment, rounded up to a multiple of slomo.batch_size so that segments
+        start on the clip's SloMo batch boundaries (segment_plan). Default DEFAULT_SEGMENT_PAIRS: ~3 GB of device
+        memory per segment at 1280x720, U = 10, and as fast per frame as one run. Consecutive segments share one
+        source frame: the last of segment k is the first of segment k+1.
+
+        Device and pinned-host memory depend on the segment length, not the clip length: one segment's source and
+        interpolated frames are held at a time, and the emulator's event buffers grow to the largest segment. The
+        rows are valid until the next iteration (return_device=True: a view of the emulator's device buffer; host
+        rows with copy=False: a view of its pinned staging buffer); copy=True returns host rows the caller owns.
+
+        Times: the scale f = src_duration_s / (max - min of the clip's interpTimes) (v2e.py:794-797) depends on the U
+        of the clip's last batch and enters every frame interval of the pixel model, so it is known before the first
+        segment. With a fixed U it follows from the shapes; with auto_upsample and more than one segment, the flow
+        network first runs on the clip's last batch (fetched through get_frames) to pick its U. A single segment
+        takes f from its own times, as run does.
+
+        Raises ValueError, naming the segment, when get_frames returns anything but uint8 [b-a, H, W] with the first
+        segment's H, W; RuntimeError, before any work, where generate_events_batch refuses the emulator (replay mode
+        with per-frame noise, a sharded emulator: run_clip_sharded takes a clip over ranks)."""
+        sl, em = self.slomo, self.emulator
+        em.check_batch_path()
+        n = int(n_frames)
+        plan = segment_plan(n, sl.batch_size, segment_pairs)
+        m = len(plan)
+        size = []
+
+        def fetch(a, b, k):
+            fr = get_frames(a, b)
+            if isinstance(fr, np.ndarray):
+                fr = torch.from_numpy(np.ascontiguousarray(fr))
+            ok = (isinstance(fr, torch.Tensor) and fr.dtype == torch.uint8 and fr.dim() == 3 and fr.shape[0] == b - a
+                  and (not size or tuple(fr.shape[1:]) == size[0]))
+            if not ok:
+                want = "[%d, %d, %d]" % ((b - a,) + size[0]) if size else "[%d, H, W]" % (b - a)
+                raise ValueError("segment %d of %d: get_frames(%d, %d) returned %s, expected uint8 %s"
+                                 % (k, m, a, b, _describe(fr), want))
+            size[:] = [tuple(fr.shape[1:])]
+            return fr
+
+        f = u_last = None
+        if m > 1:
+            if sl.auto_upsample:
+                bs = max(1, min(int(sl.batch_size), n - 1))
+                a = (n - 2) // bs * bs
+                u_last = sl.batch_upsampling(fetch(a, n, m - 1), n)
+            else:
+                u_last = int(sl.upsampling_factor)
+            f = src_duration_s / clip_span(n - 1, sl.batch_size, u_last)
+        for k, (p0, p1) in enumerate(plan):
+            fr = fetch(p0, p1 + 1, k)
+            interp, times, _, ups = sl.interpolate_frames(fr, return_ups=True, first_pair=p0, clip_frames=n)
+            del fr
+            if f is None:
+                f = src_duration_s / (np.max(times) - np.min(times))          # v2e.py:794-797
+            elif k == m - 1 and ups[-1] != u_last:
+                raise RuntimeError("the clip's last batch got U=%d, its time-scale pre-pass U=%d" % (ups[-1], u_last))
+            t = t_offset + f * times
+            em._sinks_continue = k > 0
+            try:
+                ev, offs = em.generate_events_batch(interp, t, return_device=return_device, copy=copy)
+            finally:
+                em._sinks_continue = False
+            nf = interp.shape[0]
+            del interp
+            yield ev, offs, t, nf
 
     def run_clip_sharded(self, frames_u8, src_duration_s, t_offset=0.0, group=None, return_labels=False,
                          write_sinks=False):

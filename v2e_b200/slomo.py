@@ -69,6 +69,15 @@ def clip_times(ups, n_pairs, batch_size):
     return np.concatenate(times), sum(ups) / len(ups)
 
 
+def clip_span(n_pairs, batch_size, last_U):
+    """max(interpTimes) - min(interpTimes) of a clip of n_pairs frame pairs in batches of batch_size whose last batch is
+    up-sampled last_U times: the denominator of v2e.py:794-797, known before any other batch is interpolated. The same
+    double as for clip_times(...)[0]: the times start at 0.0 and increase, so the span is the last batch's last time."""
+    bs = max(1, min(int(batch_size), n_pairs))
+    a = (n_pairs - 1) // bs * bs
+    return batch_times(a, n_pairs - a, int(last_U))[-1] - 0.0
+
+
 def _write_gray(writer, frames):
     """Writes host [H, W] uint8 frames to a video writer as cv2.cvtColor(frame, GRAY2BGR) (slomo.py:480-490): the
     three channels are made on the host, so the device-to-host copy moves one. Returns how many were written."""
@@ -317,28 +326,34 @@ class SuperSloMo(object):
         return self._engine
 
     # -- in-memory path ------------------------------------------------------------------------
-    def _batches(self, get_frames, n, H, W, out=None):
-        """The reference's loop over batches of consecutive frame pairs (slomo.py:330-444). get_frames(a, b) returns
-        source frames a .. b-1 as a uint8 [b-a, H, W] tensor (host or device). Yields, per batch,
-        (frames [U*b, H, W] uint8 device, interpTimes of the batch, U): with `out` (fixed U) the frames are a view of
-        out[U*in_ctr : U*(in_ctr+b)], otherwise a fresh block."""
+    def _upsampling(self, eng):
+        """U of the batch set on `eng` (slomo.py:366-385): the flow network's ceil(max |flow|) with auto_upsample,
+        floored at upsampling_factor, else upsampling_factor; at least 2."""
+        if self.auto_upsample:
+            U = int(np.ceil(eng.max_flow()))                          # slomo.py:366-372
+            if self.upsampling_factor is not None and self.upsampling_factor > U:
+                U = self.upsampling_factor
+        else:
+            U = self.upsampling_factor
+        return max(U, 2)                                                # slomo.py:383-385
+
+    def _batches(self, get_frames, n, H, W, out=None, pairs=None):
+        """The reference's loop over batches of consecutive frame pairs (slomo.py:330-444) of a clip of n source frames.
+        get_frames(a, b) returns source frames a .. b-1 as a uint8 [b-a, H, W] tensor (host or device). pairs=(p0, p1)
+        runs pairs p0 .. p1-1 only (p0 on a batch boundary): batches and times are still the whole clip's. Yields, per
+        batch, (frames [U*b, H, W] uint8 device, interpTimes of the batch, U): with `out` (fixed U) the frames are a
+        view of out[U*(in_ctr-p0) : U*(in_ctr-p0+b)], otherwise a fresh block."""
         bs = max(1, min(int(self.batch_size), n - 1))
+        p0, p1 = (0, n - 1) if pairs is None else pairs
         eng = self._engine_for((W, H), bs)
-        in_ctr = 0
-        while in_ctr < n - 1:
-            b = min(bs, n - 1 - in_ctr)
+        in_ctr = p0
+        while in_ctr < p1:
+            b = min(bs, p1 - in_ctr)
             fr = get_frames(in_ctr, in_ctr + b + 1).to(self.device, non_blocking=True).contiguous()
             eng.set_pairs(fr)
-            if self.auto_upsample:
-                U = int(np.ceil(eng.max_flow()))                      # slomo.py:366-372
-                if self.upsampling_factor is not None and self.upsampling_factor > U:
-                    U = self.upsampling_factor
-            else:
-                U = self.upsampling_factor
-            if U < 2:
-                U = 2                                                   # slomo.py:383-385
+            U = self._upsampling(eng)
             if out is not None:
-                blk = out[U * in_ctr: U * (in_ctr + b)]
+                blk = out[U * (in_ctr - p0): U * (in_ctr - p0 + b)]
             else:
                 blk = torch.empty((U * b, H, W), dtype=torch.uint8, device=self.device)
             for k in range(U):
@@ -348,16 +363,32 @@ class SuperSloMo(object):
             yield blk, batch_times(in_ctr, b, U), U                     # slomo.py:391-395
             in_ctr += b
 
-    def interpolate_frames(self, frames, out=None, return_ups=False, write_video=True):
+    def batch_upsampling(self, frames, clip_frames):
+        """U that one batch gets: frames, uint8 [b+1, H, W] (tensor, host or device), are the source frames of one
+        batch of a clip of clip_frames frames. Runs the flow network alone (slomo.py:343-385) and raises
+        FloatingPointError if it overflowed."""
+        n, H, W = frames.shape
+        eng = self._engine_for((W, H), max(1, min(int(self.batch_size), clip_frames - 1)))
+        eng.set_pairs(frames.to(self.device, non_blocking=True).contiguous())
+        U = self._upsampling(eng)
+        eng.check_finite()
+        return U
+
+    def interpolate_frames(self, frames, out=None, return_ups=False, write_video=True, first_pair=0, clip_frames=None):
         """frames: [N, H, W] uint8 (ndarray or tensor, host or device), N >= 2.
         Returns (out_u8 [M, H, W] device tensor, interpTimes [M] float64, avgUpsampling), and with return_ups the
         list of per-batch U's after them. Frame order and times follow slomo.py:391-400, 440: output index =
         counter + U*b + k holds the frame synthesised at t=(k+0.5)/U between source frames b and b+1, labelled with
         time b + k/U.
 
+        first_pair / clip_frames: `frames` are source frames first_pair .. first_pair + N - 1 of a clip of clip_frames
+        frames (a segment of it; first_pair on a batch boundary of the clip). The batches, their U's and the times are
+        then those of the whole clip, restricted to the segment's pairs.
+
         With video_path set (and write_video), vid_slomo gets the returned frames in order, one device-to-host copy
-        per batch, and vid_orig the N source frames; the writes are synchronous. write_video=False writes neither:
-        a rank of a sharded clip holds only part of it."""
+        per batch, and vid_orig the N source frames (without the first when first_pair > 0: the segment before wrote
+        it); the writes are synchronous. write_video=False writes neither: a rank of a sharded clip holds only part
+        of it."""
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(np.ascontiguousarray(frames))
         if frames.dtype != torch.uint8 or frames.dim() != 3:
@@ -365,11 +396,15 @@ class SuperSloMo(object):
         n, H, W = frames.shape
         if n < 2:
             raise ValueError("need at least two frames")
+        clip_n = n if clip_frames is None else int(clip_frames)
+        if first_pair < 0 or first_pair + n > clip_n:
+            raise ValueError("frames %d .. %d are not in a clip of %d" % (first_pair, first_pair + n - 1, clip_n))
         if out is None and not self.auto_upsample:
             out = torch.empty(((n - 1) * int(self.upsampling_factor), H, W), dtype=torch.uint8, device=self.device)
         fixed = out if not self.auto_upsample else None
         chunks, times, ups = [], [], []
-        for blk, tt, U in self._batches(lambda a, b: frames[a:b], n, H, W, out=fixed):
+        for blk, tt, U in self._batches(lambda a, b: frames[a - first_pair:b - first_pair], clip_n, H, W, out=fixed,
+                                        pairs=(first_pair, first_pair + n - 1)):
             times.append(tt)
             ups.append(U)
             if fixed is None:
@@ -381,7 +416,7 @@ class SuperSloMo(object):
         if fixed is None:
             out = torch.cat(chunks, 0)
         if write_video and self.ori_writer is not None:
-            self.numOrigVideoFramesWritten += _write_gray(self.ori_writer, frames.cpu().numpy())
+            self.numOrigVideoFramesWritten += _write_gray(self.ori_writer, frames[1 if first_pair else 0:].cpu().numpy())
         self._engine.check_finite()
         if return_ups:
             return out, np.concatenate(times), sum(ups) / len(ups), ups
