@@ -316,6 +316,8 @@ class OracleEmulator:
             self.cs_steps_taken.append(cs_steps.value)
         self._scidvs_started = True
         self.last_max_n = max_n.value
+        # signal rows (ON, OFF) of every iteration of this frame, empty ones included
+        self.last_iter_counts = iters[:2 * max_n.value].reshape(-1, 2).copy()
         ev = ev[:rows]
         # replay the per-iteration shuffles (emulator.py:866-870)
         out = []

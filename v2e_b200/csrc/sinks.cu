@@ -24,8 +24,15 @@ extern int v2e_set_error(int code, const char *fmt, const char *detail);
 
 namespace {
 
-// numpy float32 -> uint32 / int32 casts truncate toward zero
+// numpy float32 -> uint32 / int32 casts truncate toward zero. Past 2^32 the uint32 value here wraps mod 2^32 (through
+// int64); numpy's own result there depends on the array's length (DESIGN.md 2).
 __device__ __forceinline__ uint32_t f2u_trunc(float v) { return (uint32_t)(int64_t)v; }
+
+// numpy's float32 -> int32 cast on x86-64: truncation toward zero inside [-2^31, 2^31), INT32_MIN outside it and for
+// NaN (cvttss2si's "integer indefinite"). A plain (int32_t) cast compiles to cvt.rzi.s32.f32, which saturates.
+__device__ __forceinline__ int32_t f2i_trunc_x86(float v) {
+    return (v >= -2147483648.0f && v < 2147483648.0f) ? (int32_t)v : INT32_MIN;
+}
 
 __global__ void __launch_bounds__(256) h5_rows_kernel(const float4 *__restrict__ ev, uint64_t n, uint4 *__restrict__ out) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -44,7 +51,7 @@ aedat2_kernel(const float4 *__restrict__ ev, const uint8_t *__restrict__ labels,
     int on = 0;
     if (i < n) {
         const float4 e = ev[i];
-        const int32_t t = (int32_t)__fmul_rn(1e6f, e.x);              // aedat2_output.py:144
+        const int32_t t = f2i_trunc_x86(__fmul_rn(1e6f, e.x));        // aedat2_output.py:144
         int32_t x = (int32_t)e.y, y = (int32_t)e.z;
         if (flip_x) x = (size_x - 1) - x;                             // :148
         if (flip_y) y = (size_y - 1) - y;                             // :150

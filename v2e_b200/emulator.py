@@ -152,11 +152,14 @@ class _Sinks:
             return
         if not self.label_signal_noise:
             signnoise_label = None
+        from . import sinks
+        ev = None
+        if self.h5 is not None or self.text is not None:
+            ev = torch.from_numpy(np.ascontiguousarray(events, dtype=np.float32)).to(self.device)
         if self.h5 is not None:
-            tmp = np.array(events, dtype=np.float32)
-            tmp[:, 0] = tmp[:, 0] * 1e6
-            tmp[tmp[:, 3] == -1, 3] = 0
-            tmp = tmp.astype(np.uint32)
+            # the device conversion write_events uses, so that both paths write the same rows (past 2^32 us the
+            # reference's numpy cast depends on the array's length, DESIGN.md 2)
+            tmp = sinks.events_to_h5_rows(ev).cpu().numpy().view(np.uint32)
             self.h5_dataset.resize(self.h5_dataset.shape[0] + tmp.shape[0], axis=0)
             self.h5_dataset[-tmp.shape[0]:] = tmp
         if self.aedat2 is not None:
@@ -168,8 +171,6 @@ class _Sinks:
             # come from the device, one copy and one write for the frame
             if self.text.file is None:
                 raise Exception('output file closed already')
-            from . import sinks
-            ev = torch.from_numpy(np.ascontiguousarray(events, dtype=np.float32)).to(self.device)
             lab = None if signnoise_label is None else torch.from_numpy(np.asarray(signnoise_label, np.uint8))
             self.text.numEventsWritten += sinks.write_text(self.text.file, ev, lab)
 
