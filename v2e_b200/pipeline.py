@@ -11,7 +11,7 @@ import numpy as np
 import torch
 
 from .emulator import EventEmulator
-from .slomo import SuperSloMo, clip_span
+from .slomo import SuperSloMo, batch_times, clip_span
 
 logger = logging.getLogger(__name__)
 
@@ -23,21 +23,60 @@ logger = logging.getLogger(__name__)
 DEFAULT_SEGMENT_PAIRS = 64
 
 
-def segment_plan(n_frames, batch_size, segment_pairs=None):
+def segment_plan(n_frames, batch_size, segment_pairs=None, world=1, auto_upsample=False):
     """The segments V2EPipeline.run_segments runs a clip of n_frames source frames in, as pair ranges [(p0, p1)]:
     segment k interpolates pairs p0 .. p1-1 from source frames p0 .. p1, so consecutive segments share one source
     frame. segment_pairs (default DEFAULT_SEGMENT_PAIRS) is rounded up to a multiple of batch_size, which puts every
-    boundary on a SloMo batch boundary of the clip; the last segment takes the pairs that are left."""
-    n_frames = int(n_frames)
+    boundary on a SloMo batch boundary of the clip; the last segment takes the pairs that are left.
+
+    world > 1: the segments of V2EPipeline.run_segments_sharded over `world` ranks, each one that run_clip_sharded
+    accepts: at least `world` pairs, or with auto_upsample (whose batches are dealt to the ranks whole) at least
+    `world` batches. segment_pairs is raised to that minimum before it is rounded, a shorter last segment is folded
+    into the one before it, and a clip shorter than one segment raises ValueError. world=1 gives the plan above."""
+    n_frames, world = int(n_frames), int(world)
     if n_frames < 2:
         raise ValueError("n_frames=%d: a clip needs at least two source frames" % n_frames)
+    if world < 1:
+        raise ValueError("world=%d: a clip needs at least one rank" % world)
     sp = DEFAULT_SEGMENT_PAIRS if segment_pairs is None else int(segment_pairs)
     if sp < 1:
         raise ValueError("segment_pairs=%d: a segment needs at least one frame pair" % sp)
     bs = max(1, int(batch_size))
-    sp = -(-sp // bs) * bs
+    unit = bs if auto_upsample else 1                    # pairs per share a rank must get at least one of
+    sp = -(-max(sp, world * unit) // bs) * bs
     n_pairs = n_frames - 1
-    return [(p0, min(p0 + sp, n_pairs)) for p0 in range(0, n_pairs, sp)]
+    plan = [(p0, min(p0 + sp, n_pairs)) for p0 in range(0, n_pairs, sp)]
+    p0, p1 = plan[-1]
+    if -(-(p1 - p0) // unit) < world:
+        if len(plan) == 1:
+            raise ValueError("fewer batches of frame pairs than ranks" if auto_upsample else
+                             "fewer frame pairs than ranks")
+        plan[-2:] = [(plan[-2][0], p1)]
+    return plan
+
+
+def sharded_times(n_pairs, batch_size, pairs, ups):
+    """interpTimes of pairs p0 .. p1-1 (p0 on a SloMo batch boundary) of a clip of n_pairs frame pairs sharded over
+    ranks: these elements of the times run_clip_sharded builds for the whole clip, bit for bit. ups: the fixed U (an
+    int: np.arange(n_pairs * U) * (1 / U), slomo.py:391-395 for the whole clip), or the list of U's of the batches in
+    [p0, p1) (auto_upsample: each batch's batch_times, as slomo.clip_times concatenates them)."""
+    p0, p1 = pairs
+    if isinstance(ups, (int, np.integer)):
+        U = int(ups)
+        return np.arange(p0 * U, p1 * U) * (1.0 / U)
+    bs = max(1, min(int(batch_size), n_pairs))
+    starts = range(p0, p1, bs)
+    if len(ups) != len(starts):
+        raise ValueError("%d U's for %d batches" % (len(ups), len(starts)))
+    return np.concatenate([batch_times(a, min(bs, n_pairs - a), int(U)) for a, U in zip(starts, ups)])
+
+
+def sharded_span(n_pairs, batch_size, last_U, auto_upsample):
+    """max - min of the times run_clip_sharded builds for a clip of n_pairs frame pairs whose last batch gets last_U
+    (the fixed U without auto_upsample): the denominator of v2e.py:794-797, the same double."""
+    if auto_upsample:
+        return clip_span(n_pairs, batch_size, last_U)
+    return (n_pairs * int(last_U) - 1) * (1.0 / int(last_U)) - 0.0
 
 
 def _describe(x):
@@ -161,61 +200,173 @@ class V2EPipeline:
         emulator's write_events -- the files a single-GPU V2EPipeline.run writes. Only that rank's emulator may be built
         with sink keywords (dvs_text, dvs_aedat2, ...); the others are built without, since they would open, and
         truncate, the same paths. The ranks check this together before any data moves and all raise ValueError when
-        another rank holds sinks. The return values are those of write_sinks=False."""
+        another rank holds sinks. The return values are those of write_sinks=False.
+        The clip is run_segments_sharded's single segment; a clip of any length streams through that."""
+        if isinstance(frames_u8, np.ndarray):
+            frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
+        n = frames_u8.shape[0]
+        (res,) = self.run_segments_sharded(lambda a, b: frames_u8[a:b], n, src_duration_s, t_offset,
+                                           segment_pairs=max(n - 1, 1), group=group, return_labels=return_labels,
+                                           write_sinks=write_sinks)
+        return res
+
+    def run_segments_sharded(self, get_frames, n_frames, src_duration_s, t_offset=0.0, segment_pairs=None, group=None,
+                             return_labels=False, write_sinks=False):
+        """ONE clip of any length over the ranks of `group`, segment by segment: a generator that yields, per segment,
+        what run_clip_sharded returns for that segment's interpolated frames -- (rows [M_r, 4] float32 host array of
+        this rank's rows (global y), interp_times_s, n_interp_frames), and the labels of the rows with return_labels.
+        Concatenated, the segments are what one run_clip_sharded(all frames, src_duration_s, t_offset) returns on a
+        fresh pipeline: every rank's rows (in the same order with row_order, the same multiset per frame without), the
+        times, frame counts, labels and emulator counters, and with write_sinks the first rank's event files.
+
+        Every rank calls it with the same arguments. get_frames(a, b) returns source frames a .. b-1 as uint8
+        [b-a, H, W], an ndarray or a tensor, on the host or the device (run_segments' contract); a rank asks only for
+        the frames its own pairs need. segment_pairs (default DEFAULT_SEGMENT_PAIRS per rank) is the segment length in
+        source frame pairs of the whole group: segments start on the clip's SloMo batch boundaries and each holds at
+        least `world` pairs, or with auto_upsample `world` batches (segment_plan(..., world, auto_upsample)).
+
+        Per segment every rank interpolates its share of the segment's pairs (write_video=False), the row bands are
+        exchanged (parallel.exchange_frame_bands) and the band emulator runs one generate_events_band_batch call, or
+        frame by frame in replay mode with noise; its state carries over to the next segment. write_sinks: the first
+        rank gathers, merges and writes each segment's bands. Device memory on a rank depends on the segment length,
+        not the clip length.
+
+        Times: the scale f of v2e.py:794-797 depends on the U of the clip's last batch. With a fixed U it follows from
+        the shapes; with auto_upsample and more than one segment the last rank runs the flow network on the clip's last
+        batch first (SuperSloMo.batch_upsampling) and broadcasts its U; the segment holding that batch raises
+        RuntimeError on every rank when its U differs. A single segment takes f from its own times.
+
+        Raises, on every rank and before any work, what run_clip_sharded raises: RuntimeError without a shard,
+        ValueError for return_labels without label_signal_noise, write_sinks without row_order or with sinks on another
+        rank than the first, and too short a clip. The frames a segment's get_frames calls return are checked by one
+        all-gather before any frame moves: every rank raises ValueError naming the segment and the rank whose frames
+        are not uint8 [b-a, H, W] with the clip's H, W."""
         import torch.distributed as dist
         from . import parallel
-        from .slomo import clip_times
         world, rank = dist.get_world_size(group), dist.get_rank(group)
+        write_sinks = self._sharded_refusals(group, return_labels, write_sinks)
+        sl, em = self.slomo, self.emulator
+        n = int(n_frames)
+        if n - 1 < world:
+            raise ValueError("fewer frame pairs than ranks")
+        auto = bool(sl.auto_upsample)
+        bs = max(1, min(int(sl.batch_size), n - 1))
+        if segment_pairs is None:
+            segment_pairs = DEFAULT_SEGMENT_PAIRS * world
+        plan = segment_plan(n, sl.batch_size, segment_pairs, world=world, auto_upsample=auto)
+        m = len(plan)
+        if rank == 0 and sl.writes_video():
+            logger.warning("video_path ignored: a clip sharded over ranks writes no upsampler video")
+        comm = em.device if dist.get_backend(group) == "nccl" else "cpu"
+        size = []
+
+        def fetch(a, b, k, mine=True):
+            """get_frames(a, b) on this rank (when mine), checked on every rank by one all-gather of (ok, H, W)."""
+            fr, ok, hw = None, 1, (-1, -1)
+            if mine:
+                fr = get_frames(a, b)
+                if isinstance(fr, np.ndarray):
+                    fr = torch.from_numpy(np.ascontiguousarray(fr))
+                ok = int(isinstance(fr, torch.Tensor) and fr.dtype == torch.uint8 and fr.dim() == 3
+                         and fr.shape[0] == b - a)
+                if ok:
+                    hw = tuple(fr.shape[1:])
+            v = torch.tensor([ok, hw[0], hw[1], a, b], dtype=torch.int64, device=comm)
+            vs = [torch.empty_like(v) for _ in range(world)]
+            dist.all_gather(vs, v, group=group)
+            vs = [x.tolist() for x in vs]
+            if not size:
+                size[:] = [tuple(x[1:3]) for x in vs if x[0] and x[1] >= 0][:1]
+            bad = [r for r, x in enumerate(vs) if not x[0] or (x[1] >= 0 and tuple(x[1:3]) != size[0])]
+            if bad:
+                r = bad[0]
+                want = "[%d, %d, %d]" % ((vs[r][4] - vs[r][3],) + size[0]) if size else "[%d, H, W]" % (vs[r][4] - vs[r][3])
+                got = "" if r != rank else ": it returned %s" % _describe(fr)
+                raise ValueError("segment %d of %d: rank %d's get_frames(%d, %d) did not return uint8 %s%s"
+                                 % (k, m, r, vs[r][3], vs[r][4], want, got))
+            return fr
+
+        f = u_last = None
+        if m > 1:
+            if auto:
+                a = (n - 2) // bs * bs
+                fr = fetch(a, n, m - 1, mine=rank == world - 1)
+                u = torch.tensor([0 if fr is None else sl.batch_upsampling(fr, n)], dtype=torch.int64, device=comm)
+                del fr
+                dist.broadcast(u, group=group, group_src=world - 1)
+                u_last = int(u.item())
+            else:
+                u_last = int(sl.upsampling_factor)
+            f = src_duration_s / sharded_span(n - 1, sl.batch_size, u_last, auto)
+        for k, (s0, s1) in enumerate(plan):
+            if auto:
+                p0, p1 = parallel.batch_pair_range(s1 - s0, bs, rank, world)
+            else:
+                p0, p1 = parallel.pair_range(s1 - s0, rank, world)
+            p0, p1 = p0 + s0, p1 + s0
+            fr = fetch(p0, p1 + 1, k)
+            H = size[0][0]
+            if auto:
+                local, _, _, ups_l = sl.interpolate_frames(fr, return_ups=True, write_video=False, first_pair=p0,
+                                                           clip_frames=n)
+                # every rank's per-batch U's (a few ints; each rank knows how many batches every rank holds)
+                nb = [-(-(b - a) // bs) for a, b in (parallel.batch_pair_range(s1 - s0, bs, r, world)
+                                                     for r in range(world))]
+                send = torch.zeros(max(nb), dtype=torch.int64, device=local.device)
+                send[:len(ups_l)] = torch.tensor(ups_l, dtype=torch.int64)
+                recv = [torch.empty_like(send) for _ in range(world)]
+                dist.all_gather(recv, send, group=group)
+                ups = [u for r in range(world) for u in recv[r][:nb[r]].tolist()]
+                times = sharded_times(n - 1, bs, (s0, s1), ups)
+                if k == m - 1 and u_last is not None and ups[-1] != u_last:
+                    raise RuntimeError("the clip's last batch got U=%d, its time-scale pre-pass U=%d"
+                                       % (ups[-1], u_last))
+            else:
+                local, times_l, _ = sl.interpolate_frames(fr, write_video=False)
+                U = int(sl.upsampling_factor)
+                times = sharded_times(n - 1, bs, (s0, s1), U)
+                assert np.allclose(times_l + p0, times[(p0 - s0) * U:(p1 - s0) * U])
+            del fr
+            if f is None:
+                f = src_duration_s / (np.max(times) - np.min(times))        # v2e.py:794-797
+            t = t_offset + f * times
+            bands = parallel.exchange_frame_bands(local, H, group=group, halo=em.cs_halo_rows(H))
+            del local
+            res = self._band_events(bands, t, H, k > 0, group, return_labels, write_sinks)
+            del bands
+            yield res
+
+    def _sharded_refusals(self, group, return_labels, write_sinks):
+        """run_clip_sharded's refusals, raised on every rank together. Returns whether the group's first rank writes
+        event files."""
+        import torch.distributed as dist
+        world = dist.get_world_size(group)
         em = self.emulator
         if em.shard is None:
             raise RuntimeError("run_clip_sharded needs EventEmulator(shard=(rank, world, group))")
         if return_labels and not em.label_signal_noise:
             raise ValueError("return_labels=True needs label_signal_noise=True")
-        if write_sinks:
-            if em.row_order is None:
-                raise ValueError("write_sinks=True needs EventEmulator(row_order='canonical' or 'shuffled'): the bands "
-                                 "are merged by their sort keys")
-            # every rank learns who holds sinks, so that all of them raise (none waits in a collective)
-            nccl = dist.get_backend(group) == "nccl"
-            flag = torch.tensor([0 if em._sinks is None else 1], dtype=torch.int64,
-                                device=em.device if nccl else "cpu")
-            flags = [torch.zeros_like(flag) for _ in range(world)]
-            dist.all_gather(flags, flag, group=group)
-            flags = [int(f.item()) for f in flags]
-            bad = [r for r in range(1, world) if flags[r]]
-            if bad:
-                raise ValueError("write_sinks=True: only the group's first rank may hold sinks, ranks %s do; build "
-                                 "their emulators without dvs_* keywords" % bad)
-            write_sinks = bool(flags[0])
-        if isinstance(frames_u8, np.ndarray):
-            frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
-        n, H, W = frames_u8.shape
-        if n - 1 < world:
-            raise ValueError("fewer frame pairs than ranks")
-        if rank == 0 and self.slomo.writes_video():
-            logger.warning("video_path ignored: a clip sharded over ranks writes no upsampler video")
-        if self.slomo.auto_upsample:
-            bs = max(1, min(int(self.slomo.batch_size), n - 1))
-            p0, p1 = parallel.batch_pair_range(n - 1, bs, rank, world)
-            local, _, _, ups_l = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1], return_ups=True,
-                                                              write_video=False)
-            # every rank's per-batch U's (a few ints; each rank knows how many batches every rank holds)
-            nb = [-(-(b - a) // bs) for a, b in (parallel.batch_pair_range(n - 1, bs, r, world) for r in range(world))]
-            send = torch.zeros(max(nb), dtype=torch.int64, device=local.device)
-            send[:len(ups_l)] = torch.tensor(ups_l, dtype=torch.int64)
-            recv = [torch.empty_like(send) for _ in range(world)]
-            dist.all_gather(recv, send, group=group)
-            ups = [u for r in range(world) for u in recv[r][:nb[r]].tolist()]
-            times, _ = clip_times(ups, n - 1, bs)
-        else:
-            p0, p1 = parallel.pair_range(n - 1, rank, world)
-            local, times_l, _ = self.slomo.interpolate_frames(frames_u8[p0:p1 + 1], write_video=False)
-            U = int(self.slomo.upsampling_factor)
-            times = np.arange((n - 1) * U) * (1.0 / U)                       # slomo.py:391-395 for the whole clip
-            assert np.allclose(times_l + p0, times[p0 * U:p1 * U])
-        bands = parallel.exchange_frame_bands(local, H, group=group, halo=em.cs_halo_rows(H))
-        f = src_duration_s / (np.max(times) - np.min(times))            # v2e.py:794-797
-        t = t_offset + f * times
+        if not write_sinks:
+            return False
+        if em.row_order is None:
+            raise ValueError("write_sinks=True needs EventEmulator(row_order='canonical' or 'shuffled'): the bands "
+                             "are merged by their sort keys")
+        # every rank learns who holds sinks, so that all of them raise (none waits in a collective)
+        nccl = dist.get_backend(group) == "nccl"
+        flag = torch.tensor([0 if em._sinks is None else 1], dtype=torch.int64, device=em.device if nccl else "cpu")
+        flags = [torch.zeros_like(flag) for _ in range(world)]
+        dist.all_gather(flags, flag, group=group)
+        flags = [int(f.item()) for f in flags]
+        bad = [r for r in range(1, world) if flags[r]]
+        if bad:
+            raise ValueError("write_sinks=True: only the group's first rank may hold sinks, ranks %s do; build "
+                             "their emulators without dvs_* keywords" % bad)
+        return bool(flags[0])
+
+    def _band_events(self, bands, t, H, cont, group, return_labels, write_sinks):
+        """The pixel model on this rank's bands of one segment's frames: what run_segments_sharded yields. cont: the
+        segment is not the clip's first (the sinks continue the AEDAT-2.0 rule across segments)."""
+        em = self.emulator
         extra = dict(return_labels=True) if return_labels else {}
         if em.rng_mode == "device" or not (em.leak_rate_hz > 0 or em.shot_noise_rate_hz > 0 or em.photoreceptor_noise):
             # chunks of frames through the multi-frame kernels: one all-reduce(MAX) of the frame maxima per chunk
@@ -226,7 +377,11 @@ class V2EPipeline:
                 return (res[0], t, bands.shape[0]) + tuple(res[2:])
             rows, offs, *labels, keys = em.generate_events_band_batch(bands, t, H, return_device=True,
                                                                       return_keys=True, **extra)
-            self._write_merged(rows, keys, offs, group)
+            em._sinks_continue = cont
+            try:
+                self._write_merged(rows, keys, offs, group)
+            finally:
+                em._sinks_continue = False
             labels = [labels[0].cpu().numpy().astype(bool)] if labels else []
             return (rows.cpu().numpy(), t, bands.shape[0]) + tuple(labels)
         assert not write_sinks, "row_order needs rng_mode='device', which takes the batched path"
