@@ -45,7 +45,7 @@ def test_cuda_renderer_matches_reference_fixtures():
             got = np.zeros((0, H, W)) if got is None else got
             assert got.dtype == np.float64 and got.shape == want.shape and np.array_equal(got, want), name
         done += 1
-    assert done == 7
+    assert done == 18
 
 
 @pytest.mark.gpu

@@ -19,19 +19,21 @@ int v2e_set_error(int code, const char *fmt, const char *detail);
 
 namespace {
 
-// blockIdx.y = frame; events [start, end) of that frame, grid-stride in x
+// frames grid-stride in y (a packet may finish more frames than gridDim.y can hold); events [start, end) of a frame,
+// grid-stride in x
 __global__ void __launch_bounds__(256)
 render_scatter_kernel(const float4 *__restrict__ ev, const int64_t *__restrict__ starts, const int64_t *__restrict__ ends,
-                      int H, int W, int32_t *__restrict__ acc) {
-    const int f = blockIdx.y;
-    const int64_t s = starts[f], e = ends[f];
-    int32_t *a = acc + (size_t)f * H * W;
-    for (int64_t i = s + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (int64_t)gridDim.x * blockDim.x) {
-        const float4 r = ev[i];                     // [t, x, y, p]
-        // hist2d_numba_seq: i = y * delta with delta = 1 / ((H - 0) / H) = 1: bin = int(y) if 0 <= y < H
-        const double yy = (double)r.z, xx = (double)r.y;
-        if (yy >= 0.0 && yy < (double)H && xx >= 0.0 && xx < (double)W)
-            atomicAdd(&a[(int)yy * W + (int)xx], r.w == 1.0f ? 1 : -1);     // pol_on = (p == 1), everything else is OFF
+                      int n_frames, int H, int W, int32_t *__restrict__ acc) {
+    for (int f = blockIdx.y; f < n_frames; f += gridDim.y) {
+        const int64_t s = starts[f], e = ends[f];
+        int32_t *a = acc + (size_t)f * H * W;
+        for (int64_t i = s + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (int64_t)gridDim.x * blockDim.x) {
+            const float4 r = ev[i];                     // [t, x, y, p]
+            // hist2d_numba_seq: i = y * delta with delta = 1 / ((H - 0) / H) = 1: bin = int(y) if 0 <= y < H
+            const double yy = (double)r.z, xx = (double)r.y;
+            if (yy >= 0.0 && yy < (double)H && xx >= 0.0 && xx < (double)W)
+                atomicAdd(&a[(int)yy * W + (int)xx], r.w == 1.0f ? 1 : -1);     // pol_on = (p == 1), everything else is OFF
+        }
     }
 }
 
@@ -111,8 +113,9 @@ extern "C" int v2e_render_frames(const float *events_dev, const int64_t *starts_
         int gx = (int)((max_events_per_frame + 255) / 256);
         if (gx > 1184) gx = 1184;
         if (gx < 1) gx = 1;
-        dim3 grid(gx, n_frames);
-        render_scatter_kernel<<<grid, 256, 0, st>>>((const float4 *)events_dev, starts_dev, ends_dev, height, width, acc_dev);
+        dim3 grid(gx, n_frames < 65535 ? n_frames : 65535);
+        render_scatter_kernel<<<grid, 256, 0, st>>>((const float4 *)events_dev, starts_dev, ends_dev, n_frames, height, width,
+                                                    acc_dev);
     }
     render_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(acc_dev, n, full_scale_count, frames_f64_dev, frames_u8_dev);
     CU(cudaGetLastError());

@@ -49,10 +49,16 @@ class EventRenderer(object):
             self.frameIntevalS = 1 / self.frame_rate_hz
         elif mode == ExposureMode.COUNT:
             self.event_count = int(self.exposure_value)
+            if self.event_count < 1:                      # a frame of 0 events never advances: renderer.py:283-285
+                raise ValueError("ExposureMode.COUNT needs an event count of at least 1, got %r" % (exposure_value,))
         elif mode == ExposureMode.AREA_COUNT:
             self.area_count = int(self.exposure_value)
             if not area_dimension:
                 raise ValueError("ExposureMode.AREA_COUNT needs area_dimension")
+            # the event that closes a frame opens the next one and counts 1 there: with area_count 1 that frame closes
+            # on the same event again and the scan never advances (renderer.py:254-265)
+            if self.area_count < 2:
+                raise ValueError("ExposureMode.AREA_COUNT needs an area count of at least 2, got %r" % (exposure_value,))
         self.video_output_file_name = dvs_vid
         self.video_output_file = None
         self.frame_times_output_file = None
@@ -116,7 +122,10 @@ class EventRenderer(object):
             self.currentFrameStartTime = np.float32(t0)
         cur = self.currentFrameStartTime
         curs = [cur]
-        while float(curs[-1]) <= t1 and len(curs) < 1 << 20:
+        while float(curs[-1]) <= t1:
+            if len(curs) >= 1 << 20:
+                raise ValueError("a DURATION packet may span at most 2^20 frame intervals of %g s; this one runs from "
+                                 "%r s to %r s: pass it in shorter packets" % (self.frameIntevalS, float(cur), t1))
             curs.append(curs[-1] + self.frameIntevalS)
         c = torch.tensor(np.asarray(curs, dtype=np.float64), device=ts.device)
         tsd = ts.double()
@@ -140,7 +149,9 @@ class EventRenderer(object):
         if self.area_counts is None:
             self._cells = (1 + width // self.area_dimension, 1 + height // self.area_dimension)
             self.area_counts = torch.zeros(self._cells, dtype=torch.int32, device=self.device)
-        cap = n // max(self.area_count, 1) + 2
+        # every frame but the first advances at least area_count - 1 events: the event that closes a frame is counted
+        # again as the first of the next one
+        cap = n // (self.area_count - 1) + 2
         st_t = torch.empty((cap,), dtype=torch.int64, device=self.device)
         en_t = torch.empty((cap,), dtype=torch.int64, device=self.device)
         nf = torch.zeros((1,), dtype=torch.int32, device=self.device)
