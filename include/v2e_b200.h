@@ -37,7 +37,7 @@ typedef enum V2eStatus {
 typedef enum V2eFrameDtype { V2E_U8 = 0, V2E_F32 = 1, V2E_F64 = 2 } V2eFrameDtype;
 
 const char *v2e_last_error(void);
-int v2e_version(void);    /* the ABI version, 205 (205: v2e_merge_bands) */
+int v2e_version(void);    /* the ABI version, 206 (205: v2e_merge_bands; 206: v2e_render_plan) */
 /* ABI guard for bindings that mirror the structs (ctypes): version and the sizes of V2eEmuCfg / V2eFrameInfo /
  * V2eUNetWeights as this library was compiled. A binding whose own sizes differ must refuse to load. */
 int v2e_abi_info(int *version, int *emu_cfg_size, int *frame_info_size, int *unet_weights_size);
@@ -570,13 +570,28 @@ int v2e_merge_bands(const float *rows_dev, const uint64_t *keys_dev, uint64_t n,
  * frames_f64_dev (nullable): (frame + fs) / (2 fs) float64, what the reference returns; frames_u8_dev (nullable):
  * uint8(img * 255), what it writes to the AVI (renderer.py:345-347). max_events_per_frame sizes the grid. */
 /* ------------------------------------------------------------------------- */
-/* ExposureMode.AREA_COUNT (renderer.py:246-261): frame slices of one packet -- a frame ends when a cell of
+/* The frame plan of one call (ABI 206): P packets, packet p the rows [packets_dev[2p], packets_dev[2p+1]) of rows0_dev
+ * when p == 0 and first_from_rows0 (a packet assembled from two calls' rows), of rows_dev otherwise ([n][4] float32,
+ * 16-byte aligned, times non-decreasing within a packet). For every frame any packet finishes, in packet order:
+ * starts_dev / ends_dev (end-exclusive rows of the packet's array), times_dev (the frame-times file's time, the float32
+ * or float64 value the reference computes). hdr_dev [8] int64: status (0 ok; 1 more than max_frames frames, nothing
+ * usable: call again with room for hdr[1]; 2 a DURATION packet spans 2^20 frame intervals or more: hdr[5] the packet,
+ * hdr[6] / hdr[7] its first start and last row time as double bits), frame count, largest slice (rows), the DURATION
+ * start to carry into the next call (double bits) and whether it is set. packet_first_dev [P+1]: each packet's first
+ * frame, then the frame count. Enqueue only; nothing is written outside these buffers.
+ * v2e_render_plan: exposure_mode 1 DURATION (interval; f64_starts: frame starts are summed in float64, else float32;
+ * cur / has_cur: the carried start; bounds_dev: [max_frames][2] double scratch), 2 COUNT (count), 4 SOURCE.
+ * v2e_render_area_scan: ExposureMode.AREA_COUNT (renderer.py:246-261) -- a frame ends when a cell of
  * area_dimension x area_dimension pixels has collected area_count events. counts_dev: [cells_w][cells_h] int32,
- * persistent between packets (zero it once). Sequential by definition: one thread walks the packet.
- * *n_frames_dev = finished frames (their slices in starts_dev / ends_dev), or -1 if more than max_frames. */
-int v2e_render_area_scan(const float *events_dev, int64_t n, int area_dimension, int area_count, int cells_w, int cells_h,
-                         int32_t *counts_dev, int64_t *starts_dev, int64_t *ends_dev, int max_frames,
-                         int32_t *n_frames_dev, void *stream);
+ * persistent between packets and calls (zero it once). Sequential by definition: one thread walks the packets. */
+int v2e_render_plan(const float *rows0_dev, const float *rows_dev, const int64_t *packets_dev, int n_packets,
+                    int first_from_rows0, int exposure_mode, double interval, int f64_starts, int64_t count, double cur,
+                    int has_cur, double *bounds_dev, int64_t *starts_dev, int64_t *ends_dev, double *times_dev,
+                    int64_t max_frames, int64_t *hdr_dev, int64_t *packet_first_dev, void *stream);
+int v2e_render_area_scan(const float *rows0_dev, const float *rows_dev, const int64_t *packets_dev, int n_packets,
+                         int first_from_rows0, int area_dimension, int area_count, int cells_w, int cells_h,
+                         int32_t *counts_dev, int64_t *starts_dev, int64_t *ends_dev, double *times_dev,
+                         int64_t max_frames, int64_t *hdr_dev, int64_t *packet_first_dev, void *stream);
 int v2e_render_frames(const float *events_dev, const int64_t *starts_dev, const int64_t *ends_dev, int n_frames,
                       int64_t max_events_per_frame, int height, int width, int full_scale_count, int32_t *acc_dev,
                       double *frames_f64_dev, uint8_t *frames_u8_dev, void *stream);

@@ -52,7 +52,7 @@ class V2eProbeSample(ctypes.Structure):
 
 V2E_OK, V2E_E_INVALID, V2E_E_CUDA, V2E_E_CAPACITY, V2E_E_ITER_CAP, V2E_E_STATE, V2E_E_UNSUPPORTED, V2E_E_FALLBACK = \
     0, -1, -2, -3, -4, -5, -6, -7
-ABI_VERSION = 205
+ABI_VERSION = 206
 U8, F32, F64 = 0, 1, 2
 
 _vp, _i, _d, _u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint64
@@ -134,7 +134,10 @@ _SIGS = {
     "v2e_prep_create": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(_vp)]),
     "v2e_prep_destroy": (_i, [_vp]),
     "v2e_prep_run": (_i, [_vp, _vp, _i, _vp, _vp]),
-    "v2e_render_area_scan": (_i, [_vp, ctypes.c_int64, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp]),
+    "v2e_render_plan": (_i, [_vp, _vp, _vp, _i, _i, _i, _d, _i, ctypes.c_int64, _d, _i, _vp, _vp, _vp, _vp,
+                             ctypes.c_int64, _vp, _vp, _vp]),
+    "v2e_render_area_scan": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, ctypes.c_int64, _vp, _vp,
+                                  _vp]),
     "v2e_render_frames": (_i, [_vp, _vp, _vp, _i, ctypes.c_int64, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "v2e_events_to_h5_rows": (_i, [_vp, _u64, _vp, _vp]),
     "v2e_events_to_aedat2": (_i, [_vp, _u64, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),

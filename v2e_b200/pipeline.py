@@ -86,9 +86,13 @@ def _describe(x):
 
 
 class V2EPipeline:
-    def __init__(self, slomo: SuperSloMo, emulator: EventEmulator):
+    def __init__(self, slomo: SuperSloMo, emulator: EventEmulator, renderer=None):
+        """renderer (optional): a v2e_b200.renderer.EventRenderer the runs feed with every segment's rows, in the packets
+        v2e.py's stage-3 loop renders (slomo.batch_size frames per packet, v2e.py:826-846), so that it writes the DVS
+        video and its frame-times file as v2e.py does. The caller owns it and calls its cleanup() after the clip."""
         self.slomo = slomo
         self.emulator = emulator
+        self.renderer = renderer
 
     def run(self, frames_u8, src_duration_s, t_offset=0.0, return_device=False, copy=False):
         """frames_u8: [N,H,W] uint8 source frames covering `src_duration_s` seconds.
@@ -130,10 +134,14 @@ class V2EPipeline:
         network first runs on the clip's last batch (fetched through get_frames) to pick its U. A single segment
         takes f from its own times, as run does.
 
+        With a renderer, each segment's rows go from the emulator's device buffer to renderer.render_frame_rows before
+        the segment is yielded, frame i counted from the clip's first interpolated frame; the packet that straddles a
+        segment boundary is held by the renderer, and the clip's last segment renders the leftover packet.
+
         Raises ValueError, naming the segment, when get_frames returns anything but uint8 [b-a, H, W] with the first
         segment's H, W; RuntimeError, before any work, where generate_events_batch refuses the emulator (replay mode
         with per-frame noise, a sharded emulator: run_clip_sharded takes a clip over ranks)."""
-        sl, em = self.slomo, self.emulator
+        sl, em, rd = self.slomo, self.emulator, self.renderer
         em.check_batch_path()
         n = int(n_frames)
         plan = segment_plan(n, sl.batch_size, segment_pairs)
@@ -154,6 +162,7 @@ class V2EPipeline:
             return fr
 
         f = u_last = None
+        first = 0                                           # the clip's index of the segment's first interpolated frame
         if m > 1:
             if sl.auto_upsample:
                 bs = max(1, min(int(sl.batch_size), n - 1))
@@ -173,11 +182,17 @@ class V2EPipeline:
             t = t_offset + f * times
             em._sinks_continue = k > 0
             try:
-                ev, offs = em.generate_events_batch(interp, t, return_device=return_device, copy=copy)
+                ev, offs = em.generate_events_batch(interp, t, return_device=return_device or rd is not None, copy=copy)
             finally:
                 em._sinks_continue = False
             nf = interp.shape[0]
             del interp
+            if rd is not None:
+                rd.render_frame_rows(ev, offs, first, sl.batch_size, end_of_clip=k == m - 1,
+                                     height=em.output_height, width=em.output_width)
+                if not return_device:
+                    ev = em._rows_to_host(ev.shape[0], copy=copy)
+            first += nf
             yield ev, offs, t, nf
 
     def run_clip_sharded(self, frames_u8, src_duration_s, t_offset=0.0, group=None, return_labels=False,
@@ -197,10 +212,12 @@ class V2EPipeline:
         write_sinks=True (needs row_order) writes the clip's event files: every rank's rows, sort keys, frame offsets and
         shot counts are gathered on the group's first rank (parallel.gather_band_outputs), which merges the bands on the
         device into the one-GPU stream (parallel.merge_by_key_device) and passes it, with its labels, to its own
-        emulator's write_events -- the files a single-GPU V2EPipeline.run writes. Only that rank's emulator may be built
-        with sink keywords (dvs_text, dvs_aedat2, ...); the others are built without, since they would open, and
-        truncate, the same paths. The ranks check this together before any data moves and all raise ValueError when
-        another rank holds sinks. The return values are those of write_sinks=False.
+        emulator's write_events -- the files a single-GPU V2EPipeline.run writes -- and, when that rank's pipeline has a
+        renderer, to the renderer: the DVS video and frame-times file of a single-GPU run. Only that rank's emulator may
+        be built with sink keywords (dvs_text, dvs_aedat2, ...) and only its pipeline may hold a renderer; the others
+        are built without, since they would open, and truncate, the same paths. The ranks check this together before
+        any data moves and all raise ValueError when another rank holds sinks or a renderer. The return values are those
+        of write_sinks=False. Without write_sinks no rank renders (rank 0 logs a warning when it holds a renderer).
         The clip is run_segments_sharded's single segment; a clip of any length streams through that."""
         if isinstance(frames_u8, np.ndarray):
             frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
@@ -245,6 +262,9 @@ class V2EPipeline:
         from . import parallel
         world, rank = dist.get_world_size(group), dist.get_rank(group)
         write_sinks = self._sharded_refusals(group, return_labels, write_sinks)
+        if rank == 0 and self.renderer is not None and not write_sinks:
+            logger.warning("renderer ignored: a clip sharded over ranks is rendered from the merged stream "
+                           "write_sinks=True builds")
         sl, em = self.slomo, self.emulator
         n = int(n_frames)
         if n - 1 < world:
@@ -287,6 +307,7 @@ class V2EPipeline:
             return fr
 
         f = u_last = None
+        first = 0                                           # the clip's index of the segment's first interpolated frame
         if m > 1:
             if auto:
                 a = (n - 2) // bs * bs
@@ -332,13 +353,14 @@ class V2EPipeline:
             t = t_offset + f * times
             bands = parallel.exchange_frame_bands(local, H, group=group, halo=em.cs_halo_rows(H))
             del local
-            res = self._band_events(bands, t, H, k > 0, group, return_labels, write_sinks)
+            res = self._band_events(bands, t, H, (k > 0, k == m - 1, first), group, return_labels, write_sinks)
+            first += bands.shape[0]
             del bands
             yield res
 
     def _sharded_refusals(self, group, return_labels, write_sinks):
-        """run_clip_sharded's refusals, raised on every rank together. Returns whether the group's first rank writes
-        event files."""
+        """run_clip_sharded's refusals, raised on every rank together. Returns whether the group's first rank merges the
+        bands: write_sinks and it writes event files or renders the DVS video."""
         import torch.distributed as dist
         world = dist.get_world_size(group)
         em = self.emulator
@@ -351,21 +373,29 @@ class V2EPipeline:
         if em.row_order is None:
             raise ValueError("write_sinks=True needs EventEmulator(row_order='canonical' or 'shuffled'): the bands "
                              "are merged by their sort keys")
-        # every rank learns who holds sinks, so that all of them raise (none waits in a collective)
+        # every rank learns who holds sinks (bit 0) or a renderer (bit 1), so that all of them raise (none waits in a
+        # collective)
         nccl = dist.get_backend(group) == "nccl"
-        flag = torch.tensor([0 if em._sinks is None else 1], dtype=torch.int64, device=em.device if nccl else "cpu")
+        flag = torch.tensor([(em._sinks is not None) | (self.renderer is not None) << 1], dtype=torch.int64,
+                            device=em.device if nccl else "cpu")
         flags = [torch.zeros_like(flag) for _ in range(world)]
         dist.all_gather(flags, flag, group=group)
         flags = [int(f.item()) for f in flags]
-        bad = [r for r in range(1, world) if flags[r]]
+        bad = [r for r in range(1, world) if flags[r] & 1]
         if bad:
             raise ValueError("write_sinks=True: only the group's first rank may hold sinks, ranks %s do; build "
                              "their emulators without dvs_* keywords" % bad)
+        bad = [r for r in range(1, world) if flags[r] & 2]
+        if bad:
+            raise ValueError("write_sinks=True: only the group's first rank may hold a renderer, ranks %s do; build "
+                             "their pipelines without one" % bad)
         return bool(flags[0])
 
-    def _band_events(self, bands, t, H, cont, group, return_labels, write_sinks):
-        """The pixel model on this rank's bands of one segment's frames: what run_segments_sharded yields. cont: the
-        segment is not the clip's first (the sinks continue the AEDAT-2.0 rule across segments)."""
+    def _band_events(self, bands, t, H, seg, group, return_labels, write_sinks):
+        """The pixel model on this rank's bands of one segment's frames: what run_segments_sharded yields. seg: (the
+        segment is not the clip's first (the sinks continue the AEDAT-2.0 rule across segments), it is the clip's last,
+        the clip's index of its first frame)."""
+        cont = seg[0]
         em = self.emulator
         extra = dict(return_labels=True) if return_labels else {}
         if em.rng_mode == "device" or not (em.leak_rate_hz > 0 or em.shot_noise_rate_hz > 0 or em.photoreceptor_noise):
@@ -379,7 +409,7 @@ class V2EPipeline:
                                                                       return_keys=True, **extra)
             em._sinks_continue = cont
             try:
-                self._write_merged(rows, keys, offs, group)
+                self._write_merged(rows, keys, offs, group, seg, H, bands.shape[-1])
             finally:
                 em._sinks_continue = False
             labels = [labels[0].cpu().numpy().astype(bool)] if labels else []
@@ -396,8 +426,9 @@ class V2EPipeline:
             return rows, t, bands.shape[0], (np.concatenate(labs) if labs else np.zeros((0,), bool))
         return rows, t, bands.shape[0]
 
-    def _write_merged(self, rows, keys, offs, group):
-        """write_sinks: the bands of every rank to the group's first rank, merged there and written to its sinks."""
+    def _write_merged(self, rows, keys, offs, group, seg, H, W):
+        """write_sinks: the bands of every rank to the group's first rank, merged there and written to its sinks and
+        rendered by its renderer (seg: see _band_events; H, W: the frame size)."""
         from . import parallel
         from .sinks import signnoise_labels
         em = self.emulator
@@ -408,3 +439,6 @@ class V2EPipeline:
         merged, moffs = parallel.merge_by_key_device(streams, ks, os_, ss, device=em.device)
         labels = signnoise_labels(moffs, np.sum(ss, axis=0), em.device) if em.label_signal_noise else None
         em.write_events(merged, labels)
+        if self.renderer is not None:
+            self.renderer.render_frame_rows(merged, moffs, seg[2], self.slomo.batch_size, end_of_clip=seg[1],
+                                            height=H, width=W)
