@@ -37,7 +37,7 @@ typedef enum V2eStatus {
 typedef enum V2eFrameDtype { V2E_U8 = 0, V2E_F32 = 1, V2E_F64 = 2 } V2eFrameDtype;
 
 const char *v2e_last_error(void);
-int v2e_version(void);    /* the ABI version, 206 (205: v2e_merge_bands; 206: v2e_render_plan) */
+int v2e_version(void);    /* the ABI version, 207 (205: v2e_merge_bands; 206: v2e_render_plan; 207: v2e_mjpeg_*) */
 /* ABI guard for bindings that mirror the structs (ctypes): version and the sizes of V2eEmuCfg / V2eFrameInfo /
  * V2eUNetWeights as this library was compiled. A binding whose own sizes differ must refuse to load. */
 int v2e_abi_info(int *version, int *emu_cfg_size, int *frame_info_size, int *unet_weights_size);
@@ -595,6 +595,23 @@ int v2e_render_area_scan(const float *rows0_dev, const float *rows_dev, const in
 int v2e_render_frames(const float *events_dev, const int64_t *starts_dev, const int64_t *ends_dev, int n_frames,
                       int64_t max_events_per_frame, int height, int width, int full_scale_count, int32_t *acc_dev,
                       double *frames_f64_dev, uint8_t *frames_u8_dev, void *stream);
+
+/* ------------------------------------------------------------------------- */
+/* Greyscale Motion-JPEG (ABI 207): the frames of v2e's AVI videos encoded on the device. Every frame is a baseline
+ * JPEG, 8-bit, one component, with the Annex K tables and a restart interval of one MCU row; the exact format is
+ * DESIGN.md section 4.4 (restated by oracle/mjpeg_oracle.py).
+ * v2e_mjpeg_bound: the bytes n_frames frames of width x height can take at most (every byte stuffed), -1 for a size
+ * outside 1..65535. v2e_mjpeg_create: an encoder for frames of width x height at quality 1..100, for calls of up to
+ * max_frames frames; allocates its scratch on the current device (348 bytes per 8x8 block per frame).
+ * v2e_mjpeg_encode: frames_dev [n_frames][height][width] uint8, contiguous; writes the n JPEGs one after another
+ * from out_dev (which holds v2e_mjpeg_bound(width, height, n_frames) bytes) and their sizes to sizes_dev [n_frames]
+ * int64: frame f starts at the sum of the sizes before it. V2E_E_CAPACITY for more than max_frames frames. Enqueue
+ * only. */
+int64_t v2e_mjpeg_bound(int width, int height, int n_frames);
+int v2e_mjpeg_create(int width, int height, int quality, int max_frames, void **handle);
+int v2e_mjpeg_encode(void *handle, const uint8_t *frames_dev, int n_frames, uint8_t *out_dev, int64_t *sizes_dev,
+                     void *stream);
+int v2e_mjpeg_destroy(void *handle);
 
 #ifdef __cplusplus
 }

@@ -7,5 +7,6 @@ include/v2e_b200.h) is loaded on first use and there is no CPU fallback.
 from .emulator import EventEmulator  # noqa: F401
 from .slomo import SuperSloMo  # noqa: F401
 from .pipeline import V2EPipeline  # noqa: F401
+from .video import MjpegWriter  # noqa: F401
 
-__all__ = ["EventEmulator", "SuperSloMo", "V2EPipeline"]
+__all__ = ["EventEmulator", "SuperSloMo", "V2EPipeline", "MjpegWriter"]

@@ -52,7 +52,7 @@ class V2eProbeSample(ctypes.Structure):
 
 V2E_OK, V2E_E_INVALID, V2E_E_CUDA, V2E_E_CAPACITY, V2E_E_ITER_CAP, V2E_E_STATE, V2E_E_UNSUPPORTED, V2E_E_FALLBACK = \
     0, -1, -2, -3, -4, -5, -6, -7
-ABI_VERSION = 206
+ABI_VERSION = 207
 U8, F32, F64 = 0, 1, 2
 
 _vp, _i, _d, _u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint64
@@ -158,6 +158,10 @@ _SIGS = {
     "v2e_emu_set_model_states": (_i, [_vp, ctypes.c_uint32, _vp]),
     "v2e_emu_model_state_read": (_i, [_vp, _vp, _u64, ctypes.POINTER(_i), _vp]),
     "v2e_emu_model_state_device": (_i, [_vp]),
+    "v2e_mjpeg_bound": (ctypes.c_int64, [_i, _i, _i]),
+    "v2e_mjpeg_create": (_i, [_i, _i, _i, _i, ctypes.POINTER(_vp)]),
+    "v2e_mjpeg_destroy": (_i, [_vp]),
+    "v2e_mjpeg_encode": (_i, [_vp, _vp, _i, _vp, _vp, _vp]),
 }
 
 

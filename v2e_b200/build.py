@@ -24,6 +24,7 @@ UNITS = {
     "sinks.cu": [],
     "prep.cu": [],
     "render.cu": [],
+    "mjpeg.cu": [],
 }
 
 

@@ -2183,7 +2183,7 @@ static int fail(int code, const char *fmt, const char *detail = "") {
 
 int v2e_set_error(int code, const char *fmt, const char *detail) { return fail(code, fmt, detail); }
 extern "C" const char *v2e_last_error(void) { return g_err; }
-extern "C" int v2e_version(void) { return 206; }
+extern "C" int v2e_version(void) { return 207; }
 extern "C" int v2e_abi_info(int *version, int *emu_cfg_size, int *frame_info_size, int *unet_weights_size) {
     if (version) *version = v2e_version();
     if (emu_cfg_size) *emu_cfg_size = (int)sizeof(V2eEmuCfg);

@@ -10,6 +10,8 @@ the device for all packets of a call at once (v2e_render_plan; AREA_COUNT, a seq
 device too, in chunks of RENDER_CHUNK_FRAMES frames. render_events_to_frames renders one packet; render_frame_rows
 renders the rows of consecutive pixel-model frames in the packets v2e.py forms. Writing the AVI (`dvs_vid`) is the
 reference's job: it is delegated to v2ecore.v2e_utils.video_writer when that imports, otherwise ignored with a warning.
+`video_writer` (a factory with that function's signature, e.g. v2e_b200.video.MjpegWriter) replaces it for this object's
+video; a writer with write_frames gets each chunk's uint8 frames on the device, with no host copy and no GRAY2BGR.
 """
 import ctypes
 import logging
@@ -38,7 +40,7 @@ class ExposureMode(Enum):
 class EventRenderer(object):
     def __init__(self, full_scale_count=3, output_path=None, dvs_vid=None, preview=False,
                  exposure_mode=ExposureMode.DURATION, exposure_value=1 / 300.0, area_dimension=None,
-                 frame_times_suffix='-frame_times.txt', avi_frame_rate=30, device="cuda:0"):
+                 frame_times_suffix='-frame_times.txt', avi_frame_rate=30, device="cuda:0", video_writer=None):
         mode = exposure_mode if isinstance(exposure_mode, ExposureMode) else ExposureMode(getattr(exposure_mode, "value", exposure_mode))
         self.exposure_mode = mode
         self.exposure_value = exposure_value
@@ -66,6 +68,7 @@ class EventRenderer(object):
             if self.area_count < 2:
                 raise ValueError("ExposureMode.AREA_COUNT needs an area count of at least 2, got %r" % (exposure_value,))
         self.video_output_file_name = dvs_vid
+        self.video_writer = video_writer
         self.video_output_file = None
         self.frame_times_output_file = None
         self.preview = preview
@@ -90,15 +93,18 @@ class EventRenderer(object):
             self.frame_times_output_file = None
 
     def _check_outputs_open(self):
-        """renderer.py:141-170, through the reference's own writer when it imports."""
+        """renderer.py:141-170, through the reference's own writer when it imports, or the video_writer factory."""
         if self.video_output_file is not None or not (self.output_path and type(self.video_output_file_name) is str):
             return
-        try:
-            from v2ecore.v2e_utils import checkAddSuffix, video_writer
-        except ImportError as e:
-            logger.warning("dvs_vid ignored: v2ecore.v2e_utils.video_writer is not importable (%s)", e)
-            self.video_output_file_name = None
-            return
+        if self.video_writer is not None:
+            video_writer, checkAddSuffix = self.video_writer, _with_suffix
+        else:
+            try:
+                from v2ecore.v2e_utils import checkAddSuffix, video_writer
+            except ImportError as e:
+                logger.warning("dvs_vid ignored: v2ecore.v2e_utils.video_writer is not importable (%s)", e)
+                self.video_output_file_name = None
+                return
         fn = checkAddSuffix(os.path.join(self.output_path, self.video_output_file_name), '.avi')
         self.video_output_file = video_writer(fn, self.height, self.width, frame_rate=self.avi_frame_rate)
         fn = checkAddSuffix(os.path.join(self.output_path, self.video_output_file_name), self.dvs_frame_times_suffix)
@@ -199,15 +205,16 @@ class EventRenderer(object):
         want_u8 = self.video_output_file is not None
         if F == 0 or not (want_u8 or want_img):
             return F, None
+        on_device = want_u8 and hasattr(self.video_output_file, "write_frames")
         starts, ends = self._bufs["starts"], self._bufs["ends"]
         img = torch.empty((F, H, W), dtype=torch.float64, device=self.device) if want_img else None
         ch = min(RENDER_CHUNK_FRAMES, F)
         acc = self._buf("acc", ch, torch.int32, shape=(H, W))
         u8 = self._buf("u8", ch, torch.uint8, shape=(H, W)) if want_u8 else None
-        u8_h = self._buf("u8_host", ch, torch.uint8, pinned=True, shape=(H, W)) if want_u8 else None
+        u8_h = self._buf("u8_host", ch, torch.uint8, pinned=True, shape=(H, W)) if want_u8 and not on_device else None
         p = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
         k0 = int(first[1]) if rows0 is not None else 0          # packet 0's frames read rows0
-        if want_u8:
+        if want_u8 and not on_device:
             import cv2
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream(self.device)
@@ -220,11 +227,15 @@ class EventRenderer(object):
                         n, big, H, W, int(self.full_scale_count), p(acc), None if img is None else p(img[c]), p(u8), sp))
                     if not want_u8:
                         continue
-                    u8_h[:n].copy_(u8[:n], non_blocking=True)
-                    stream.synchronize()
-                    host = u8_h[:n].numpy()
+                    if on_device:
+                        self.video_output_file.write_frames(u8[:n])
+                    else:
+                        u8_h[:n].copy_(u8[:n], non_blocking=True)
+                        stream.synchronize()
+                        host = u8_h[:n].numpy()
                     for f in range(n):
-                        self.video_output_file.write(cv2.cvtColor(host[f], cv2.COLOR_GRAY2BGR))
+                        if not on_device:
+                            self.video_output_file.write(cv2.cvtColor(host[f], cv2.COLOR_GRAY2BGR))
                         self.frame_times_output_file.write('{}\t{:10.6f}\n'.format(self.numFramesWritten, times[c + f]))
                         self.numFramesWritten += 1
         return F, img
@@ -311,6 +322,12 @@ class EventRenderer(object):
         if rows.shape[0]:
             buf[at:need].copy_(rows)
         return buf
+
+
+def _with_suffix(path, suffix):
+    """The path with its extension replaced by suffix, unless it already ends in suffix (what the reference's
+    checkAddSuffix does to the video and frame-times names)."""
+    return path if path.endswith(suffix) else os.path.splitext(path)[0] + suffix
 
 
 def cut_packets(offsets, first_frame, packet_frames, held=0, end_of_clip=False):

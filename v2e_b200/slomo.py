@@ -16,6 +16,8 @@ reference on a CUDA machine, this class always applies it.
 With `video_path` set, both paths write the reference's two videos (slomo.py:288-303, 468-491): `vid_orig`, the
 source frames, and `vid_slomo`, the interpolated frames in output order, each converted GRAY2BGR on the host and
 written through v2ecore.v2e_utils.video_writer (its codec) when that imports; otherwise a warning and no files.
+`video_writer` (a factory with that function's signature, e.g. v2e_b200.video.MjpegWriter) replaces it for this object's
+videos; writers with write_frames get each batch's uint8 frames on the device, with no host copy and no GRAY2BGR.
 `preview` windows are not opened.
 """
 import atexit
@@ -87,6 +89,12 @@ def _write_gray(writer, frames):
         writer.write(cv2.cvtColor(f, cv2.COLOR_GRAY2BGR))
         n += 1
     return n
+
+
+def _write_device(writer, frames):
+    """Hands a writer with write_frames uint8 [n, H, W] frames (a tensor, host or device); returns n."""
+    writer.write_frames(frames)
+    return int(frames.shape[0])
 
 
 def _weights_struct(state_dict, in_ch, out_ch, keep):
@@ -240,9 +248,10 @@ class SloMoEngine:
 class SuperSloMo(object):
     def __init__(self, model: str, auto_upsample: bool, upsampling_factor: object, batch_size=1,
                  video_path=None, vid_orig='original.avi', vid_slomo='slomo.avi', preview=False,
-                 avi_frame_rate=30, device="cuda:0", state_dicts=None):
+                 avi_frame_rate=30, device="cuda:0", state_dicts=None, video_writer=None):
         """`model`: checkpoint path as in the reference (slomo.py:44-54); `state_dicts` (extension):
-        a dict with 'state_dictFC' / 'state_dictAT' used instead of loading `model`."""
+        a dict with 'state_dictFC' / 'state_dictAT' used instead of loading `model`; `video_writer` (extension): the
+        factory that opens vid_orig / vid_slomo instead of v2ecore.v2e_utils.video_writer."""
         if not torch.cuda.is_available():
             raise RuntimeError("v2e_b200.SuperSloMo needs a CUDA device; there is no CPU fallback")
         self.device = device
@@ -259,6 +268,7 @@ class SuperSloMo(object):
         self.preview, self.avi_frame_rate = preview, avi_frame_rate
         self.ori_writer = self.slomo_writer = None      # opened on the first batch (slomo.py:288-303)
         self._writers_opened = False
+        self.video_writer = video_writer
         self.numOrigVideoFramesWritten = self.numSlomoVideoFramesWritten = 0
         self._state_dicts = state_dicts
         self._engine = None
@@ -293,11 +303,13 @@ class SuperSloMo(object):
         if self._writers_opened or not self.writes_video():
             return
         self._writers_opened = True
-        try:
-            from v2ecore.v2e_utils import video_writer
-        except ImportError as e:
-            logger.warning("video_path ignored: v2ecore.v2e_utils is not importable (%s)", e)
-            return
+        video_writer = self.video_writer
+        if video_writer is None:
+            try:
+                from v2ecore.v2e_utils import video_writer
+            except ImportError as e:
+                logger.warning("video_path ignored: v2ecore.v2e_utils is not importable (%s)", e)
+                return
         if self.vid_orig is not None:
             self.ori_writer = video_writer(os.path.join(self.video_path, self.vid_orig), H, W,
                                            frame_rate=self.avi_frame_rate)
@@ -411,11 +423,15 @@ class SuperSloMo(object):
                 chunks.append(blk)
             if write_video:
                 self._open_writers(H, W)
-                if self.slomo_writer is not None:
+                if hasattr(self.slomo_writer, "write_frames"):
+                    self.numSlomoVideoFramesWritten += _write_device(self.slomo_writer, blk)
+                elif self.slomo_writer is not None:
                     self.numSlomoVideoFramesWritten += _write_gray(self.slomo_writer, blk.cpu().numpy())
         if fixed is None:
             out = torch.cat(chunks, 0)
-        if write_video and self.ori_writer is not None:
+        if write_video and hasattr(self.ori_writer, "write_frames"):
+            self.numOrigVideoFramesWritten += _write_device(self.ori_writer, frames[1 if first_pair else 0:])
+        elif write_video and self.ori_writer is not None:
             self.numOrigVideoFramesWritten += _write_gray(self.ori_writer, frames[1 if first_pair else 0:].cpu().numpy())
         self._engine.check_finite()
         if return_ups:
@@ -457,15 +473,20 @@ class SuperSloMo(object):
         times, ups, out_ctr = [], [], 0
         for blk, tt, U in self._batches(get_frames, len(files), H, W):
             self._open_writers(H, W)
+            if hasattr(self.slomo_writer, "write_frames"):
+                self.numSlomoVideoFramesWritten += _write_device(self.slomo_writer, blk)
             host = blk.cpu().numpy()
             for i in range(host.shape[0]):
                 Image.fromarray(host[i]).save(os.path.join(output_folder, str(out_ctr + i) + ".png"))
-            if self.slomo_writer is not None:
+            if self.slomo_writer is not None and not hasattr(self.slomo_writer, "write_frames"):
                 self.numSlomoVideoFramesWritten += _write_gray(self.slomo_writer, host)
             out_ctr += host.shape[0]
             times.append(tt)
             ups.append(U)
-        if self.ori_writer is not None:
+        if hasattr(self.ori_writer, "write_frames"):
+            for a in range(0, len(files), 64):             # the source frames in blocks of 64 per encode
+                self.numOrigVideoFramesWritten += _write_device(self.ori_writer, get_frames(a, min(a + 64, len(files))))
+        elif self.ori_writer is not None:
             self.numOrigVideoFramesWritten += _write_gray(self.ori_writer, (np.load(f) for f in files))
         self._engine.check_finite()
         interp_times, avg = np.concatenate(times), sum(ups) / len(ups)
