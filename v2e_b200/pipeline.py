@@ -4,6 +4,9 @@ SuperSloMo up-sampling -> DVS events, everything device-resident.
 The reference hands frames from SloMo to the emulator as 8-bit PNG files in a temp dir
 (slomo.py:440-444 -> v2e.py:832 read_image); here the uint8 frames stay in HBM. Times follow
 v2e.py:794-797: interpTimes (units of source-frame intervals) scaled to the clip's duration.
+Without an upsampler (V2EPipeline(None, emulator): --disable_slomo, or a timestamp resolution that needs no
+upsampling) the source frames go to the pixel model themselves, at interpTimes = range(n) (v2e.py:776-797);
+run_synthetic runs v2e.py's --synthetic_input loop (v2e.py:580-607).
 """
 import logging
 
@@ -22,8 +25,16 @@ logger = logging.getLogger(__name__)
 # bench_stream.py measures the same time per frame at 16, 64 and 256 pairs as one run.
 DEFAULT_SEGMENT_PAIRS = 64
 
+# Source frames per segment without an upsampler (V2EPipeline(None, ...).run_segments, run_synthetic): the interpolated
+# frames of a DEFAULT_SEGMENT_PAIRS segment at U = 10, so that a segment holds as many frames on the device (and as
+# large an event buffer) as in the SloMo mode.
+DEFAULT_SEGMENT_FRAMES = 10 * DEFAULT_SEGMENT_PAIRS
 
-def segment_plan(n_frames, batch_size, segment_pairs=None, world=1, auto_upsample=False):
+# v2e.py's --batch_size default: the frames per rendered DVS packet when no upsampler sets it
+DEFAULT_BATCH_SIZE = 8
+
+
+def segment_plan(n_frames, batch_size, segment_pairs=None, world=1, auto_upsample=False, upsampler=True):
     """The segments V2EPipeline.run_segments runs a clip of n_frames source frames in, as pair ranges [(p0, p1)]:
     segment k interpolates pairs p0 .. p1-1 from source frames p0 .. p1, so consecutive segments share one source
     frame. segment_pairs (default DEFAULT_SEGMENT_PAIRS) is rounded up to a multiple of batch_size, which puts every
@@ -32,25 +43,32 @@ def segment_plan(n_frames, batch_size, segment_pairs=None, world=1, auto_upsampl
     world > 1: the segments of V2EPipeline.run_segments_sharded over `world` ranks, each one that run_clip_sharded
     accepts: at least `world` pairs, or with auto_upsample (whose batches are dealt to the ranks whole) at least
     `world` batches. segment_pairs is raised to that minimum before it is rounded, a shorter last segment is folded
-    into the one before it, and a clip shorter than one segment raises ValueError. world=1 gives the plan above."""
+    into the one before it, and a clip shorter than one segment raises ValueError. world=1 gives the plan above.
+
+    upsampler=False: the segments of a clip that runs without an upsampler, as frame ranges [(a, b)]: segment k runs
+    source frames a .. b-1, so segments share no frame. segment_pairs counts frames (default DEFAULT_SEGMENT_FRAMES)
+    and is not rounded; each segment holds at least `world` frames. batch_size and auto_upsample are not used. A clip
+    still needs two frames: v2e.py divides its duration by n_frames - 1."""
     n_frames, world = int(n_frames), int(world)
     if n_frames < 2:
         raise ValueError("n_frames=%d: a clip needs at least two source frames" % n_frames)
     if world < 1:
         raise ValueError("world=%d: a clip needs at least one rank" % world)
-    sp = DEFAULT_SEGMENT_PAIRS if segment_pairs is None else int(segment_pairs)
+    what = "frame pair" if upsampler else "frame"
+    sp = (DEFAULT_SEGMENT_PAIRS if upsampler else DEFAULT_SEGMENT_FRAMES) if segment_pairs is None else int(segment_pairs)
     if sp < 1:
-        raise ValueError("segment_pairs=%d: a segment needs at least one frame pair" % sp)
-    bs = max(1, int(batch_size))
+        raise ValueError("segment_pairs=%d: a segment needs at least one %s" % (sp, what))
+    auto_upsample = auto_upsample and upsampler
+    bs = max(1, int(batch_size)) if upsampler else 1
     unit = bs if auto_upsample else 1                    # pairs per share a rank must get at least one of
     sp = -(-max(sp, world * unit) // bs) * bs
-    n_pairs = n_frames - 1
-    plan = [(p0, min(p0 + sp, n_pairs)) for p0 in range(0, n_pairs, sp)]
+    n_units = n_frames - 1 if upsampler else n_frames
+    plan = [(p0, min(p0 + sp, n_units)) for p0 in range(0, n_units, sp)]
     p0, p1 = plan[-1]
     if -(-(p1 - p0) // unit) < world:
         if len(plan) == 1:
             raise ValueError("fewer batches of frame pairs than ranks" if auto_upsample else
-                             "fewer frame pairs than ranks")
+                             "fewer %ss than ranks" % what)
         plan[-2:] = [(plan[-2][0], p1)]
     return plan
 
@@ -86,13 +104,33 @@ def _describe(x):
 
 
 class V2EPipeline:
-    def __init__(self, slomo: SuperSloMo, emulator: EventEmulator, renderer=None):
-        """renderer (optional): a v2e_b200.renderer.EventRenderer the runs feed with every segment's rows, in the packets
-        v2e.py's stage-3 loop renders (slomo.batch_size frames per packet, v2e.py:826-846), so that it writes the DVS
-        video and its frame-times file as v2e.py does. The caller owns it and calls its cleanup() after the clip."""
+    def __init__(self, slomo: SuperSloMo, emulator: EventEmulator, renderer=None, batch_size=None):
+        """slomo: the upsampler, or None to run without one, as v2e.py does with --disable_slomo or when the timestamp
+        resolution needs no upsampling (v2e.py:414-422, 470-478): the source frames themselves then go to the pixel
+        model, frame i at t_offset + i * src_duration_s / (n_frames - 1) (v2e.py:776-797), and no upsampler video is
+        written.
+
+        renderer (optional): a v2e_b200.renderer.EventRenderer the runs feed with every segment's rows, in the packets
+        v2e.py's stage-3 loop renders (batch_size frames per packet, v2e.py:826-846), so that it writes the DVS
+        video and its frame-times file as v2e.py does. The caller owns it and calls its cleanup() after the clip.
+
+        batch_size: v2e.py's --batch_size, the frames per rendered packet. With slomo it is slomo.batch_size, and any
+        other value raises ValueError; without, it defaults to DEFAULT_BATCH_SIZE (v2e's default)."""
+        if slomo is not None:
+            if batch_size is not None and batch_size != slomo.batch_size:
+                raise ValueError("batch_size=%r differs from slomo.batch_size=%r: v2e.py renders packets of the "
+                                 "upsampler's batch size" % (batch_size, slomo.batch_size))
+        elif int(DEFAULT_BATCH_SIZE if batch_size is None else batch_size) < 1:
+            raise ValueError("batch_size=%r: a packet needs at least one frame" % (batch_size,))
         self.slomo = slomo
         self.emulator = emulator
         self.renderer = renderer
+        self._batch_size = None if slomo is not None else int(DEFAULT_BATCH_SIZE if batch_size is None else batch_size)
+
+    @property
+    def batch_size(self):
+        """The frames per rendered DVS packet: slomo.batch_size, or the constructor's batch_size without an upsampler."""
+        return self.slomo.batch_size if self.slomo is not None else self._batch_size
 
     def run(self, frames_u8, src_duration_s, t_offset=0.0, return_device=False, copy=False):
         """frames_u8: [N,H,W] uint8 source frames covering `src_duration_s` seconds.
@@ -103,7 +141,8 @@ class V2EPipeline:
             frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
         n = frames_u8.shape[0]
         (res,) = self.run_segments(lambda a, b: frames_u8[a:b], n, src_duration_s, t_offset,
-                                   segment_pairs=max(n - 1, 1), return_device=return_device, copy=copy)
+                                   segment_pairs=max(n - 1, 1) if self.slomo is not None else max(n, 1),
+                                   return_device=return_device, copy=copy)
         return res
 
     def run_segments(self, get_frames, n_frames, src_duration_s, t_offset=0.0, segment_pairs=None,
@@ -138,13 +177,23 @@ class V2EPipeline:
         the segment is yielded, frame i counted from the clip's first interpolated frame; the packet that straddles a
         segment boundary is held by the renderer, and the clip's last segment renders the leftover packet.
 
+        Without an upsampler (slomo None) the segments are disjoint runs of source frames: segment_pairs counts frames
+        (default DEFAULT_SEGMENT_FRAMES, the interpolated frames of a default SloMo segment at U = 10, so as much device
+        memory per segment), each segment's frames go to generate_events_batch as they are, and frame i gets the time
+        t_offset + f * i with f = src_duration_s / (n_frames - 1) in float64, v2e.py:794-797 over interpTimes =
+        range(n_frames). The yields have the same form, n_interp_frames being the segment's frame count. Frames
+        get_frames returns on the device are read in place; host frames go up in one copy per segment.
+
         Raises ValueError, naming the segment, when get_frames returns anything but uint8 [b-a, H, W] with the first
         segment's H, W; RuntimeError, before any work, where generate_events_batch refuses the emulator (replay mode
         with per-frame noise, a sharded emulator: run_clip_sharded takes a clip over ranks)."""
-        sl, em, rd = self.slomo, self.emulator, self.renderer
+        sl, em = self.slomo, self.emulator
         em.check_batch_path()
         n = int(n_frames)
-        plan = segment_plan(n, sl.batch_size, segment_pairs)
+        if sl is None:
+            plan = segment_plan(n, 1, segment_pairs, upsampler=False)
+        else:
+            plan = segment_plan(n, sl.batch_size, segment_pairs)
         m = len(plan)
         size = []
 
@@ -162,8 +211,9 @@ class V2EPipeline:
             return fr
 
         f = u_last = None
-        first = 0                                           # the clip's index of the segment's first interpolated frame
-        if m > 1:
+        if sl is None:
+            f = src_duration_s / np.int64(n - 1)              # v2e.py:794-797 over interpTimes = range(n)
+        elif m > 1:
             if sl.auto_upsample:
                 bs = max(1, min(int(sl.batch_size), n - 1))
                 a = (n - 2) // bs * bs
@@ -171,7 +221,12 @@ class V2EPipeline:
             else:
                 u_last = int(sl.upsampling_factor)
             f = src_duration_s / clip_span(n - 1, sl.batch_size, u_last)
-        for k, (p0, p1) in enumerate(plan):
+
+        def segment(k):
+            nonlocal f
+            p0, p1 = plan[k]
+            if sl is None:
+                return fetch(p0, p1, k), t_offset + f * np.arange(p0, p1), k == m - 1
             fr = fetch(p0, p1 + 1, k)
             interp, times, _, ups = sl.interpolate_frames(fr, return_ups=True, first_pair=p0, clip_frames=n)
             del fr
@@ -179,20 +234,92 @@ class V2EPipeline:
                 f = src_duration_s / (np.max(times) - np.min(times))          # v2e.py:794-797
             elif k == m - 1 and ups[-1] != u_last:
                 raise RuntimeError("the clip's last batch got U=%d, its time-scale pre-pass U=%d" % (ups[-1], u_last))
-            t = t_offset + f * times
+            return interp, t_offset + f * times, k == m - 1
+        yield from self._emulate(segment, 0, return_device, copy)
+
+    def run_synthetic(self, source, segment_frames=None, t_offset=0.0, return_device=False, copy=False):
+        """v2e.py's --synthetic_input loop (v2e.py:580-607) segment by segment: a generator that yields, per segment,
+        (events [M,4] float32, frame offsets [T+1], times_s [T], T), as run_segments does.
+
+        source: a v2ecore.base_synthetic_input, or anything with its next_frame() -> (frame [H, W] or None at the end,
+        time in seconds). Frames may be uint8, float32 or float64 (log_input / HDR frames), ndarrays or tensors, every
+        one of the first frame's shape and dtype; other numeric dtypes are read as float64. Each frame gets the
+        source's own time plus t_offset. Up to segment_frames frames (default DEFAULT_SEGMENT_FRAMES) are pulled per
+        segment and copied as they arrive (a source may reuse its frame array), into a buffer of pinned host memory
+        (for host frames) that goes to the device in one copy, and run by one generate_events_batch call. The caller
+        owns the source and calls its cleanup().
+
+        With a renderer the rows are rendered in the synthetic loop's packets, which end one frame later than
+        stage 3's: that loop counts frame i as i + 1 before its `% batch_size == 0` test, so the packet closes after
+        frame i when (i + 1) % batch_size == 0 and frame i has rows, and the leftover rows are rendered at the end.
+
+        Raises ValueError, naming the frame, for a frame of another shape or dtype than the first, or not [H, W];
+        RuntimeError, before any work, where generate_events_batch refuses the emulator."""
+        em = self.emulator
+        em.check_batch_path()
+        sf = DEFAULT_SEGMENT_FRAMES if segment_frames is None else int(segment_frames)
+        if sf < 1:
+            raise ValueError("segment_frames=%d: a segment needs at least one frame" % sf)
+        dev = torch.device(em.device)
+        nxt = source.next_frame()
+        if nxt[0] is None:
+            return
+        want = []                                           # the first frame's (shape, dtype)
+        stage = [None, None]                                # the segment buffer, the event its last upload records
+        pulled = 0                                          # frames taken from the source so far
+
+        def segment(k):
+            nonlocal nxt, pulled
+            buf, uploaded = stage
+            if uploaded is not None:
+                uploaded.synchronize()                      # the previous segment's frames have left the buffer
+            fr, t = nxt
+            times = []
+            while fr is not None and len(times) < sf:
+                x = torch.as_tensor(fr)
+                if not want:
+                    want[:] = [tuple(x.shape), x.dtype]
+                if x.dim() != 2 or tuple(x.shape) != want[0] or x.dtype != want[1]:
+                    raise ValueError("frame %d: next_frame() returned %s, expected [H, W] like frame 0 (%s %s)"
+                                     % (pulled, _describe(fr), str(want[1]).replace("torch.", ""), list(want[0])))
+                if buf is None:
+                    dt = x.dtype if x.dtype in (torch.uint8, torch.float32, torch.float64) else torch.float64
+                    pin = x.device.type == "cpu" and dev.type == "cuda"
+                    buf = stage[0] = torch.empty((sf,) + want[0], dtype=dt, device=x.device, pin_memory=pin)
+                buf[len(times)].copy_(x)
+                times.append(float(t))
+                pulled += 1
+                fr, t = source.next_frame()
+            nxt = (fr, t)
+            frames = buf[:len(times)].to(dev, non_blocking=True)
+            if buf.is_pinned():
+                stage[1] = torch.cuda.Event()
+                stage[1].record(torch.cuda.current_stream(dev))
+            return frames, t_offset + np.asarray(times, np.float64), fr is None
+        yield from self._emulate(segment, 1, return_device, copy)
+
+    def _emulate(self, segment, first, return_device, copy):
+        """The pixel model and the renderer over a clip's segments, what every single-GPU run yields: segment(k)
+        returns segment k's frames [T, H, W], their times in seconds and whether it is the clip's last segment. first:
+        the index the render loop gives the clip's first frame (v2e.py's stage-3 loop 0, its synthetic loop 1)."""
+        em, rd = self.emulator, self.renderer
+        k, last = 0, False
+        while not last:
+            fr, t, last = segment(k)
             em._sinks_continue = k > 0
             try:
-                ev, offs = em.generate_events_batch(interp, t, return_device=return_device or rd is not None, copy=copy)
+                ev, offs = em.generate_events_batch(fr, t, return_device=return_device or rd is not None, copy=copy)
             finally:
                 em._sinks_continue = False
-            nf = interp.shape[0]
-            del interp
+            nf = fr.shape[0]
+            del fr
             if rd is not None:
-                rd.render_frame_rows(ev, offs, first, sl.batch_size, end_of_clip=k == m - 1,
+                rd.render_frame_rows(ev, offs, first, self.batch_size, end_of_clip=last,
                                      height=em.output_height, width=em.output_width)
                 if not return_device:
                     ev = em._rows_to_host(ev.shape[0], copy=copy)
             first += nf
+            k += 1
             yield ev, offs, t, nf
 
     def run_clip_sharded(self, frames_u8, src_duration_s, t_offset=0.0, group=None, return_labels=False,
@@ -223,8 +350,8 @@ class V2EPipeline:
             frames_u8 = torch.from_numpy(np.ascontiguousarray(frames_u8))
         n = frames_u8.shape[0]
         (res,) = self.run_segments_sharded(lambda a, b: frames_u8[a:b], n, src_duration_s, t_offset,
-                                           segment_pairs=max(n - 1, 1), group=group, return_labels=return_labels,
-                                           write_sinks=write_sinks)
+                                           segment_pairs=max(n - 1, 1) if self.slomo is not None else max(n, 1),
+                                           group=group, return_labels=return_labels, write_sinks=write_sinks)
         return res
 
     def run_segments_sharded(self, get_frames, n_frames, src_duration_s, t_offset=0.0, segment_pairs=None, group=None,
@@ -253,6 +380,11 @@ class V2EPipeline:
         batch first (SuperSloMo.batch_upsampling) and broadcasts its U; the segment holding that batch raises
         RuntimeError on every rank when its U differs. A single segment takes f from its own times.
 
+        Without an upsampler (slomo None) the segments are disjoint runs of source frames, segment_pairs counting
+        frames (default DEFAULT_SEGMENT_FRAMES per rank, at least `world` per segment); each rank fetches its contiguous
+        run of a segment's frames (parallel.pair_range over frames) and passes it to the band exchange; the times are
+        run_segments' (t_offset + f * i, f = src_duration_s / (n_frames - 1)).
+
         Raises, on every rank and before any work, what run_clip_sharded raises: RuntimeError without a shard,
         ValueError for return_labels without label_signal_noise, write_sinks without row_order or with sinks on another
         rank than the first, and too short a clip. The frames a segment's get_frames calls return are checked by one
@@ -267,15 +399,20 @@ class V2EPipeline:
                            "write_sinks=True builds")
         sl, em = self.slomo, self.emulator
         n = int(n_frames)
-        if n - 1 < world:
-            raise ValueError("fewer frame pairs than ranks")
-        auto = bool(sl.auto_upsample)
-        bs = max(1, min(int(sl.batch_size), n - 1))
-        if segment_pairs is None:
-            segment_pairs = DEFAULT_SEGMENT_PAIRS * world
-        plan = segment_plan(n, sl.batch_size, segment_pairs, world=world, auto_upsample=auto)
+        if sl is None:
+            plan = segment_plan(n, 1, DEFAULT_SEGMENT_FRAMES * world if segment_pairs is None else segment_pairs,
+                                world=world, upsampler=False)
+            auto = False
+        else:
+            if n - 1 < world:
+                raise ValueError("fewer frame pairs than ranks")
+            auto = bool(sl.auto_upsample)
+            bs = max(1, min(int(sl.batch_size), n - 1))
+            if segment_pairs is None:
+                segment_pairs = DEFAULT_SEGMENT_PAIRS * world
+            plan = segment_plan(n, sl.batch_size, segment_pairs, world=world, auto_upsample=auto)
         m = len(plan)
-        if rank == 0 and sl.writes_video():
+        if rank == 0 and sl is not None and sl.writes_video():
             logger.warning("video_path ignored: a clip sharded over ranks writes no upsampler video")
         comm = em.device if dist.get_backend(group) == "nccl" else "cpu"
         size = []
@@ -308,7 +445,9 @@ class V2EPipeline:
 
         f = u_last = None
         first = 0                                           # the clip's index of the segment's first interpolated frame
-        if m > 1:
+        if sl is None:
+            f = src_duration_s / np.int64(n - 1)              # v2e.py:794-797 over interpTimes = range(n)
+        elif m > 1:
             if auto:
                 a = (n - 2) // bs * bs
                 fr = fetch(a, n, m - 1, mine=rank == world - 1)
@@ -323,11 +462,13 @@ class V2EPipeline:
             if auto:
                 p0, p1 = parallel.batch_pair_range(s1 - s0, bs, rank, world)
             else:
-                p0, p1 = parallel.pair_range(s1 - s0, rank, world)
+                p0, p1 = parallel.pair_range(s1 - s0, rank, world)      # without an upsampler: frames
             p0, p1 = p0 + s0, p1 + s0
-            fr = fetch(p0, p1 + 1, k)
+            fr = fetch(p0, p1 if sl is None else p1 + 1, k)
             H = size[0][0]
-            if auto:
+            if sl is None:
+                local, times = fr.to(em.device, non_blocking=True), np.arange(s0, s1)
+            elif auto:
                 local, _, _, ups_l = sl.interpolate_frames(fr, return_ups=True, write_video=False, first_pair=p0,
                                                            clip_frames=n)
                 # every rank's per-batch U's (a few ints; each rank knows how many batches every rank holds)
@@ -440,5 +581,5 @@ class V2EPipeline:
         labels = signnoise_labels(moffs, np.sum(ss, axis=0), em.device) if em.label_signal_noise else None
         em.write_events(merged, labels)
         if self.renderer is not None:
-            self.renderer.render_frame_rows(merged, moffs, seg[2], self.slomo.batch_size, end_of_clip=seg[1],
+            self.renderer.render_frame_rows(merged, moffs, seg[2], self.batch_size, end_of_clip=seg[1],
                                             height=H, width=W)
