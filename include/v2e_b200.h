@@ -401,6 +401,23 @@ int v2e_conv2d_lrelu_sm100_strip(const void *x1_dev, int C1, const void *x2_dev,
                                  int out_mode, int co_real, float slope, void *stream);
 int v2e_conv_strip_pick_kc(int C1, int C2, int Cout_pad, int KH, int KW, int W);
 
+/* wgmma chain of the strip kernel. PAIRED: per input row, slab, column and 16 channels, one wgmma of N = BN for each
+ * of the two output rows it feeds. STACKED: one wgmma of N = 2 * BN over weight tiles stacked in shared memory with
+ * zero tiles at both ends (more resident weights, so not every layer fits). AUTO: the chain
+ * v2e_conv_strip_pick_chain names, what v2e_conv2d_lrelu_sm100_strip and the SloMo networks run. Both chains give
+ * the same output bit for bit (inputs without Inf / NaN). */
+enum {
+    V2E_STRIP_CHAIN_AUTO = -1,
+    V2E_STRIP_CHAIN_PAIRED = 0,
+    V2E_STRIP_CHAIN_STACKED = 1
+};
+int v2e_conv2d_lrelu_sm100_strip_chain(const void *x1_dev, int C1, const void *x2_dev, int C2,
+                                       const void *wgt_row_dev, const float *bias_dev, int Cout_pad, int KH,
+                                       int KW, int N, int H, int W, void *out_dev, int out_cstride,
+                                       int out_mode, int co_real, float slope, int chain, void *stream);
+/* The chain AUTO runs for a layer (no GPU needed): PAIRED or STACKED, -1 = not a strip layer. */
+int v2e_conv_strip_pick_chain(int C1, int C2, int Cout_pad, int KH, int KW, int W);
+
 /* conv2d 3x3 (+bias +LeakyReLU) over the x2 bilinear up-sampling (align_corners=False) of x_low, i.e. the first
  * convolution of an up block (model.py:140-147: interpolate -> conv1 -> leaky_relu) WITHOUT materialising the
  * up-sampled tensor: the up-sampling is folded into four phase-specific 3x3 filters over the low-resolution

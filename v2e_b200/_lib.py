@@ -105,6 +105,9 @@ _SIGS = {
     "v2e_conv2d_lrelu_sm100_strip": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
                                           ctypes.c_float, _vp]),
     "v2e_conv_strip_pick_kc": (_i, [_i, _i, _i, _i, _i, _i]),
+    "v2e_conv2d_lrelu_sm100_strip_chain": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i,
+                                                ctypes.c_float, _i, _vp]),
+    "v2e_conv_strip_pick_chain": (_i, [_i, _i, _i, _i, _i, _i]),
     "v2e_conv2d_up2_lrelu_sm100": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, ctypes.c_float, _vp]),
     "v2e_conv_up2_fold_weights": (_i, [_vp, _i, _i, _i, _i, _vp]),
     "v2e_conv_up2_supported_c": (_i, [_i, _i, _i]),

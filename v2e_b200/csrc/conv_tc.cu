@@ -310,10 +310,11 @@ constexpr int kRowTile = 128;
 // tap (r, s) is a descriptor offset: ring slot of input row y+r-ph, start + s pixels.
 //   warp 8     : TMA producer: the weights once per CTA, then one row (all slabs) per ring slot.
 //   warps 0..7 : two consumer warpgroups, taking turns over PAIRS of output rows of an item (warpgroup g:
-//                pairs g, g+2, ...). Per 64-pixel half of the strip, the pair's wgmmas (M = 64, N = BN, both rows)
-//                are one asynchronous chain over the KH+1 input rows (strip_pair_mma); then bias, LeakyReLU and
-//                the store. A ring slot is released by both warpgroups (every row of the item exactly once each)
-//                when neither needs it any more.
+//                pairs g, g+2, ...). Per 64-pixel half of the strip, the pair's wgmmas are one asynchronous chain
+//                over the KH+1 input rows: two of M = 64, N = BN per input row (strip_pair_mma), or, with the
+//                weight tiles stacked in shared memory (STACK), one of N = 2 * BN (strip_stack_mma); then bias,
+//                LeakyReLU and the store. A ring slot is released by both warpgroups (every row of the item exactly
+//                once each) when neither needs it any more.
 // POOL: F.avg_pool2d(out, 2) written beside the output (model.py:71: the pool that opens a down block). A pair
 // is rows (2k, 2k+1) of the item (items start on even rows), so both rows of a 2x2 window are in the same
 // registers; the horizontal neighbour is the lane 4 apart.
@@ -361,11 +362,12 @@ struct RowRing {
     }
 };
 
-// One committed wgmma group: output rows (row0, row0+1) of a strip item over one 64-pixel half (a_off: its start in a
-// row buffer). Input row row0+r' (r' = 0..KH) feeds row0 with tap r' and row0+1 with tap r'-1, so the two rows' MMAs
-// interleave in one chain over the KH+1 input rows. An odd last row of an item has no input row row0+KH in the
-// ring: last = KH-1 reads row row0+KH-1 in its place, and the epilogue drops the row row0+1 this makes. Every output
-// element accumulates its terms in the order (r, slab, s, channel).
+// The wgmmas of input rows row0+rp0 .. row0+rp1-1 for output rows (row0, row0+1) of a strip item over one 64-pixel
+// half (a_off: its start in a row buffer); the caller zeroes the accumulators, fences and commits, so that a pair's
+// chain can be committed in several groups (conv_strip_kernel). Input row row0+r' (r' = 0..KH) feeds row0 with tap r'
+// and row0+1 with tap r'-1, so the two rows' MMAs interleave in one chain over the KH+1 input rows. An odd last row of
+// an item has no input row row0+KH in the ring: last = KH-1 reads row row0+KH-1 in its place, and the epilogue drops
+// the row row0+1 this makes. Every output element accumulates its terms in the order (r, slab, s, channel).
 // The accumulators are zeroed before the fence and never copied inside the chain: a register move that ptxas places
 // between two wgmmas (zeroing sunk past the fence, a path that skips a loop, accumulators merged from two code
 // paths, or one accumulator used by wgmmas of two widths) makes it wait for each wgmma before the next. Hence the
@@ -373,18 +375,12 @@ struct RowRing {
 // would be a second path), and one code path for both row counts.
 template <int KW, int KC, int BN>
 __device__ __forceinline__ void strip_pair_mma(float (&acc)[2][BN / 2], const RowRing &rr, int row0, int last, int slabs,
-                                               uint64_t dr, uint64_t dw, uint32_t a_off, uint32_t row16, uint32_t slab16) {
+                                                uint64_t dr, uint64_t dw, uint32_t a_off, uint32_t row16, uint32_t slab16,
+                                                int rp0, int rp1) {
     constexpr int KH = KW, taps = KH * KW;
     constexpr uint32_t rowb16 = (KC * 2u) >> 4, tile16 = (BN * KC * 2u) >> 4;
 #pragma unroll
-    for (int k = 0; k < 2; k++) {
-#pragma unroll
-        for (int i = 0; i < BN / 2; i++) acc[k][i] = 0.f;
-        wgmma_fence_regs(acc[k]);
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int rp = 0; rp <= KH; rp++) {
+    for (int rp = rp0; rp < rp1; rp++) {
         const uint32_t a_row = rr.slot(row0 + (rp < KH ? rp : last)) * row16 + a_off;
         int sl = 0;
 #pragma unroll 1
@@ -401,10 +397,50 @@ __device__ __forceinline__ void strip_pair_mma(float (&acc)[2][BN / 2], const Ro
             }
         } while (++sl < slabs);
     }
-    wgmma_commit();
 }
 
-template <int KW, int KC, int BN, bool POOL>
+// Stacked weight tiles (STACK = true): per slab, shared memory holds Z, (s = 0: r = KH-1 .. 0), Z, (s = 1: r = KH-1
+// .. 0), Z, ..., Z -- KW * (KH+1) + 1 tiles of BN x KC, Z a zero tile. Tile (r', s) and the one after it are then
+// taps (r', s) and (r'-1, s), with Z standing for the tap r' = KH of the upper row and r'-1 = -1 of the lower row, so
+// the 2 * BN contiguous rows from tile (r', s) are the B operand of both output rows at once.
+template <int KW>
+__device__ __forceinline__ constexpr int stack_tiles() { return KW * (KW + 1) + 1; }
+// tile of tap (r, s) in its slab's stack; r = KH is the zero tile in front of column s
+template <int KW>
+__device__ __forceinline__ constexpr int stack_index(int r, int s) { return s * (KW + 1) + KW - r; }
+
+// strip_pair_mma over stacked weight tiles: input row row0+r' feeds both output rows through ONE wgmma of N = 2 * BN
+// per (slab, s, k16) -- the A window is read once, and every wgmma of the chain has the same width. acc is that
+// wgmma's fragment: columns 0..BN-1 (row row0) in acc[0 .. BN/2), BN..2BN-1 (row row0+1) in acc[BN/2 .. BN), the
+// layout of strip_pair_mma' acc[2][BN/2]. The extra terms (Z at r' = KH for the upper row, at r' = 0 for the lower
+// row) are exact zeros added to an accumulator that starts at +0 and, absent Inf / NaN inputs, never is -0, so
+// every output element is bit-identical to strip_pair_mma', summed in the same (r, slab, s, channel) order.
+template <int KW, int KC, int BN>
+__device__ __forceinline__ void strip_stack_mma(float (&acc)[BN], const RowRing &rr, int row0, int last, int slabs,
+                                                 uint64_t dr, uint64_t dw, uint32_t a_off, uint32_t row16, uint32_t slab16,
+                                                 int rp0, int rp1) {
+    constexpr int KH = KW;
+    constexpr uint32_t rowb16 = (KC * 2u) >> 4, tile16 = (BN * KC * 2u) >> 4, wslab16 = stack_tiles<KW>() * tile16;
+#pragma unroll
+    for (int rp = rp0; rp < rp1; rp++) {
+        const uint32_t a_row = rr.slot(row0 + (rp < KH ? rp : last)) * row16 + a_off;
+        int sl = 0;
+#pragma unroll 1
+        do {
+            const uint32_t a_lo = a_row + (uint32_t)sl * slab16;
+            const uint32_t w_lo = (uint32_t)sl * wslab16 + (uint32_t)stack_index<KW>(rp, 0) * tile16;
+#pragma unroll
+            for (int s = 0; s < KW; s++) {
+#pragma unroll
+                for (int j = 0; j < KC / 16; j++)
+                    wgmma_f16<2 * BN>(acc, desc_add(dr, a_lo + (uint32_t)s * rowb16 + 2u * j),
+                                      desc_add(dw, w_lo + (uint32_t)(s * (KH + 1)) * tile16 + 2u * j), 1u);
+            }
+        } while (++sl < slabs);
+    }
+}
+
+template <int KW, int KC, int BN, bool POOL, bool STACK>
 __global__ void __launch_bounds__(kStripThreads, 1)
 conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                   const __grid_constant__ CUtensorMap tmB, const StripParams p) {
@@ -423,6 +459,16 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int split = (int)blockIdx.x % p.n_split, co_off = split * BN;
     const int item0 = (int)blockIdx.x / p.n_split, item_step = (int)gridDim.x / p.n_split;
 
+    if constexpr (STACK) {
+        // the zero tiles of the stacks, before any wgmma can read them (the fence hands them to the async proxy)
+        constexpr int z_vec = (int)tile_bytes / 16, z_per_slab = KW + 1;
+        for (int i = threadIdx.x; i < slabs * z_per_slab * z_vec; i += blockDim.x) {
+            const int z = i / z_vec, sl = z / z_per_slab, s = z % z_per_slab;
+            ((uint4 *)(smem + ((size_t)sl * stack_tiles<KW>() + (size_t)s * (KH + 1)) * tile_bytes))[i % z_vec] =
+                make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async();
+    }
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.nslot; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
         mbar_init(&w_bar, 1);
@@ -438,9 +484,12 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (warp == kProducerWarp) {
         // ===== TMA producer =====
         if (lane == 0) {
-            mbar_expect_tx(&w_bar, (uint32_t)p.w_bytes);
-            for (int t = 0; t < slabs * taps; t++)              // tile (slab, tap) of this CTA's output channels
-                tma_load_2d(smem + (size_t)t * tile_bytes, &tmB, &w_bar, 0, t * p.cout_pad + co_off);
+            mbar_expect_tx(&w_bar, (uint32_t)(slabs * taps) * tile_bytes);
+            for (int t = 0; t < slabs * taps; t++) {            // tile (slab, tap) of this CTA's output channels
+                const int sl = t / taps, tap = t % taps;
+                const int dst = STACK ? sl * stack_tiles<KW>() + stack_index<KW>(tap / KW, tap % KW) : t;
+                tma_load_2d(smem + (size_t)dst * tile_bytes, &tmB, &w_bar, 0, t * p.cout_pad + co_off);
+            }
             uint32_t cnt = 0;                                   // input rows loaded so far (all items)
             for (int item = item0; item < p.n_items; item += item_step) {
                 const int tx = item % p.tiles_x, rest = item / p.tiles_x;
@@ -484,9 +533,22 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 rr.release_upto(2 * q, lane);                   // rows only the other warpgroup needed
                 const bool two = 2 * q + 1 < rows_out;          // an odd last row is the pair's upper row alone
                 rr.wait_upto(2 * q + KH + (two ? 1 : 0));
-                float acc[2][2][BN / 2];                        // [64-pixel half][output row 2q, 2q+1]
-                auto issue = [&](int hf) {
-                    strip_pair_mma<KW, KC, BN>(acc[hf], rr, 2 * q, two ? KH : KH - 1, slabs, dr, dw, hf * half16, row16, slab16);
+                // [64-pixel half][output row 2q in 0 .. BN/2-1, row 2q+1 in BN/2 .. BN-1] (strip_stack_mma' fragment)
+                float acc[2][BN];
+                auto rows = [&](int hf) -> float (&)[2][BN / 2] { return *reinterpret_cast<float (*)[2][BN / 2]>(acc[hf]); };
+                auto zero = [&](int hf) {
+#pragma unroll
+                    for (int i = 0; i < BN; i++) acc[hf][i] = 0.f;
+                    wgmma_fence_regs(acc[hf]);
+                };
+                // the wgmmas of input rows 2q+rp0 .. 2q+rp1-1 for half hf
+                auto issue = [&](int hf, int rp0, int rp1) {
+                    if constexpr (STACK)
+                        strip_stack_mma<KW, KC, BN>(acc[hf], rr, 2 * q, two ? KH : KH - 1, slabs, dr, dw, hf * half16,
+                                                     row16, slab16, rp0, rp1);
+                    else
+                        strip_pair_mma<KW, KC, BN>(rows(hf), rr, 2 * q, two ? KH : KH - 1, slabs, dr, dw, hf * half16,
+                                                    row16, slab16, rp0, rp1);
                 };
                 const int y = ya + 2 * q;
                 auto epilogue = [&](int hf) {
@@ -497,10 +559,10 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         const bool inb = px < p.W;
                         const size_t pix = ((size_t)n * p.H + y) * p.W + px;
                         __half2 h0[BN / 8], h1[BN / 8];
-                        epilogue_row<BN>(acc[hf][0], i, inb, pix, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
+                        epilogue_row<BN>(rows(hf)[0], i, inb, pix, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
                                          p.out_cstride, co_off, h0);
                         if (two) {
-                            epilogue_row<BN>(acc[hf][1], i, inb, pix + p.W, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
+                            epilogue_row<BN>(rows(hf)[1], i, inb, pix + p.W, lane, p.bias + co_off, p.slope, p.out_mode, p.out,
                                              p.out_cstride, co_off, h1);
                             if (POOL) {
                                 // 2x2 average of the stored (fp16) activations; pixel m+1 is the lane 4 apart
@@ -520,24 +582,40 @@ conv_strip_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                 };
                 if constexpr (kOverlap) {
-                    issue(0);
-                    issue(1);
+                    // one chain over both halves in three commit groups: input rows 2q, 2q+1 of both halves, the rest
+                    // of half 0, the rest of half 1. Rows 2q and 2q+1 are this pair's alone (the other warpgroup's
+                    // pairs start at 2q-2 and 2q+2), so they go back to the producer as soon as the first group has
+                    // completed: with a short ring (split layers: 4 or 7 slots where two pairs in flight need KH+3)
+                    // the rows of the other warpgroup's next pair then load while this pair's chain still runs,
+                    // instead of after it. Half 0's epilogue runs under half 1's remaining wgmmas.
+                    zero(0);
+                    zero(1);
+                    wgmma_fence();
+                    issue(0, 0, 2);
+                    issue(1, 0, 2);
+                    wgmma_commit();
+                    issue(0, 2, KH + 1);
+                    wgmma_commit();
+                    issue(1, 2, KH + 1);
+                    wgmma_commit();
+                    wgmma_wait<2>();
+                    rr.release_upto(2 * q + 2, lane);
                     wgmma_wait<1>();
-                    wgmma_fence_regs(acc[0][0]);
-                    wgmma_fence_regs(acc[0][1]);
+                    wgmma_fence_regs(acc[0]);
                     epilogue(0);
                     wgmma_wait<0>();
-                    wgmma_fence_regs(acc[1][0]);
-                    wgmma_fence_regs(acc[1][1]);
+                    wgmma_fence_regs(acc[1]);
                     rr.release_upto(min(rows_in, 2 * q + 4), lane);    // next pair starts at 2q+4
                     epilogue(1);
                 } else {
 #pragma unroll
                     for (int hf = 0; hf < 2; hf++) {
-                        issue(hf);
+                        zero(hf);
+                        wgmma_fence();
+                        issue(hf, 0, KH + 1);
+                        wgmma_commit();
                         wgmma_wait<0>();
-                        wgmma_fence_regs(acc[hf][0]);
-                        wgmma_fence_regs(acc[hf][1]);
+                        wgmma_fence_regs(acc[hf]);
                         if (hf == 1) rr.release_upto(min(rows_in, 2 * q + 4), lane);
                         epilogue(hf);
                     }
@@ -993,6 +1071,7 @@ extern "C" int v2e_conv2d_lrelu_sm100(const void *x1_dev, int C1, const void *x2
 struct V2eStripLaunch {
     CUtensorMap tmA, tmA2, tmB;
     StripParams p;
+    int stacked;                  // conv_strip_kernel<.., STACK>
     int grid;
     size_t smem;
 };
@@ -1015,18 +1094,25 @@ static int make_rowseg_tmap(CUtensorMap *tm, const void *ptr, int N, int H, int 
 // Shared memory of one CTA (227 KB on sm_90, 228 KB per SM): the whole budget, or half of it for two CTAs per SM.
 constexpr size_t kSmemFull = 222 * 1024, kSmemHalf = 110 * 1024;
 
-// Strip configuration of a layer: ring slots (one input row, all slabs, each), CTAs per SM, output-channel split.
-// Returns 0 when the layer does not fit (resident weights of a slice of >= 16 output channels + KH+1 ring rows:
+// Resident weights of one CTA class: KH*KW tiles of BN x KC per slab, or KW*(KH+1)+1 with the zero tiles of the
+// stacked layout (strip_stack_mma).
+static size_t strip_w_bytes(int slabs, int KH, int KW, int bn, int kc, int stacked) {
+    return (size_t)slabs * (stacked ? KW * (KH + 1) + 1 : KH * KW) * bn * kc * 2;
+}
+
+// Strip configuration of a layer and chain: ring slots (one input row, all slabs, each), CTAs per SM, output-channel
+// split. Returns 0 when the layer does not fit (resident weights of a slice of >= 16 output channels + KH+1 ring rows:
 // the rows a pair of output rows reads). Two CTAs per SM when the weights and KH+3 rows (both warpgroups busy)
 // fit in half of the shared memory.
-static int strip_config(int C1, int C2, int Cout_pad, int KH, int KW, int kc, int *nslot, int *ctas_per_sm, int *n_split) {
+static int strip_config(int C1, int C2, int Cout_pad, int KH, int KW, int kc, int stacked, int *nslot, int *ctas_per_sm,
+                        int *n_split) {
     if (Cout_pad > 64) return 0;
     const int slabs = (C1 + C2) / kc;
     const size_t row = (((size_t)(kRowTile + KW - 1) * kc * 2 + 1023) & ~(size_t)1023) * slabs;
     for (int split = 1; split <= 2; split++) {
         const int bn = Cout_pad / split;
         if (bn < 16 || bn % 16) break;
-        const size_t wb = ((size_t)slabs * KH * KW * bn * kc * 2 + 1023) & ~(size_t)1023;
+        const size_t wb = (strip_w_bytes(slabs, KH, KW, bn, kc, stacked) + 1023) & ~(size_t)1023;
         const int two = wb + 2048 + (size_t)(KH + 3) * row <= kSmemHalf;
         const size_t budget = two ? kSmemHalf : kSmemFull;
         if (wb + 2048 + (size_t)(KH + 1) * row > budget) continue;
@@ -1048,34 +1134,67 @@ int v2e_strip_pick(int C1, int C2, int Cout_pad, int KH, int KW, int W, int *nsl
     const int g = C2 ? (C1 < C2 ? C1 : C2) : C1;
     const int kc = g % 64 == 0 ? 64 : (g % 32 == 0 ? 32 : 16);
     int ns, cps, nsp;
-    if (!strip_config(C1, C2, Cout_pad, KH, KW, kc, &ns, &cps, &nsp)) return 0;
+    if (!strip_config(C1, C2, Cout_pad, KH, KW, kc, 0, &ns, &cps, &nsp)) return 0;
     if (nslot_out) *nslot_out = ns;
     return kc;
 }
 
+// The chain V2E_STRIP_CHAIN_AUTO runs: stacked (strip_stack_mma) where a CTA class has BN <= 32 output channels and the
+// stacked weights fit with the CTAs per SM and the output-channel split of the paired chain. Per input row and k16 the
+// paired chain reads 2 x (2 KB of A + BN x 32 B of B) and the stacked one 2 KB + 2 x BN x 32 B: a third fewer operand
+// bytes at BN = 32, 40 % at BN = 16, but only a quarter at BN = 64, which does not pay for the (KH+1)/KH MACs there
+// (down1.conv1 measured 1-2.5 % slower stacked; conv2 11-14 % and conv3 9 % faster, bench_strip.py, DESIGN.md 5).
+static int strip_auto_stacked(int C1, int C2, int Cout_pad, int KH, int KW, int kc) {
+    int ns0, cps0, nsp0, ns1, cps1, nsp1;
+    if (!strip_config(C1, C2, Cout_pad, KH, KW, kc, 0, &ns0, &cps0, &nsp0) || Cout_pad / nsp0 > 32 ||
+        !strip_config(C1, C2, Cout_pad, KH, KW, kc, 1, &ns1, &cps1, &nsp1))
+        return 0;
+    return cps1 == cps0 && nsp1 == nsp0;
+}
+
+// Plan of a layer that qualifies (kc from v2e_strip_pick) under a chain request; 0 when a stacked chain was asked
+// for and its weights do not fit.
+static int strip_plan(int C1, int C2, int Cout_pad, int KH, int KW, int kc, int chain, int *nslot, int *ctas_per_sm,
+                      int *n_split, int *stacked) {
+    *stacked = chain == V2E_STRIP_CHAIN_AUTO ? strip_auto_stacked(C1, C2, Cout_pad, KH, KW, kc)
+                                             : chain == V2E_STRIP_CHAIN_STACKED;
+    return strip_config(C1, C2, Cout_pad, KH, KW, kc, *stacked, nslot, ctas_per_sm, n_split);
+}
+
+extern "C" int v2e_conv_strip_pick_chain(int C1, int C2, int Cout_pad, int KH, int KW, int W) {
+    const int kc = v2e_strip_pick(C1, C2, Cout_pad, KH, KW, W, nullptr);
+    return kc ? strip_auto_stacked(C1, C2, Cout_pad, KH, KW, kc) : -1;
+}
+
 size_t v2e_strip_launch_size(void) { return sizeof(V2eStripLaunch); }
 
-// 1 when the layer's strip configuration has a pooled epilogue (conv_strip_kernel<KW, KC, BN, true>): one CTA per SM
-// (the pooled variant keeps a row of activations in registers), even image size
+// a pooled epilogue (conv_strip_kernel<KW, KC, BN, true, .>) exists for these: one CTA per SM (the pooled variant keeps
+// a row of activations in registers), >= 32 output channels per CTA class, even image size
+static bool strip_pool_ok(int KW, int KC, int H, int W, int ctas_per_sm, int bn) {
+    return !(H & 1) && !(W & 1) && ((KW == 7 && KC == 32) || (KW == 5 && KC == 64)) && ctas_per_sm == 1 && bn >= 32;
+}
+
+// 1 when the layer's strip configuration (V2E_STRIP_CHAIN_AUTO) has a pooled epilogue
 int v2e_strip_pool_supported(int C1, int C2, int Cout_pad, int KH, int KW, int H, int W) {
-    if ((H & 1) || (W & 1) || Cout_pad < 32) return 0;
     const int KC = v2e_strip_pick(C1, C2, Cout_pad, KH, KW, W, nullptr);
-    if (!((KW == 7 && KC == 32) || (KW == 5 && KC == 64))) return 0;
-    int ns, cps, nsp;
-    if (!strip_config(C1, C2, Cout_pad, KH, KW, KC, &ns, &cps, &nsp)) return 0;
-    return cps == 1 && Cout_pad / nsp >= 32;
+    int ns, cps, nsp, st;
+    if (!KC || !strip_plan(C1, C2, Cout_pad, KH, KW, KC, V2E_STRIP_CHAIN_AUTO, &ns, &cps, &nsp, &st)) return 0;
+    return strip_pool_ok(KW, KC, H, W, cps, Cout_pad / nsp);
 }
 
 int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2, int C2, const void *wgt_row,
                       const float *bias, int Cout_pad, int KH, int KW, int N, int H, int W, void *out,
                       int out_cstride, int out_mode, int co_real, float slope, int n_sms, void *pool_out,
-                      int pool_cstride) {
+                      int pool_cstride, int chain) {
     memset(L, 0, sizeof(*L));
     StripParams &p = L->p;
+    if (chain < V2E_STRIP_CHAIN_AUTO || chain > V2E_STRIP_CHAIN_STACKED)
+        return v2e_set_error(V2E_E_INVALID, "strip: unknown chain%s", "");
     const int KC = v2e_strip_pick(C1, C2, Cout_pad, KH, KW, W, nullptr);
-    int nslot = 0, ctas_per_sm = 0, n_split = 0;
-    if (!KC || !strip_config(C1, C2, Cout_pad, KH, KW, KC, &nslot, &ctas_per_sm, &n_split))
-        return v2e_set_error(V2E_E_INVALID, "layer does not qualify for the strip kernel%s", "");
+    int nslot = 0, ctas_per_sm = 0, n_split = 0, stacked = 0;
+    if (!KC || !strip_plan(C1, C2, Cout_pad, KH, KW, KC, chain, &nslot, &ctas_per_sm, &n_split, &stacked))
+        return v2e_set_error(V2E_E_INVALID, "layer does not qualify for the strip kernel (with this chain)%s", "");
+    L->stacked = stacked;
     p.N = N; p.H = H; p.W = W; p.C1 = C1; p.C2 = C2; p.KH = KH; p.KW = KW; p.KC = KC;
     p.n_split = n_split; p.cout_pad = Cout_pad; p.BN = Cout_pad / n_split;
     p.tiles_x = (W + kRowTile - 1) / kRowTile;
@@ -1084,7 +1203,7 @@ int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2,
     const int strips = p.tiles_x * N;
     while (seg_h > 4 * KH && (long)strips * ((H + seg_h - 1) / seg_h) < 6L * n_sms) seg_h = (seg_h + 1) / 2;
     if (pool_out) {
-        if (out_mode != 0 || !v2e_strip_pool_supported(C1, C2, Cout_pad, KH, KW, H, W))
+        if (out_mode != 0 || !strip_pool_ok(KW, KC, H, W, ctas_per_sm, p.BN))
             return v2e_set_error(V2E_E_UNSUPPORTED, "strip: this layer has no pooled epilogue%s", "");
         seg_h = (seg_h + 1) & ~1;                      // 2x2 windows never straddle two items
     }
@@ -1096,7 +1215,7 @@ int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2,
     p.nslot = nslot;
     const int slabs = (C1 + C2) / KC, taps = KH * KW;
     p.slab_bytes = (int)(((size_t)(kRowTile + KW - 1) * KC * 2 + 1023) & ~(size_t)1023);
-    p.w_bytes = slabs * taps * p.BN * KC * 2;          // resident per CTA: its slice of the output channels
+    p.w_bytes = (int)strip_w_bytes(slabs, KH, KW, p.BN, KC, stacked);   // resident per CTA: its output channels
     p.out_cstride = out_cstride; p.out_mode = out_mode; p.co_real = co_real; p.slope = slope;
     p.bias = bias; p.out = out;
     int rc;
@@ -1125,13 +1244,18 @@ int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2,
     return V2E_OK;
 }
 
-template <int KW, int KC, int BN, bool POOL>
-static cudaError_t strip_launch_t(const V2eStripLaunch *L, cudaStream_t st) {
+template <int KW, int KC, int BN, bool POOL, bool STACK>
+static cudaError_t strip_launch_s(const V2eStripLaunch *L, cudaStream_t st) {
     static PerDeviceOnce attr_once;
     if (attr_once.first())
-        cudaFuncSetAttribute(conv_strip_kernel<KW, KC, BN, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    conv_strip_kernel<KW, KC, BN, POOL><<<L->grid, kStripThreads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p);
+        cudaFuncSetAttribute(conv_strip_kernel<KW, KC, BN, POOL, STACK>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    conv_strip_kernel<KW, KC, BN, POOL, STACK><<<L->grid, kStripThreads, L->smem, st>>>(L->tmA, L->tmA2, L->tmB, L->p);
     return cudaGetLastError();
+}
+
+template <int KW, int KC, int BN, bool POOL>
+static cudaError_t strip_launch_t(const V2eStripLaunch *L, cudaStream_t st) {
+    return L->stacked ? strip_launch_s<KW, KC, BN, POOL, true>(L, st) : strip_launch_s<KW, KC, BN, POOL, false>(L, st);
 }
 
 template <int KW, int KC>
@@ -1164,18 +1288,26 @@ int v2e_strip_launch(const V2eStripLaunch *L, cudaStream_t st) {
     return V2E_OK;
 }
 
-extern "C" int v2e_conv2d_lrelu_sm100_strip(const void *x1_dev, int C1, const void *x2_dev, int C2,
-                                            const void *wgt_row_dev, const float *bias_dev, int Cout_pad, int KH,
-                                            int KW, int N, int H, int W, void *out_dev, int out_cstride,
-                                            int out_mode, int co_real, float slope, void *stream) {
+extern "C" int v2e_conv2d_lrelu_sm100_strip_chain(const void *x1_dev, int C1, const void *x2_dev, int C2,
+                                                  const void *wgt_row_dev, const float *bias_dev, int Cout_pad, int KH,
+                                                  int KW, int N, int H, int W, void *out_dev, int out_cstride,
+                                                  int out_mode, int co_real, float slope, int chain, void *stream) {
     V2eStripLaunch L;
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int rc = v2e_strip_prepare(&L, x1_dev, C1, x2_dev, C2, wgt_row_dev, bias_dev, Cout_pad, KH, KW, N, H, W,
-                               out_dev, out_cstride, out_mode, co_real, slope, sms, nullptr, 0);
+                               out_dev, out_cstride, out_mode, co_real, slope, sms, nullptr, 0, chain);
     if (rc) return rc;
     return v2e_strip_launch(&L, (cudaStream_t)stream);
+}
+
+extern "C" int v2e_conv2d_lrelu_sm100_strip(const void *x1_dev, int C1, const void *x2_dev, int C2,
+                                            const void *wgt_row_dev, const float *bias_dev, int Cout_pad, int KH,
+                                            int KW, int N, int H, int W, void *out_dev, int out_cstride,
+                                            int out_mode, int co_real, float slope, void *stream) {
+    return v2e_conv2d_lrelu_sm100_strip_chain(x1_dev, C1, x2_dev, C2, wgt_row_dev, bias_dev, Cout_pad, KH, KW, N, H, W,
+                                              out_dev, out_cstride, out_mode, co_real, slope, V2E_STRIP_CHAIN_AUTO, stream);
 }
 
 

@@ -37,7 +37,7 @@ int v2e_strip_pool_supported(int C1, int C2, int Cout_pad, int KH, int KW, int H
 int v2e_strip_prepare(V2eStripLaunch *L, const void *x1, int C1, const void *x2, int C2, const void *wgt_row,
                       const float *bias, int Cout_pad, int KH, int KW, int N, int H, int W, void *out,
                       int out_cstride, int out_mode, int co_real, float slope, int n_sms, void *pool_out,
-                      int pool_cstride);
+                      int pool_cstride, int chain);
 int v2e_strip_launch(const V2eStripLaunch *L, cudaStream_t st);
 struct V2eUpLaunch;
 int v2e_conv_up2_supported(int C, int Cout_pad, int W_out);
@@ -517,7 +517,7 @@ static int conv(V2eSlomo *h, const UNet &u, int li, const __half *x1, const __ha
     if (row)
         rc = v2e_strip_prepare(R, x1, u.c1p[li], x2, x2 ? u.c2p[li] : 0, u.w_row[li], u.b[li], u.cout_pad[li], u.L[li].k,
                                u.L[li].k, B, H, W, out, u.cout_pad[li], out_mode, u.L[li].cout, kSlope, h->n_sms,
-                               pool_out, u.cout_pad[li]);
+                               pool_out, u.cout_pad[li], V2E_STRIP_CHAIN_AUTO);
     else
         rc = v2e_conv_prepare(L, x1, u.c1p[li], x2, x2 ? u.c2p[li] : 0, u.w[li], u.b[li], u.cout_pad[li], u.L[li].k,
                               u.L[li].k, B, H, W, out, u.cout_pad[li], out_mode, u.L[li].cout, kSlope,
