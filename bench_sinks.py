@@ -8,6 +8,9 @@ Prints one JSON line per measurement:
     that end in a synchronise. The files go to a temporary directory on local disk. The sinks are the reference's
     writers (oracle/_ref/, made by build()); without them the sink lines say so. The AEDAT-2.0 writer takes only the
     jAER cameras' sizes, so its rows are packed with the 346 x 260 layout (the cost per event does not depend on it).
+  * generate_events once per frame, as v2e's frame loop calls it, on host uint8 frames of the same texture at 346 x 260
+    and 1280 x 720, with no sink, with dvs_aedat2 and with dvs_text: ms per frame, host clock around --frames frames
+    that end in a synchronise, after one such pass of warm-up.
   * parallel.merge_by_key_device against the host merge_by_key on 2 and 8 row bands of one clip: the canonical stream
     of the clip above cut into bands of rows (each band's rows keep their order, as a band's own run orders them), the
     keys those of row_order='canonical' ((p < 0) << 32 | pixel). The merged rows are checked to be the stream again.
@@ -42,11 +45,11 @@ def gpu_info():
     return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
 
 
-def clip(T, seed=0):
+def clip(T, seed=0, h=H, w=W):
     rng = np.random.default_rng(seed)
-    base = rng.integers(0, 256, (H // 8 + T + 4, W // 8 + 2 * T + 4)).astype(np.uint8)
+    base = rng.integers(0, 256, (h // 8 + T + 4, w // 8 + 2 * T + 4)).astype(np.uint8)
     big = np.kron(base, np.ones((8, 8), np.uint8))
-    return np.stack([np.ascontiguousarray(big[k:k + H, 2 * k:2 * k + W]) for k in range(T)])
+    return np.stack([np.ascontiguousarray(big[k:k + h, 2 * k:2 * k + w]) for k in range(T)])
 
 
 def bench_batch(frames, ts, sink, reps, folder):
@@ -72,6 +75,29 @@ def bench_batch(frames, ts, sink, reps, folder):
     return {"bench": "generate_events_batch", "size": "%dx%d" % (W, H), "sink": sink or "none", "frames": len(ts),
             "rows_per_call": int(n), "s_per_call_median": med, "s_per_call_min": float(min(times)),
             "ms_per_frame": 1e3 * med / len(ts), "reps": reps}
+
+
+def bench_frames(h, w, sink, n, reps, folder):
+    from v2e_b200 import EventEmulator
+    kw = {} if sink is None else {sink: "pf_%s_%dx%d" % (sink, w, h), "output_folder": folder}
+    em = EventEmulator(device="cuda:0", rng_mode="device", seed=1, output_width=346, output_height=260, **kw, **CLI)
+    if sink is not None and em._sinks is None:
+        return {"bench": "generate_events", "sink": sink, "result": "not available (the writers do not import)"}
+    frames = clip(n * (reps + 1), h=h, w=w)
+    times, rows = [], 0
+    for r in range(reps + 1):                                        # pass 0 warms up: first frame, buffers, files
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for k in range(r * n, (r + 1) * n):
+            ev = em.generate_events(frames[k], k / 300.)
+            rows += len(ev) if ev is not None and r > 0 else 0
+        torch.cuda.synchronize()
+        if r > 0:
+            times.append(time.perf_counter() - t0)
+    em.cleanup()
+    return {"bench": "generate_events", "size": "%dx%d" % (w, h), "sink": sink or "none", "frames": n,
+            "rows_per_frame": rows / (n * reps), "ms_per_frame_median": 1e3 * float(np.median(times)) / n,
+            "ms_per_frame_min": 1e3 * min(times) / n, "reps": reps}
 
 
 def bands_of(rows, offs, n_shot, world):
@@ -136,6 +162,9 @@ def main():
     with tempfile.TemporaryDirectory() as d:
         for sink in (None, "dvs_aedat2", "dvs_text"):
             print(json.dumps(bench_batch(frames, ts, sink, a.reps, d)), flush=True)
+        for h, w in ((260, 346), (H, W)):
+            for sink in (None, "dvs_aedat2", "dvs_text"):
+                print(json.dumps(bench_frames(h, w, sink, a.frames, a.reps, d)), flush=True)
     from v2e_b200 import EventEmulator
     em = EventEmulator(device="cuda:0", rng_mode="device", seed=1, row_order="canonical", label_signal_noise=True,
                        **CLI)

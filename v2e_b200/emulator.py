@@ -30,8 +30,8 @@ Sink keywords (dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text; emulator.py:325-357): t
 reference's own writer classes (v2ecore.output.*, h5py) when those import, and fed the way the reference feeds
 them (emulator.py:953-975); when they do not import the keyword is ignored with a warning. The DVS text body is
 formatted on the device (v2e_b200.sinks.events_to_text) and written to the writer's file. generate_events feeds the
-sinks frame by frame; generate_events_batch once per call through write_events, which builds the text, AEDAT-2.0 and
-HDF5 bytes on the device and copies only those. label_signal_noise labels every returned row signal (1) or shot noise
+sinks frame by frame, generate_events_batch once per call, both through write_events, which builds the text, AEDAT-2.0
+and HDF5 bytes on the device and copies only those. label_signal_noise labels every returned row signal (1) or shot noise
 (0) -- `last_signnoise_label`, generate_events_batch(..., return_labels=True) -- and passes the labels to the text and
 AEDAT-2.0 sinks. A pixel-sharded emulator labels its own rows (generate_events_band(_batch)(..., return_labels=True))
 and writes no sink itself: a file needs the merged stream, which V2EPipeline.run_clip_sharded(..., write_sinks=True)
@@ -102,13 +102,12 @@ def _linlog_lut():
 
 
 class _Sinks:
-    """The reference's event writers, driven the way emulator.py:325-357 / :953-975 / :401-421 drives them."""
+    """The reference's event writers, opened and closed the way emulator.py:325-357 / :401-421 does;
+    EventEmulator.write_events feeds them."""
 
     def __init__(self, output_folder, dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text, output_width, output_height,
-                 label_signal_noise, device):
+                 label_signal_noise):
         self.h5 = self.h5_dataset = self.aedat2 = self.aedat4 = self.text = None
-        self.label_signal_noise = label_signal_noise
-        self.device = device
         folder = output_folder if output_folder is not None else "."
 
         def suffix(path, sfx):        # v2e_utils.checkAddSuffix
@@ -146,34 +145,6 @@ class _Sinks:
     def any(self):
         return any(x is not None for x in (self.h5, self.aedat2, self.aedat4, self.text))
 
-    def append(self, events, signnoise_label=None):
-        """emulator.py:953-975 (rows are a host float32 [N,4] array; signnoise_label a bool [N] array or None)."""
-        if events is None or len(events) == 0:
-            return
-        if not self.label_signal_noise:
-            signnoise_label = None
-        from . import sinks
-        ev = None
-        if self.h5 is not None or self.text is not None:
-            ev = torch.from_numpy(np.ascontiguousarray(events, dtype=np.float32)).to(self.device)
-        if self.h5 is not None:
-            # the device conversion write_events uses, so that both paths write the same rows (past 2^32 us the
-            # reference's numpy cast depends on the array's length, DESIGN.md 2)
-            tmp = sinks.events_to_h5_rows(ev).cpu().numpy().view(np.uint32)
-            self.h5_dataset.resize(self.h5_dataset.shape[0] + tmp.shape[0], axis=0)
-            self.h5_dataset[-tmp.shape[0]:] = tmp
-        if self.aedat2 is not None:
-            self.aedat2.appendEvents(events, signnoise_label=signnoise_label)
-        if self.aedat4 is not None:
-            self.aedat4.appendEvents(events, signnoise_label=None)
-        if self.text is not None:
-            # DVSTextOutput.appendEvents (ae_text_output.py:68-101) formats one line per Python call; the same lines
-            # come from the device, one copy and one write for the frame
-            if self.text.file is None:
-                raise Exception('output file closed already')
-            lab = None if signnoise_label is None else torch.from_numpy(np.asarray(signnoise_label, np.uint8))
-            self.text.numEventsWritten += sinks.write_text(self.text.file, ev, lab)
-
     def close(self):
         for w in (self.h5, self.aedat2, self.aedat4, self.text):
             if w is not None:
@@ -210,6 +181,20 @@ def _append_aedat2(w, ev, labels, dropping=None):
     w.numOffEvents += n - on
     w.file.flush()
     return k == n
+
+
+def _frame_labels(n, fi):
+    """label_signal_noise (emulator.py:889-923): the labels of a frame's n rows, whose control block is fi. Signal rows
+    (leak included) come first, labelled True; the frame's last n_shot_on + n_shot_off rows are shot noise, False."""
+    label = np.ones(n, dtype=bool)
+    label[n - (int(fi.n_shot_on) + int(fi.n_shot_off)):] = False
+    return label
+
+
+def _replay_noise(em):
+    """Replay mode with per-frame noise (leak, shot or photoreceptor): the host draws every frame's noise fields in the
+    reference's order, so the emulator `em` runs its frames one by one through the single-frame phases."""
+    return em.rng_mode == "replay" and (em.leak_rate_hz > 0 or em.shot_noise_rate_hz > 0 or em.photoreceptor_noise)
 
 
 def _finalize(lib, box, sinks, spx, ms_writers=None):
@@ -473,7 +458,7 @@ class EventEmulator(object):
         self._aedat2_dropped_all = False
         if dvs_h5 or dvs_aedat2 or dvs_aedat4 or dvs_text:
             sk = _Sinks(output_folder, dvs_h5, dvs_aedat2, dvs_aedat4, dvs_text, output_width, output_height,
-                        label_signal_noise, self.device)
+                        label_signal_noise)
             if sk.any():
                 self._sinks = sk
                 self.dvs_h5, self.dvs_aedat2, self.dvs_aedat4, self.dvs_text = sk.h5, sk.aedat2, sk.aedat4, sk.text
@@ -887,26 +872,19 @@ class EventEmulator(object):
             return None
         if fr.shape != (self._H, self._W):
             raise ValueError("frame size changed")
-        per_frame_rng = (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or self.photoreceptor_noise)
-        if self.rng_mode == "replay" and (per_frame_rng or self.exact_order):
+        if _replay_noise(self) or (self.rng_mode == "replay" and self.exact_order):
             ev = self._phase_frame(fr, code, t_frame)
         else:
             total, _, _ = self._run_step(fr.unsqueeze(0), code, [t_frame], self.frame_counter)
             ev = self._rows_to_host(total)
         self.t_previous = t_frame
-        if ev is not None and len(ev) > 0:
-            label = None
-            if self.label_signal_noise:
-                # emulator.py:889-923: signal rows (leak included) first, labelled 1; the frame's shot-noise rows are
-                # its last n_shot_on + n_shot_off rows, labelled 0
-                fi = self.last_frame_info
-                label = np.ones(len(ev), dtype=bool)
-                label[len(ev) - (int(fi.n_shot_on) + int(fi.n_shot_off)):] = False
-                self.last_signnoise_label = label
-            if self._sinks is not None:
-                self._sinks.append(ev, label)
-            return ev
-        return None
+        if ev is None or len(ev) == 0:
+            return None
+        if self.label_signal_noise:
+            self.last_signnoise_label = _frame_labels(len(ev), self.last_frame_info)
+        if self._sinks is not None:
+            self.write_events(ev, self.last_signnoise_label)
+        return ev
 
     def _pr_vrms(self, delta_time):
         """emulator.py:695-697 -> emulator_utils.py:177-295: host-side calibration of the Gaussian noise
@@ -1033,7 +1011,11 @@ class EventEmulator(object):
                 sr_dev = field(self.rng.rand)
                 _lib.check(L.v2e_emu_phase_shot(h, fp, code, t_frame, tp, p(sr_dev), cap, st))
             _lib.check(L.v2e_emu_phase_emit(h, t_frame, tp, p(self._ev_dev), cap, st))
-            fi = self._collect_one(fp, code, t_frame, tp, st)
+
+            def resume(first, base):        # a capacity abort left the frame counted: only its emission runs again
+                _lib.check(L.v2e_emu_step(h, fp, code, 1, (ctypes.c_double * 1)(t_frame), tp, None, None,
+                                          p(self._ev_dev), self._ev_dev.shape[0], base, first, 1, st))
+            fi = self._collect([t_frame], self.frame_counter, resume)[1][0]
             self.last_frame_info = fi
             n_ev = int(fi.n_events)
             ev = self._ev_dev[:n_ev].clone() if counts is None and return_device else self._rows_to_host(n_ev)
@@ -1049,26 +1031,38 @@ class EventEmulator(object):
             ev[:, 2] += ye0
         return torch.from_numpy(ev).to(self.device) if return_device and counts is not None else ev
 
-    def _collect_one(self, fp, code, t_frame, tp, st):
-        """Control block of the single frame just emitted. On V2E_E_CAPACITY (the frame is counted, its state
-        advanced, nothing emitted) the buffer grows and only the emission is re-run (v2e_emu_step resume)."""
-        L, h = self._lib, self._h
-        info = (_lib.V2eFrameInfo * 1)()
+    def _collect(self, t_frames, fc0, relaunch, keep=False):
+        """Collects the step just launched over the frames at t_frames (frame counters fc0, fc0 + 1, ...). On
+        V2E_E_CAPACITY (frames done..T-1 counted, nothing emitted from frame `done` on) the event buffer grows to at
+        least twice the rows those frames need, keeping the rows before frame `done` when `keep`, and
+        relaunch(done, row) emits again into it, from frame `done` at `row`; then the step is collected again.
+        Returns (rc, control blocks [T], done, rows) of the last collect: rc is V2E_OK, the step's probe samples and
+        model-state planes drained, or V2E_E_FALLBACK, which only a v2e_emu_fused_emit chunk returns."""
+        T = len(t_frames)
+        info = (_lib.V2eFrameInfo * T)()
         done, rows = ctypes.c_int(0), ctypes.c_uint64(0)
-        rc = L.v2e_emu_collect(h, info, 1, ctypes.byref(done), ctypes.byref(rows), st)
-        if rc == _lib.V2E_E_CAPACITY:
-            self._grow_event_buffer(int(info[0].n_events) + 1024)
+        st = self._stream()
+        while True:
+            rc = self._lib.v2e_emu_collect(self._h, info, T, ctypes.byref(done), ctypes.byref(rows), st)
+            if rc != _lib.V2E_E_CAPACITY:
+                break
+            first = done.value
+            base = int(info[first].ev_base)
+            # a multi-frame (fused) step reports the rows of every frame of the chunk; the frame-by-frame
+            # kernels only those up to the frame that did not fit
+            need = max(int(info[f].ev_base) + int(info[f].n_events) for f in range(first, T))
+            grow = 2 * max(need, self._ev_dev.shape[0])
+            if keep:
+                self._grow_event_buffer(grow, keep=base)
+            else:
+                self._grow_event_buffer(grow)
             self._bind_keys()
-            ts = (ctypes.c_double * 1)(t_frame)
-            _lib.check(L.v2e_emu_step(h, fp, code, 1, ts, tp, None, None,
-                                      ctypes.c_void_p(self._ev_dev.data_ptr()), self._ev_dev.shape[0], 0,
-                                      0, 1, st))
-            _lib.check(L.v2e_emu_collect(h, info, 1, ctypes.byref(done), ctypes.byref(rows), st))
-        else:
+            relaunch(first, base)
+        if rc != _lib.V2E_E_FALLBACK:
             _lib.check(rc)
-        self._drain_probes([t_frame])
-        self._drain_states([t_frame], self.frame_counter)
-        return info[0]
+            self._drain_probes(t_frames)
+            self._drain_states(t_frames, fc0)
+        return rc, info, done.value, int(rows.value)
 
     # pixel-sharded path (SURVEY.md 8e, BASELINE config 5): this rank owns rows [y0, y1) ---------------
     def cs_halo_rows(self, H):
@@ -1117,10 +1111,7 @@ class EventEmulator(object):
         ev = self._phase_frame(fr, code, t_frame, return_device)
         self.t_previous = t_frame
         if ev is not None and self.label_signal_noise:
-            fi = self.last_frame_info
-            label = np.ones(len(ev), dtype=bool)
-            label[len(ev) - (int(fi.n_shot_on) + int(fi.n_shot_off)):] = False
-            self.last_signnoise_label = label
+            self.last_signnoise_label = _frame_labels(len(ev), self.last_frame_info)
         return ev
 
     def _cs_iterate(self, fp, code, t_frame, tp, cap, lrp, st, W):
@@ -1182,8 +1173,7 @@ class EventEmulator(object):
             raise ValueError("return_labels=True needs label_signal_noise=True")
         if return_keys and self.row_order is None:
             raise ValueError("return_keys=True needs row_order='canonical' or 'shuffled'")
-        if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
-                                          self.photoreceptor_noise):
+        if _replay_noise(self):
             raise RuntimeError("batched sharded operation with per-frame noise needs rng_mode='device'")
         self._want_keys = bool(return_keys)
         self._ms_chunks = []
@@ -1225,27 +1215,18 @@ class EventEmulator(object):
                 # the one exchange of the chunk: frame maxima (emulator.py:773-775), MAX over the ranks
                 mx = torch.as_tensor(_DevView(L.v2e_emu_max_vec_dev(self._h), (Tc,), "<i4", self), device=self.device)
                 dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=group)
-                info = (_lib.V2eFrameInfo * Tc)()
-                done, rows = ctypes.c_int(0), ctypes.c_uint64(0)
-                while True:
+
+                def emit(*_):               # after a capacity abort: the whole chunk again, from row 0
                     _lib.check(L.v2e_emu_fused_emit(self._h, ctypes.c_void_p(self._ev_dev.data_ptr()),
                                                     self._ev_dev.shape[0], 0, st))
-                    rc = L.v2e_emu_collect(self._h, info, Tc, ctypes.byref(done), ctypes.byref(rows), st)
-                    if rc != _lib.V2E_E_CAPACITY:
-                        break
-                    need = max(int(info[k].ev_base) + int(info[k].n_events) for k in range(Tc))
-                    self._grow_event_buffer(2 * need)
-                    self._bind_keys()
+                emit()
+                rc, info, done, nrows = self._collect(t_frames[a:b], self.frame_counter + 1, emit)
                 if rc == _lib.V2E_E_FALLBACK:
-                    return int(done.value)
-                _lib.check(rc)
-                self._drain_probes(t_frames[a:b])
-                self._drain_states(t_frames[a:b], self.frame_counter + 1)
+                    return done
                 for k in range(Tc):
                     self._account(info[k])
                     offs.append(state["total"] + int(info[k].ev_base) + int(info[k].n_events))
                     n_shot.append(int(info[k].n_shot_on) + int(info[k].n_shot_off))
-                nrows = int(rows.value)
                 ev = self._ev_dev[:nrows].clone()
                 ev[:, 2] += y0
                 out.append(ev)
@@ -1351,33 +1332,19 @@ class EventEmulator(object):
         with torch.cuda.device(self.device):
             st = self._stream()
             self._grow_event_buffer(self.event_rows_hint or max(2 * n, 1 << 16))
-            info = (_lib.V2eFrameInfo * T)()
-            done, rows = ctypes.c_int(0), ctypes.c_uint64(0)
-            first, resume, base = 0, 0, int(base_row)
             if self.photoreceptor_noise:
                 tps = [float(self.t_previous)] + [float(t) for t in t_frames[:-1]]
                 vr = (ctypes.c_double * T)(*[self._pr_vrms(float(t) - tp_) for t, tp_ in zip(t_frames, tps)])
-            while True:
-                if self.photoreceptor_noise and not resume:
-                    _lib.check(L.v2e_emu_set_pr_noise(h, None, vr, T))
+                _lib.check(L.v2e_emu_set_pr_noise(h, None, vr, T))
+
+            def step(first, base, resume=1):
                 _lib.check(L.v2e_emu_step(h, ctypes.c_void_p(frames_dev.data_ptr()), code, T, ts,
                                           float(self.t_previous), None, None,
                                           ctypes.c_void_p(self._ev_dev.data_ptr()), self._ev_dev.shape[0],
                                           base, first, resume, st))
-                rc = L.v2e_emu_collect(h, info, T, ctypes.byref(done), ctypes.byref(rows), st)
-                if rc != _lib.V2E_E_CAPACITY:
-                    _lib.check(rc)
-                    break
-                # grow (keeping rows already written) and resume at the frame that did not fit
-                first, resume = done.value, 1
-                base = int(info[first].ev_base)
-                # a multi-frame (fused) step reports the rows of every frame of the chunk; the frame-by-frame
-                # kernels only those up to the frame that did not fit
-                need = max(int(info[f].ev_base) + int(info[f].n_events) for f in range(first, T))
-                self._grow_event_buffer(max(2 * need, 2 * self._ev_dev.shape[0]), keep=base)
-            self._drain_probes(t_frames)
-            self._drain_states(t_frames, fc0)
-            total = int(rows.value)
+            step(0, int(base_row), 0)
+            # on a capacity abort the rows already written are kept and the step resumes at the frame that did not fit
+            _, info, _, total = self._collect(t_frames, fc0, step, keep=True)
             offsets = np.array([int(info[f].ev_base) for f in range(T)] + [total], np.int64)
             n_shot = np.array([int(info[f].n_shot_on) + int(info[f].n_shot_off) for f in range(T)], np.int64)
             for f in range(T):
@@ -1388,8 +1355,7 @@ class EventEmulator(object):
     def check_batch_path(self):
         """Raises RuntimeError where generate_events_batch cannot run this emulator: replay mode with per-frame noise,
         or a sharded emulator."""
-        if self.rng_mode == "replay" and (self.leak_rate_hz > 0 or self.shot_noise_rate_hz > 0 or
-                                          self.photoreceptor_noise):
+        if _replay_noise(self):
             raise RuntimeError("generate_events_batch with per-frame noise needs rng_mode='device' "
                                "(replay mode must interleave host draws frame by frame)")
         if self.shard is not None:
@@ -1482,6 +1448,7 @@ class EventEmulator(object):
         lab = sinks._labels(labels, ev) if self.label_signal_noise and labels is not None else None
         with torch.cuda.device(self.device):
             if sk.h5 is not None:
+                # on the device: past 2^32 us the reference's numpy cast depends on the array's length (DESIGN.md 2)
                 tmp = sinks.events_to_h5_rows(ev).cpu().numpy().view(np.uint32)
                 sk.h5_dataset.resize(sk.h5_dataset.shape[0] + n, axis=0)
                 sk.h5_dataset[-n:] = tmp

@@ -13,7 +13,7 @@ import logging
 import numpy as np
 import torch
 
-from .emulator import EventEmulator
+from .emulator import EventEmulator, _replay_noise
 from .slomo import SuperSloMo, batch_times, clip_span
 
 logger = logging.getLogger(__name__)
@@ -539,7 +539,7 @@ class V2EPipeline:
         cont = seg[0]
         em = self.emulator
         extra = dict(return_labels=True) if return_labels else {}
-        if em.rng_mode == "device" or not (em.leak_rate_hz > 0 or em.shot_noise_rate_hz > 0 or em.photoreceptor_noise):
+        if not _replay_noise(em):
             # chunks of frames through the multi-frame kernels: one all-reduce(MAX) of the frame maxima per chunk
             # (frame by frame -- one all-reduce each -- for a chunk the refractory filter touches, for the
             # centre-surround model, whose Euler iteration exchanges halo rows, and for SCIDVS / photoreceptor noise)
